@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W             (N > 1 is launched by torchrun, one rank per GPU)
     python bench.py --impl reference --gpus N --steps K --warmup W   (the reference's torch-CPU path, rank 0 only)
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR  (also writes the last timed step's results as .npy)
 
 A "step" is one pass of the hot path over one resident synthetic rollout: ``train_epochs(n_epochs=4)`` =
 4 x shuffle + 16 x (memory.sample(8192) + learner.update), exactly the loop of
@@ -35,25 +36,26 @@ WORKLOAD = ("PPO-Clip train_epochs(4) = 16 x (sample 8192 + update) over a resid
 
 # ------------------------------------------------------------------------------------------------ helpers
 def measured_peaks():
-    """(HBM GB/s, sustained dense bf16 TFLOP/s, source)."""
+    """(HBM GB/s, dense bf16 TFLOP/s, source)."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         try:
             d = json.load(open(p))
-            return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", 1400.0)), "measured (MEASURED_PEAKS.json)"
+            return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", 989.0)), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, 1400.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, 989.0, "H100 SXM data sheet (700 W card; a lower power limit lowers the clocks)"
 
 
-def ncu_traffic(kernel_key):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture of that kernel at the
-    bench shape (profiles/r02_traffic.json, written by tools/ncu_traffic.py from the .ncu-rep); None when not captured."""
-    p = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    try:
-        return json.load(open(p)).get(kernel_key, {}).get("dram_bytes_per_launch")
-    except Exception:
-        return None
+def dump_outputs(out_dir, info, model):
+    """What the timed path computed in its last step: the info dict train_epochs returned (one float64 array per key) and
+    every parameter of the model it updated (float32, ~13 MB), as DIR/<name>.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in info.items():
+        if not isinstance(v, dict):
+            np.save(os.path.join(out_dir, "info_%s.npy" % k), np.asarray(float(v), dtype=np.float64))
+    for k, v in model.state_dict().items():
+        np.save(os.path.join(out_dir, "param_%s.npy" % k), v.detach().float().cpu().numpy())
 
 
 class ClockSampler:
@@ -199,8 +201,8 @@ def run_reference_arm(args):
     line = {"impl": "reference", "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": args.gpus,
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True,
             "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
-            "config": {"workload": WORKLOAD, "arm": "reference torch-CPU path (oracle port: the reference is Python "
-                       "and /root/reference does not travel to the GPU box)", "cpu_threads": info["cores"]},
+            "config": {"workload": WORKLOAD, "arm": "reference torch-CPU path (oracle port of the reference's Python "
+                       "code)", "cpu_threads": info["cores"]},
             "cpu_baseline": {"value": value, "unit": UNIT, "cores": info["cores"], "kind": "port",
                              "sample": info["sample"]},
             "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
@@ -354,6 +356,8 @@ def run_own_arm(args):
     barrier()
     elapsed_ms = e0.elapsed_time(e1)
     _log("timed region done: %.1f ms/step" % (elapsed_ms / args.steps))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, info, agent.model)
     launches = _lib.launch_count - launches0
     clocks = sampler.stop() if sampler else None
     t = torch.tensor([elapsed_ms], dtype=torch.float64, device=device)
@@ -453,16 +457,14 @@ def run_own_arm(args):
         n_upd = max(1, N_MINIBATCH)
         top = max(per_layer.items(), key=lambda kv: kv[1][0])
         ach = tot_fl / (tot_ms * 1e-3) / 1e12
-        roofline = {"kernel": "conv_tc_kernel (K12: tcgen05 gathered-operand GEMM; %d launches per update: forward, data and "
+        roofline = {"kernel": "conv_tc_kernel (K12: wgmma gathered-operand GEMM; %d launches per update: forward, data and "
                               "weight gradients of conv1-3 + the 6400->512 layer)" % (len(flog) // n_upd),
                     "bound": "tensor", "achieved": ach, "peak": tc_peak, "unit": "TFLOP/s", "frac": ach / tc_peak,
-                    "traffic": ncu_traffic("conv_tc_kernel:update_B%d_P%d" % (N_ENVS * T // N_MINIBATCH // world, args.tc_planes)),
-                    "peak_source": peak_src + ", bf16_tflops_sustained",
+                    "peak_source": peak_src + ", dense bf16",
                     "algorithmic_flops_per_update": tot_fl / n_upd,
                     "what": "algorithmic bf16 tensor FLOPs = 2 x real output sites x N x K (padding / halo / garbage sites of the padded "
                             "layouts NOT counted) x the plane products float32-grade arithmetic keeps (6 for 3x3 planes, 3 for "
-                            "the raw-pixel first layer) / summed CUDA-event time of the K12 launches; traffic = DRAM bytes of "
-                            "those launches per update (ncu --set full of one update at this shape, profiles/r02_traffic.json)",
+                            "the raw-pixel first layer) / summed CUDA-event time of the K12 launches",
                     "fp32_equivalent_tflops": tot_eq / (tot_ms * 1e-3) / 1e12,
                     "avg_update_ms": tot_ms / n_upd, "launches_timed": len(flog),
                     "timed": "CUDA events around every K12 launch of one eager epoch run right after the timed region",
@@ -479,7 +481,6 @@ def run_own_arm(args):
         ach = alg_bytes / (k3_ms * 1e-3) / 1e9
         roofline = {"kernel": "gather_obs_kernel (K3: minibatch gather + u8->float)", "bound": "hbm",
                     "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak,
-                    "traffic": ncu_traffic("gather_obs_kernel:%s:%d" % (args.compute, B_local)),
                     "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_bytes,
                     "avg_launch_ms": k3_ms, "launches_timed": len(prof["xb_gather_obs"]),
                     "timed": "CUDA events around every K3 launch of one eager epoch run right after the timed region",
@@ -504,10 +505,10 @@ def run_own_arm(args):
                                       if world > 1 else "dp1 (single GPU, no collective)",
                        "compute": {"fp32": "fp32, TF32 disabled (reference arithmetic)", "fp32_cl": "fp32, TF32 disabled, channels-last convolutions", "tf32": "fp32 storage, TF32 convs/matmuls",
                                    "bf16": "bf16 autocast convs, fp32 master weights",
-                                   "tc": "tcgen05 layers (K12): every fp32 operand as %d bf16 planes (exact to 2^-%d), raw uint8 pixels as "
-                                         "one exact plane, fp32 accumulation in TMEM per product order; heads / loss / Adam fp32"
+                                   "tc": "wgmma layers (K12): every fp32 operand as %d bf16 planes (exact to 2^-%d), raw uint8 pixels as "
+                                         "one exact plane, fp32 accumulation per product order; heads / loss / Adam fp32"
                                          % (args.tc_planes, 8 * args.tc_planes)}[args.compute],
-                       "l2": "inputs (925 MB uint8 rollout / G) exceed the 126 MB L2; no explicit flush",
+                       "l2": "inputs (925 MB uint8 rollout / G) exceed the 50 MB L2; no explicit flush",
                        "cuda_graph": bool(cfg.use_cuda_graph)},
             "clocks": clocks, "e2e": e2e, "gpu_launches": launches, "roofline": roofline, "cpu_baseline": cpu,
             "phases": phases, "parity_vs_1gpu": parity,
@@ -523,13 +524,15 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="xuance_b200", choices=["xuance_b200", "reference"])
     ap.add_argument("--compute", default="tc", choices=["fp32", "fp32_cl", "tf32", "bf16", "tc"],
-                    help="'tc' (default) = the K12 tcgen05 layers, float32-grade split-bf16 arithmetic; 'fp32' = cuDNN / cuBLAS "
+                    help="'tc' (default) = the K12 wgmma layers, float32-grade split-bf16 arithmetic; 'fp32' = cuDNN / cuBLAS "
                          "CUDA-core fp32 (round 1's headline); 'tf32' / 'bf16' = reduced-precision library paths, for context")
     ap.add_argument("--tc-planes", type=int, default=3, choices=[2, 3],
                     help="with --compute tc: bf16 planes per operand (3 = float32-grade, 2 = ~1e-5 forward error)")
     ap.add_argument("--e2e-steps", type=int, default=3)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--graph", type=int, default=-1, help="CUDA-graph the minibatch update: 1/0; default: on (every N)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's info dict and the updated parameters as DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl != "reference":
         args.warmup = 3

@@ -1,5 +1,5 @@
 /*
- * xb200.h - C-ABI of the B200-native rollout->update hot path for agi-brain/xuance (v1.4.4 @ 4f0b05b).
+ * xb200.h - C-ABI of the H100-native rollout->update hot path for agi-brain/xuance (v1.4.4 @ 4f0b05b).
  *
  * The reference has NO native/FFI layer (SURVEY.md section 8b): its hot path is Python classes resolved
  * through registries.  This header is therefore the boundary a maintainer would bind from those classes
@@ -161,7 +161,7 @@ int xb_qmix_td(const float *q_tot, const float *q_tot_next, const float *rewards
                const float *filled, const float *filled_sum, int B, int n, int T, float gamma, float grad_scale,
                float *dq_tot, float *stats, double *scratch, void *stream);
 
-/* Tensor-core forward of the whole mixer (hypernet GEMMs + epilogue in ONE kernel; tcgen05.mma with TMEM
+/* Tensor-core forward of the whole mixer (hypernet GEMMs + epilogue in ONE kernel; wgmma with register
  * accumulators, bf16 hi/lo split operands, 3 MMAs per product, fp32 accumulate): q_tot[R] from states[R,S], q[R,n]
  * and the raw Linear parameters of QMIX_Mixer (q_mix_head.py:52-64): w_l1[4] / b_l1[4] are HOST arrays of 4 device
  * pointers to the first-layer weights [32,S] / biases [32] of hyper_w_1, hyper_b_1, hyper_w_2, hyper_b_2 (in that
@@ -229,12 +229,12 @@ int xb_categorical_act(const float *logits, const float *uniforms, const float *
 int xb_rms_update_normalize(const float *x, int N, int64_t D, float *mean, float *var, double count, int update,
                             float *out, float clip_range, float eps, void *stream);
 
-/* ---------------------------------------------------------------- K12: tensor-core layers (tcgen05 / TMEM) ------
+/* ---------------------------------------------------------------- K12: tensor-core layers (wgmma / TMA) ----------
  * The pixel encoders' convolutions and hidden layer (NatureCNN of AC_CNN_Atari / Basic_CNN: rl_models/representations/cnn.py:
  * 45-50, 84-101; layers.py:16-65), forward, data gradient and weight gradient, that cuDNN runs as CUDA-core fp32 kernels
  * (85 % of the fp32 PPO update).  Every float32 operand travels as 1-3 bfloat16 "planes" (x = sum of its planes; plane q =
  * bf16 of the residual left by the planes before it: 1 plane is exact for integers <= 256 such as raw uint8 pixels, 2
- * planes are exact to 2^-16, 3 planes to 2^-24); products are accumulated in float32 in TMEM, one accumulator per order of
+ * planes are exact to 2^-16, 3 planes to 2^-24); products are accumulated in float32 registers, one accumulator per order of
  * magnitude (plane-index sum), added smallest first in the epilogue.  planes_a <= planes_b; kept products: index sum <
  * planes_b.
  * xb_split_bf16       : x (float32[n]) -> planes[0] = bf16(x), planes[1] = bf16(x - planes[0]), [planes[2] = ...]

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE (see oracle/__init__.py).  Restatement of the reference's agent-side loops that drive the hot path,
-used to prove the drop-in claim in two steps: tests/test_dropin_reference.py runs THIS function and the live
-``xuance.torch.agents.core.on_policy.OnPolicyAgent.train_epochs`` against recording fakes and requires identical call
-sequences (build container, where /root/reference exists); tests/test_gpu_dropin.py runs this function over the real
+used to prove the drop-in claim in two steps: tests/test_dropin_reference.py runs THIS function against recording fakes
+and requires the call sequence the reference's ``xuance.torch.agents.core.on_policy.OnPolicyAgent.train_epochs`` produced
+(recorded by tests/golden/make_reference_live.py); tests/test_gpu_dropin.py runs this function over the real
 xuance_b200 buffer + learner on the GPU and requires the result of the product agent's own ``train_epochs``."""
 import numpy as np
 

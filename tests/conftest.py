@@ -9,8 +9,8 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
-    config.addinivalue_line("markers", "reference: needs the live reference at /root/reference (build container)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
+    config.addinivalue_line("markers", "reference: needs a checkout of the reference package (XB_REFERENCE_ROOT)")
 
 
 def pytest_collection_modifyitems(config, items):

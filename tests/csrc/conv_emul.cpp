@@ -36,12 +36,12 @@ extern "C" int emul_gemm_gather(int PA, int PB, const float *in, int64_t in_plan
     const int n_tiles = N_total / N;
     const float nan = std::numeric_limits<float>::quiet_NaN();
     uint32_t it = 0;
-    std::vector<double> acc((size_t)TM * PB * N);       // PB accumulator groups of N columns (TMEM columns g*N + n)
+    std::vector<double> acc((size_t)TM * PB * N);       // PB accumulator groups of N columns (accumulator columns g*N + n)
     for (int64_t work = 0; work < m_tiles * n_tiles; ++work) {
         const int64_t tile = work / n_tiles;
         const int nt = (int)(work % n_tiles);
         const int64_t w_off = (int64_t)nt * N * K;
-        std::fill(acc.begin(), acc.end(), nan);         // TMEM is not cleared: the first MMA must initialise every group
+        std::fill(acc.begin(), acc.end(), nan);         // accumulators start undefined: the first MMA must initialise every group
         for (int kc = 0; kc < n_chunks; ++kc, ++it) {
             const uint32_t base = (it % stages) * stage_bytes;
             for (uint32_t i = 0; i < stage_bytes / 2; ++i) smem[base / 2 + i] = nan;     // poison the stage

@@ -94,3 +94,39 @@ def same_structure(a, b, path=""):
         assert np.array_equal(np.asarray(a), np.asarray(b)), path
     else:
         assert a == b, (path, a, b)
+
+
+def seeded_state_dict(sd, seed):
+    """A state dict with the keys / shapes / dtypes of ``sd`` and values that depend only on (seed, key): uniform in
+    +-1/sqrt(fan_in).  Loaded into a reference model and into its oracle restatement (same keys), it gives both the same
+    initial weights without storing them."""
+    import zlib
+    out = {}
+    for k, v in sd.items():
+        if not torch.is_floating_point(v):
+            out[k] = v.clone()
+            continue
+        fan_in = int(np.prod(v.shape[1:])) if v.dim() > 1 else 100
+        rng = np.random.default_rng([seed, zlib.crc32(k.encode())])
+        out[k] = torch.from_numpy(rng.uniform(-1.0, 1.0, size=tuple(v.shape)).astype(np.float32) / np.sqrt(fan_in)).to(v.dtype)
+    return out
+
+
+def param_sample(sd, n=64):
+    """A fixed sample of every floating tensor of a state dict (up to ``n`` elements at key-seeded positions), float64."""
+    import zlib
+    out = {}
+    for k, v in sd.items():
+        if not torch.is_floating_point(v):
+            continue
+        flat = v.detach().reshape(-1).double().cpu().numpy()
+        idx = np.random.default_rng(zlib.crc32(k.encode())).choice(flat.size, size=min(n, flat.size), replace=False)
+        out[k] = flat[np.sort(idx)]
+    return out
+
+
+def digest(a):
+    """sha256 of an array's values as float64 (equal digests <=> np.array_equal for the arrays the buffers hold)."""
+    import hashlib
+    a = np.asarray(a, dtype=np.float64)
+    return hashlib.sha256(repr(a.shape).encode() + a.tobytes()).hexdigest()

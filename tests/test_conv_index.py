@@ -2,7 +2,7 @@
 
 The kernel cannot run here, so its data movement is emulated on the host WITH THE KERNEL'S OWN index functions
 (xuance_b200/csrc/conv_index.h is compiled into tests/csrc/conv_emul.cpp by g++): units are staged into an emulated
-shared-memory image, read back the way the tcgen05 descriptors address it, and the result is compared with torch's fp64
+shared-memory image, read back the way the wgmma descriptors address it, and the result is compared with torch's fp64
 convolution / autograd on the un-split operands - which also checks the split-bf16 numerics claim (three products of
 hi/lo bf16 pairs reproduce the fp32 result to ~1e-5)."""
 import ctypes

@@ -1,79 +1,17 @@
-"""CPU, build container only (needs /root/reference): the drop-in claim of INTEGRATION.md section A, executed.
-
-1. The registry / seam patch printed in INTEGRATION.md is extracted from the markdown and exec'd against the imported,
-   unmodified reference; afterwards the reference's own lookups resolve to the xuance_b200 classes.
-2. The reference's ``OnPolicyAgent._build_memory`` (on_policy.py:65-104) is run, unmodified, on a minimal agent object: it
-   reaches the xuance_b200 buffer constructor with exactly the keyword arguments that constructor accepts (on this CPU-only
-   box the constructor then stops at the CUDA allocation - there is no CPU fallback to fall into).
-3. The reference's own ``OnPolicyAgent.train_epochs`` (on_policy.py:182-205) and its restatement in oracle/agents.py drive
-   recording fakes with the same NumPy seed and must produce identical call sequences.  tests/test_gpu_dropin.py then runs
-   that restatement over the real xuance_b200 buffer + learner on the GPU."""
-import inspect
+"""CPU: the drop-in restatement of the reference's agent loop.  The reference's own ``OnPolicyAgent.train_epochs``
+(on_policy.py:182-205) and its restatement in oracle/agents.py drive recording fakes with the same NumPy seed and must
+produce identical call sequences (the reference's sequence is recorded in tests/golden/reference_live.pkl.gz by
+tests/golden/make_reference_live.py).  tests/test_gpu_dropin.py then runs that restatement over the real xuance_b200
+buffer + learner on the GPU."""
+import gzip
 import os
-import re
-from argparse import Namespace
+import pickle
 from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
-pytestmark = pytest.mark.reference
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def patched():
-    from oracle.ref_loader import import_reference
-    import_reference()
-    md = open(os.path.join(ROOT, "INTEGRATION.md")).read()
-    section = md[md.index("Registering inside an existing XuanCe checkout"):]
-    code = re.search(r"```python\n(.*?)```", section, re.S).group(1)
-    ns = {}
-    exec(compile(code, "INTEGRATION.md#A", "exec"), ns)
-    return ns
-
-
-def test_registry_patch_from_the_document_resolves_to_xb200(patched):
-    import xuance.torch.agents.core.on_policy as core
-    from xuance.torch.learners import REGISTRY_Learners
-    import xuance_b200.common as xc
-    from xuance_b200.torch.learners import PPO_Learner
-    assert REGISTRY_Learners["PPO_Learner"] is PPO_Learner
-    assert core.DummyOnPolicyBuffer is xc.DummyOnPolicyBuffer and core.DummyOnPolicyBuffer_Atari is xc.DummyOnPolicyBuffer_Atari
-    # the reference resolves its learner through the registry at build time (agents/base/agent.py: _build_learner)
-    from xuance.torch.agents.base.agent import Agent
-    src = inspect.getsource(Agent._build_learner)
-    assert "REGISTRY_Learners[self.config.learner]" in src
-
-
-@pytest.mark.parametrize("atari", [False, True])
-def test_reference_build_memory_reaches_the_xb200_buffer(patched, atari, monkeypatch):
-    import xuance.torch.agents.core.on_policy as core
-    import xuance_b200.common as xc
-    from xuance_b200.common import Box, Discrete
-    cls = xc.DummyOnPolicyBuffer_Atari if atari else xc.DummyOnPolicyBuffer
-    seen = {}
-    real_init = cls.__init__
-
-    def spy(self, *a, **kw):
-        seen.update(kw)
-        inspect.signature(real_init).bind(self, *a, **kw)          # the reference's kwargs fit the constructor
-        return real_init(self, *a, **kw)
-    monkeypatch.setattr(cls, "__init__", spy)
-    obs_space = Box(0, 255, (84, 84, 4), np.uint8) if atari else Box(-1, 1, (4,), np.float32)
-    agent = SimpleNamespace(observation_space=obs_space, action_space=Discrete(4), n_envs=4, horizon_size=8, n_minibatch=2,
-                            gamma=0.99, gae_lam=0.95, is_tensor_memory=False,
-                            config=Namespace(use_gae=True, use_advnorm=True, env_name="Atari" if atari else "Classic"))
-    import torch
-    if torch.cuda.is_available():
-        buf = core.OnPolicyAgent._build_memory(agent, {"old_logp": ()})
-        assert isinstance(buf, cls) and buf.observations.is_cuda
-    else:
-        with pytest.raises((RuntimeError, AssertionError)):       # CUDA allocation: no CPU fallback behind the seam
-            core.OnPolicyAgent._build_memory(agent, {"old_logp": ()})
-    assert set(seen) == {"observation_space", "action_space", "auxiliary_shape", "n_envs", "horizon_size", "use_gae",
-                         "use_advnorm", "gamma", "gae_lam"}
-    assert agent.buffer_size == 32 and agent.batch_size == 16
 
 
 class _Recorder:
@@ -91,17 +29,15 @@ class _Recorder:
 
 
 @pytest.mark.parametrize("buffer_size,batch_size,n_epochs", [(64, 16, 4), (60, 16, 3)])
-def test_train_epochs_restatement_equals_the_live_reference(patched, buffer_size, batch_size, n_epochs):
-    import xuance.torch.agents.core.on_policy as core
+def test_train_epochs_restatement_equals_the_live_reference(buffer_size, batch_size, n_epochs):
     from oracle.agents import reference_train_epochs
-    runs = []
-    for fn in (core.OnPolicyAgent.train_epochs, reference_train_epochs):
-        rec = _Recorder()
-        agent = SimpleNamespace(buffer_size=buffer_size, batch_size=batch_size, memory=rec, learner=rec)
-        np.random.seed(11)
-        info = fn(agent, n_epochs)
-        runs.append((rec.calls, info))
-    (a, ia), (b, ib) = runs
+    with gzip.open(os.path.join(ROOT, "tests", "golden", "reference_live.pkl.gz"), "rb") as fh:
+        want = pickle.load(fh)["train_epochs"][(buffer_size, batch_size, n_epochs)]
+    rec = _Recorder()
+    agent = SimpleNamespace(buffer_size=buffer_size, batch_size=batch_size, memory=rec, learner=rec)
+    np.random.seed(11)
+    info = reference_train_epochs(agent, n_epochs)
+    a, ia, b, ib = want["calls"], want["info"], rec.calls, info
     assert ia == ib and len(a) == len(b) and len(a) == 2 * n_epochs * -(-buffer_size // batch_size)
     for (ka, va), (kb, vb) in zip(a, b):
         assert ka == kb and (np.array_equal(va, vb) if ka == "sample" else va == vb)

@@ -129,7 +129,7 @@ def test_qmix_learner_matches_oracle(detach, double_q, graph):
 
 @pytest.mark.parametrize("R,n,S,fusable", [(1920, 5, 98, True), (128, 5, 98, True), (1000, 8, 112, True), (77, 3, 17, False), (245760, 5, 98, True), (300, 2, 160, False), (999, 5, 98, True), (129, 4, 104, True)])
 def test_tensor_core_mixer_forward(R, n, S, fusable):
-    """K9-TC (tcgen05.mma, TMEM accumulators, bf16 hi/lo split x 4 products) vs the fp32 torch-CPU mixer."""
+    """K9-TC (wgmma, register accumulators, bf16 hi/lo split x 4 products) vs the fp32 torch-CPU mixer."""
     from xuance_b200.torch.rl_models import QMIX_Mixer
     torch.manual_seed(R + n)
     om = MixerOracle(S, 32, 32, n)

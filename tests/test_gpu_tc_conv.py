@@ -3,8 +3,8 @@ preparation, forward (2 / 3 planes, raw uint8 single plane), data gradient with 
 (MN-major operands, site splits, column tiles), the Linear layer in all three modes, the whole encoder forward + backward
 next to cuDNN fp32, and a PPO update with compute="tc" next to the fp32 learner.
 
-Tolerances.  Operands with 3 planes are exact to 2^-24; what remains is the float32 accumulation in TMEM, which TRUNCATES
-on every addition of a 16-deep product block (measured on B200: results are biased toward zero by ~0.5 ulp per K step of
+Tolerances.  Operands with 3 planes are exact to 2^-24; what remains is the float32 accumulation of the tensor core, which
+truncates on every addition of a 16-deep product block (results are biased toward zero by up to ~0.5 ulp per K step of
 the hi.hi accumulator).  For O(1) outputs of K <= 576 layers that is <= 3e-6; the 6400-deep Linear and the long site
 reductions of the weight gradients carry proportionally more and are bounded by cutting the reduction (wgrad_splits)."""
 import os
@@ -58,7 +58,7 @@ def _forward_conv(B, H, W, C, N, k, s, planes, atol):
 
 
 LAYERS = [(2, 84, 84, 4, 32, 8, 4), (3, 21, 21, 32, 64, 4, 2), (5, 10, 10, 64, 64, 3, 1), (256, 21, 21, 32, 64, 4, 2)]
-if os.environ.get("XB_SANITIZE") == "1":       # tools/sanitize.sh: compute-sanitizer slows kernels 10-100x
+if os.environ.get("XB_SANITIZE") == "1":       # under compute-sanitizer, which slows kernels 10-100x
     LAYERS = LAYERS[:3]
 
 

@@ -1,226 +1,162 @@
-"""CPU, build container only (needs /root/reference): the oracle next to the LIVE, unmodified reference on fresh
-seeded inputs - the second way the oracle is pinned (the first is tests/golden).  Skipped where the reference is absent."""
+"""CPU: the oracle next to the unmodified reference on fresh seeded inputs - the second way the oracle is pinned (the first
+is tests/golden/*.npz).  The reference's side was recorded by tests/golden/make_reference_live.py into
+tests/golden/reference_live.pkl.gz; models start from helpers.seeded_state_dict on both sides, final parameters are
+compared on helpers.param_sample."""
+import gzip
+import os
+import pickle
 import random
-from argparse import Namespace
 
 import numpy as np
 import pytest
 import torch
-import torch.nn as nn
 
-from helpers import synth_rollout, fill_buffers, qmix_episode_stream, same_structure as _same
+from helpers import synth_rollout, fill_buffers, qmix_episode_stream, same_structure as _same, seeded_state_dict, \
+    param_sample, digest
 
-pytestmark = pytest.mark.reference
+FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_live.pkl.gz")
 
 
 @pytest.fixture(scope="module")
 def ref():
-    from oracle.ref_loader import import_reference
-    return import_reference()
+    with gzip.open(FIXTURE, "rb") as fh:
+        return pickle.load(fh)
+
+
+def _close_params(sd, want, rtol=1e-5, atol=1e-6):
+    got = param_sample(sd)
+    assert set(got) == set(want)
+    for k in want:
+        np.testing.assert_allclose(got[k], want[k], rtol=rtol, atol=atol, err_msg=k)
 
 
 @pytest.mark.parametrize("seed,use_gae", [(0, True), (1, True), (2, False)])
 def test_onpolicy_buffer_live(ref, seed, use_gae):
-    from gymnasium.spaces import Box, Discrete
-    from xuance.common.memory_tools import DummyOnPolicyBuffer
     from oracle.onpolicy import OnPolicyBufferOracle
+    r = ref["onpolicy"][seed]
     rng = np.random.default_rng(seed)
     N, T = 5, 33
     ro = synth_rollout(rng, N, T, (3,), obs_dtype=np.float32, p_term=0.1)
-    r = DummyOnPolicyBuffer(Box(-1, 1, (3,)), Discrete(4), {'old_logp': ()}, N, T, use_gae=use_gae)
     o = OnPolicyBufferOracle((3,), (), {'old_logp': ()}, N, T, use_gae=use_gae)
-    fill_buffers([r, o], ro, [(4, 1, np.float32(0.2)), (9, 3, 0.0), (20, 1, np.float32(-0.7))])
-    assert np.array_equal(r.returns, o.returns) and np.array_equal(r.advantages, o.advantages)
+    fill_buffers([o], ro, [(4, 1, np.float32(0.2)), (9, 3, 0.0), (20, 1, np.float32(-0.7))])
+    assert np.array_equal(r["returns"], o.returns) and np.array_equal(r["advantages"], o.advantages)
     idx = rng.permutation(N * T)[:50]
-    s1, s2 = r.sample(idx), o.sample(idx)
+    s2 = o.sample(idx)
     for k in ('obs', 'actions', 'returns', 'values', 'advantages'):
-        assert np.array_equal(s1[k], s2[k]) and s1[k].dtype == s2[k].dtype, k
+        assert np.array_equal(r["sample"][k], s2[k]) and r["sample"][k].dtype == s2[k].dtype, k
 
 
 @pytest.mark.parametrize("alpha", [0.5, 0.6])
 def test_per_buffer_live(ref, alpha):
-    from gymnasium.spaces import Box, Discrete
-    from xuance.common.memory_tools import PerOffPolicyBuffer
     from oracle.replay import PerReplayOracle
+    events = iter(ref["per"][alpha])
     rng = np.random.default_rng(int(alpha * 10))
     N, S, B = 4, 64, 32
-    r = PerOffPolicyBuffer(Box(-1, 1, (3,)), Discrete(4), None, N, N * S, B, alpha=alpha)
-    r._max_priority = np.ones(N, np.float32)       # canonical float32 rule (oracle/replay.py docstring)
     o = PerReplayOracle((3,), (), N, N * S, B, alpha=alpha)
     for t in range(100):
         st = (rng.normal(size=(N, 3)).astype(np.float32), rng.integers(0, 4, N), rng.normal(size=N).astype(np.float32),
               rng.random(N) < 0.1, rng.normal(size=(N, 3)).astype(np.float32))
-        r.store(*st), o.store(*st)
+        o.store(*st)
         if t > 10 and t % 3 == 0:
-            random.seed(t)
-            s1 = r.sample(0.4)
+            r = next(events)
+            assert r["t"] == t
             random.seed(t)
             s2 = o.sample(0.4)
-            assert np.array_equal(s1['step_choices'], s2['step_choices']) and np.array_equal(s1['weights'], s2['weights'])
+            assert np.array_equal(r['step_choices'], s2['step_choices']) and np.array_equal(r['weights'], s2['weights'])
             td = np.abs(rng.normal(size=B)).astype(np.float32)
             td[3] = 0
-            r.update_priorities(s1['step_choices'], td), o.update_priorities(s2['step_choices'], td)
+            o.update_priorities(s2['step_choices'], td)
             for i in range(N):
-                assert np.array_equal(np.array(r._it_sum[i]._value, dtype=np.float64), o.sum[i].v.astype(np.float64))
-                assert np.array_equal(np.array(r._it_min[i]._value, dtype=np.float64), o.min[i].v.astype(np.float64))
-            assert np.array_equal(r._max_priority, o.max_priority)
+                assert r["sum"][i] == digest(o.sum[i].v.astype(np.float64))
+                assert r["min"][i] == digest(o.min[i].v.astype(np.float64))
+            assert np.array_equal(r["max_priority"], o.max_priority)
 
 
-def _qmix_pair(n, obs_dim, A, S, T, lr_decay=0.5):
-    from gymnasium.spaces import Discrete
-    from xuance.common import BaseCallback, AgentGrouping
-    from xuance.torch.rl_models.representations.rnn import Basic_RNN
-    from xuance.torch.rl_models.representations.agent_feature import AgentFeatureEncoder
-    from xuance.torch.rl_models.modules.identity_encoder import build_identity_encoder, IdentityFeatureFusion
-    from xuance.torch.rl_models.critics.base_critics import DiscreteActionValueCritic
-    from xuance.torch.rl_models.heads.q_mix_head import QMIX_Mixer
-    from xuance.torch.rl_models.architectures.multi_agent.value_factorization import MixingQNetwork
-    from xuance.torch.learners.multi_agent_rl.qmix_learner import QMIX_Learner
+def _qmix_oracle(n, obs_dim, A, S, total_iters, lr_decay=0.5, seed=0):
     from oracle.qmix import QMIXModelOracle, QMIXLearnerOracle
     keys = [f"agent_{i}" for i in range(n)]
-    rep = Basic_RNN(input_shape=(obs_dim,), hidden_sizes=None, initialize=nn.init.orthogonal_, activation=nn.ReLU,
-                    device='cpu', fc_hidden_sizes=[64], recurrent_hidden_size=64, N_recurrent_layers=1, dropout=0, rnn='GRU')
-    enc = AgentFeatureEncoder(rep, build_identity_encoder(n, 'none', None, 'cpu'), IdentityFeatureFusion(64, 0, 'concat'))
-    q = nn.ModuleDict({'shared': DiscreteActionValueCritic(enc, Discrete(A), [64], None, nn.init.orthogonal_, nn.ReLU, 'cpu')})
-    grouping = AgentGrouping.shared(keys)
-    model = MixingQNetwork(grouping, q, QMIX_Mixer(S, 32, 32, n, 'cpu'), use_rnn=True, device='cpu')
-    cfg = Namespace(distributed_training=False, episode_length=T, use_grad_clip=False, grad_clip_norm=10, device='cpu',
-                    model_dir='/tmp/x', running_steps=100000, parallels=4, use_parameter_sharing=True, use_rnn=True,
-                    use_actions_mask=False, learning_rate=7e-4, sync_frequency=2, double_q=True, n_epochs=1,
-                    start_training=0, gamma=0.99, end_factor_lr_decay=lr_decay)
-    lrn = QMIX_Learner(cfg, grouping, model, BaseCallback())
     om = QMIXModelOracle(n, obs_dim, A, S)
-    om.load_state_dict(model.state_dict(), strict=True)
+    om.load_state_dict(seeded_state_dict(om.state_dict(), seed), strict=True)
     orc = QMIXLearnerOracle(om, keys, learning_rate=7e-4, sync_frequency=2, double_q=True, end_factor_lr_decay=lr_decay,
-                            total_iters=lrn.total_iters, detach_q_eval=True)   # the reference as it is (see oracle/qmix.py)
-    return keys, model, lrn, om, orc
+                            total_iters=total_iters, detach_q_eval=True)   # the reference as it is (see oracle/qmix.py)
+    return keys, om, orc
 
 
 def test_qmix_buffer_and_learner_live(ref):
-    from gymnasium.spaces import Box, Discrete
-    from xuance.common.memory_tools_marl import MARL_OffPolicyBuffer_RNN
     from oracle.qmix import EpisodeReplayOracle
-    torch.manual_seed(0)
+    r = ref["qmix"]
     n, obs_dim, A, S, T = 5, 72, 12, 98, 12
-    keys, model, lrn, om, orc = _qmix_pair(n, obs_dim, A, S, T)
-    init = {k: v.clone() for k, v in model.state_dict().items()}
+    keys, om, orc = _qmix_oracle(n, obs_dim, A, S, r["total_iters"])
+    init = {k: v.clone() for k, v in om.state_dict().items()}
     n_envs, C, Be = 3, 12, 6
-    rb = MARL_OffPolicyBuffer_RNN(agent_keys=keys, state_space=Box(-1, 1, (S,)),
-                                  obs_space={k: Box(-1, 1, (obs_dim,)) for k in keys},
-                                  act_space={k: Discrete(A) for k in keys}, n_envs=n_envs, buffer_size=C,
-                                  batch_size=Be, max_episode_steps=T, use_actions_mask=False)
     ob = EpisodeReplayOracle(keys, obs_dim, S, n_envs, C, Be, T)
     for ev in qmix_episode_stream(np.random.default_rng(0), keys, n_envs, T, obs_dim, A, S, 5):
         if ev[0] == 'store':
-            rb.store(**ev[1]), ob.store(**ev[1])
+            ob.store(**ev[1])
         else:
-            rb.finish_path(ev[1], **ev[2]), ob.finish_path(ev[1], **ev[2])
+            ob.finish_path(ev[1], **ev[2])
     for k in ('obs', 'actions', 'rewards', 'terminals', 'agent_mask'):
         for a in keys:
-            assert np.array_equal(rb.data[k][a], ob.data[k][a]), k
-    assert np.array_equal(rb.data['filled'], ob.data['filled']) and np.array_equal(rb.data['state'], ob.data['state'])
-    assert rb.ptr == ob.ptr and rb.size == ob.size
+            assert r["data"][k][a] == digest(ob.data[k][a]), k
+    assert r["data"]['filled'] == digest(ob.data['filled']) and r["data"]['state'] == digest(ob.data['state'])
+    assert r["ptr"] == ob.ptr and r["size"] == ob.size
     for it in range(3):
         np.random.seed(it)
-        s1 = rb.sample()
-        np.random.seed(it)
-        s2 = ob.sample()
-        i1, i2 = lrn.update(s1), orc.update(s2)
+        i2 = orc.update(ob.sample())
+        i1 = r["updates"][it]
         np.testing.assert_allclose(i1['loss_Q'], i2['loss_Q'], rtol=1e-5)
         np.testing.assert_allclose(i1['predictQ'], i2['predictQ'], rtol=1e-5, atol=1e-7)
         assert i1['learning_rate'] == i2['learning_rate']
-    sd1, sd2 = model.state_dict(), om.state_dict()
-    for k in sd1:
-        np.testing.assert_allclose(sd2[k].numpy(), sd1[k].numpy(), rtol=1e-5, atol=1e-6, err_msg=k)
-    # reference quirk pinned here: with use_rnn=True its agent networks never receive a gradient (only the mixer moves)
-    moved = {k for k in sd1 if k.startswith("individual_q_networks") and not torch.equal(sd1[k], init[k])}
+    sd = om.state_dict()
+    _close_params(sd, r["final"])
+    # reference quirk (asserted on the reference when the fixture was recorded): with use_rnn=True its agent networks
+    # never receive a gradient - only the mixer moves; the oracle in detach_q_eval mode does the same
+    moved = {k for k in sd if k.startswith("individual_q_networks") and not torch.equal(sd[k], init[k])}
     assert not moved, moved
 
 
 def test_sac_learner_live(ref):
-    from copy import deepcopy
-    from gymnasium.spaces import Box
-    from xuance.common import BaseCallback
-    from xuance.torch.rl_models.representations.mlp import Basic_Identical
-    from xuance.torch.rl_models.actors.gaussian_actors import SAC_GaussianActor
-    from xuance.torch.rl_models.critics.twin_critics import TwinActionValueCritic
-    from xuance.torch.rl_models.architectures.single_agent.actor_critic import SoftActorCritic
-    from xuance.torch.learners import SAC_Learner
     from oracle.sac import SACModelOracle, SACLearnerOracle
-    torch.manual_seed(0)
+    r = ref["sac"]
     obs_dim, act_dim, B = 17, 6, 64
-    aspace = Box(-1, 1, (act_dim,), np.float32)
-    rep = Basic_Identical((obs_dim,), device='cpu')
-    actor = SAC_GaussianActor(rep, [256, 256], aspace, None, None, nn.LeakyReLU, nn.Tanh, 'cpu')
-    critic = TwinActionValueCritic(deepcopy(rep), aspace, [256, 256], None, None, nn.LeakyReLU, 'cpu')
-    model = SoftActorCritic(actor, critic)
-    cfg = Namespace(distributed_training=False, episode_length=1000, use_grad_clip=False, grad_clip_norm=0.5, device='cpu',
-                    model_dir='/tmp/x', running_steps=100000, parallels=4, start_training=0, training_frequency=1,
-                    learning_rate_actor=1e-3, learning_rate_critic=1e-3, tau=0.005, gamma=0.99, alpha=0.2,
-                    use_automatic_entropy_tuning=True, end_factor_lr_decay=0.7)
-    lrn = SAC_Learner(cfg, model, BaseCallback())
     om = SACModelOracle(obs_dim, act_dim)
-    om.load_state_dict(model.state_dict(), strict=True)
-    orc = SACLearnerOracle(om, end_factor_lr_decay=0.7, total_iters=lrn.total_iters)
+    om.load_state_dict(seeded_state_dict(om.state_dict(), 1), strict=True)
+    orc = SACLearnerOracle(om, end_factor_lr_decay=0.7, total_iters=r["total_iters"])
     rng = np.random.default_rng(1)
     for it in range(3):
         s = {"obs": rng.normal(size=(B, obs_dim)).astype(np.float32),
              "actions": rng.uniform(-1, 1, size=(B, act_dim)).astype(np.float32),
              "obs_next": rng.normal(size=(B, obs_dim)).astype(np.float32),
              "rewards": rng.normal(size=B).astype(np.float32), "terminals": (rng.random(B) < 0.1).astype(np.float32)}
-        # the reference draws its noise from torch's global RNG: replay the same stream for the oracle
+        # the reference drew its noise from torch's global RNG seeded with 100 + it: replay the same stream
         torch.manual_seed(100 + it)
         n1 = torch.randn(B, act_dim)
         n2 = torch.randn(B, act_dim)
-        torch.manual_seed(100 + it)
-        i1 = lrn.update(**s)
         i2 = orc.update(n1, n2, **s)
         for k in ("Qloss", "Ploss", "Qvalue", "alpha", "alpha_loss"):
-            np.testing.assert_allclose(i2[k], i1[k], rtol=1e-5, atol=1e-6, err_msg=k)
-    sd1, sd2 = model.state_dict(), om.state_dict()
-    for k in sd1:
-        np.testing.assert_allclose(sd2[k].numpy(), sd1[k].numpy(), rtol=1e-5, atol=1e-6, err_msg=k)
+            np.testing.assert_allclose(i2[k], r["updates"][it][k], rtol=1e-5, atol=1e-6, err_msg=k)
+    _close_params(om.state_dict(), r["final"])
 
 
 @pytest.mark.parametrize("kind", ["a2c", "pg", "ddqn"])
 def test_sibling_learners_live(ref, kind):
     """A2C / PG / DDQN (SURVEY.md section 8f-3): oracle variants next to the reference learners."""
-    from gymnasium.spaces import Discrete
-    from xuance.common import BaseCallback
-    from xuance.torch.learners import A2C_Learner, PG_Learner, DDQN_Learner
-    from xuance.torch.rl_models.representations import AC_CNN_Atari, Basic_CNN
-    from xuance.torch.rl_models.heads import CategoricalActorHead, ValueHead
-    from xuance.torch.rl_models.architectures.single_agent.actor_critic import SharedActorCritic
-    from xuance.torch.rl_models.architectures.single_agent.deep_q_network import DeepQNetwork
     from oracle.nets import SharedActorCriticOracle, DeepQNetworkOracle
     from oracle.learners import PPOLearnerOracle, DQNLearnerOracle
-    torch.manual_seed(5)
+    r = ref["siblings"][kind]
     A, B = 5, 12
-    cfg = Namespace(distributed_training=False, episode_length=1000, use_grad_clip=True, grad_clip_norm=0.5, device="cpu",
-                    model_dir="/tmp/x", running_steps=4096 * 10, parallels=32, learning_rate=2.5e-4, end_factor_lr_decay=0.5,
-                    horizon_size=128, n_epochs=4, n_minibatch=4, vf_coef=0.25, ent_coef=0.01, gamma=0.99, sync_frequency=2,
-                    start_training=0, training_frequency=1)
     rng = np.random.default_rng(3)
     if kind == "ddqn":
-        rep = Basic_CNN(input_shape=(84, 84, 4), kernels=[8, 4, 3], strides=[4, 2, 1], filters=[32, 64, 64],
-                        activation=nn.ReLU, device="cpu")
-        model = DeepQNetwork(rep, [512], Discrete(A), None, None, nn.ReLU, "cpu")
-        lrn = DDQN_Learner(cfg, model, BaseCallback())
         om = DeepQNetworkOracle(A)
-        om.load_state_dict(model.state_dict())
+        om.load_state_dict(seeded_state_dict(om.state_dict(), 2), strict=True)
         orc = DQNLearnerOracle(om, learning_rate=2.5e-4, sync_frequency=2, use_grad_clip=True, end_factor_lr_decay=0.5,
-                               total_iters=lrn.total_iters, double_q=True)
+                               total_iters=r["total_iters"], double_q=True)
     else:
-        rep = AC_CNN_Atari(input_shape=(84, 84, 4), kernels=[8, 4, 3], strides=[4, 2, 1], filters=[32, 64, 64],
-                           activation=nn.ReLU, device="cpu", fc_hidden_sizes=[512])
-        model = SharedActorCritic(rep, CategoricalActorHead(512, [], A, None, nn.init.orthogonal_, nn.ReLU, "cpu"),
-                                  ValueHead(512, [], None, nn.init.orthogonal_, nn.ReLU, "cpu"))
-        lrn = (A2C_Learner if kind == "a2c" else PG_Learner)(cfg, model, BaseCallback())
         om = SharedActorCriticOracle(A)
-        om.load_state_dict(model.state_dict())
+        om.load_state_dict(seeded_state_dict(om.state_dict(), 2), strict=True)
         # a2c_learner.py:21: LinearLR(total_iters=config.running_steps); pg_learner.py:22: total_iters=self.total_iters
         orc = PPOLearnerOracle(om, end_factor_lr_decay=0.5, kind=kind,
-                               total_iters=cfg.running_steps if kind == "a2c" else lrn.total_iters)
+                               total_iters=4096 * 10 if kind == "a2c" else r["total_iters"])
     for it in range(3):
         s = {"obs": rng.integers(0, 256, size=(B, 84, 84, 4), dtype=np.uint8).astype(np.float32),
              "actions": rng.integers(0, A, size=B).astype(np.float32),
@@ -228,114 +164,68 @@ def test_sibling_learners_live(ref, kind):
              "aux_batch": {"old_logp": np.zeros(B, np.float32)},
              "obs_next": rng.integers(0, 256, size=(B, 84, 84, 4), dtype=np.uint8).astype(np.float32),
              "rewards": rng.normal(size=B).astype(np.float32), "terminals": (rng.random(B) < 0.2).astype(np.float32)}
-        i1, i2 = lrn.update(**s), orc.update(**s)
+        i2, i1 = orc.update(**s), r["updates"][it]
         if kind == "ddqn":
             np.testing.assert_allclose(i2["Qloss"], i1["Qloss"], rtol=1e-5)
         else:
-            np.testing.assert_allclose(i2["actor_loss"], i1["actor-loss"], rtol=1e-5, atol=1e-7)
+            np.testing.assert_allclose(i2["actor_loss"], i1["actor_loss"], rtol=1e-5, atol=1e-7)
             np.testing.assert_allclose(i2["entropy"], i1["entropy"], rtol=1e-5)
-    sd1, sd2 = model.state_dict(), om.state_dict()
-    for k in sd1:
-        np.testing.assert_allclose(sd2[k].numpy(), sd1[k].numpy(), rtol=1e-5, atol=1e-6, err_msg=k)
+    _close_params(om.state_dict(), r["final"])
 
 
 def test_multi_agent_vector_env_live(ref):
     """DummyVecMultiAgentEnv + XuanCeMultiAgentEnvWrapper (the QMIX caller side, vector_envs/dummy/dummy_vec_maenv.py:17-84,
-    environment/utils/wrapper.py:141-226) next to the live reference classes over the SAME raw synthetic environments:
-    identical observations, reward / terminated dicts, truncation flags and infos (episode_step, episode_score, agent_mask,
-    avail_actions, state, reset_obs / reset_avail_actions / reset_state at episode ends) step for step."""
-    from xuance.environment.utils.wrapper import XuanCeMultiAgentEnvWrapper as RefWrapper
-    from xuance.environment.vector_envs.dummy.dummy_vec_maenv import DummyVecMultiAgentEnv as RefVec
+    environment/utils/wrapper.py:141-226) next to the reference classes' recorded run over the SAME raw synthetic
+    environments: identical observations, reward / terminated dicts, truncation flags and infos (episode_step,
+    episode_score, agent_mask, avail_actions, state, reset_obs / reset_avail_actions / reset_state at episode ends) step
+    for step."""
     from xuance_b200.environment.ma_envs import SyntheticSMACEnv, XuanCeMultiAgentEnvWrapper
     from xuance_b200.environment.vector_envs.dummy_vec_maenv import DummyVecMultiAgentEnv
+    r = ref["ma_vec_env"]
     kw = dict(n_agents=3, obs_dim=16, state_dim=20, n_actions=5, episode_limit=7, p_death=0.1)
     n_envs = 3
-    mk_ref = [lambda env_seed=0: RefWrapper(SyntheticSMACEnv(seed=env_seed, **kw)) for _ in range(n_envs)]
-    mk_own = [lambda env_seed=0: XuanCeMultiAgentEnvWrapper(SyntheticSMACEnv(seed=env_seed, **kw)) for _ in range(n_envs)]
-    rv, ov = RefVec(mk_ref, 11), DummyVecMultiAgentEnv(mk_own, 11)
-    assert rv.num_envs == ov.num_envs and rv.agents == ov.agents and rv.num_agents == ov.num_agents
-    assert rv.max_episode_steps == ov.max_episode_steps and rv.state_space.shape == ov.state_space.shape
-    (ro, ri), (oo, oi) = rv.reset(), ov.reset()
+    ov = DummyVecMultiAgentEnv([lambda env_seed=0: XuanCeMultiAgentEnvWrapper(SyntheticSMACEnv(seed=env_seed, **kw))
+                                for _ in range(n_envs)], 11)
+    assert r["num_envs"] == ov.num_envs and r["agents"] == list(ov.agents) and r["num_agents"] == ov.num_agents
+    assert r["max_episode_steps"] == ov.max_episode_steps and r["state_shape"] == tuple(ov.state_space.shape)
+    (ro, ri), (oo, oi) = r["reset"], ov.reset()
     _same(ro, oo, "reset obs"), _same(ri, oi, "reset info")
-    rng = np.random.default_rng(2)
     ends = 0
-    for t in range(40):
-        # a random AVAILABLE action per agent (the same for both stacks)
-        acts = [{a: int(rng.choice(np.flatnonzero(rv.buf_avail_actions[e][a]))) for a in rv.agents} for e in range(n_envs)]
-        r, o = rv.step(acts), ov.step(acts)
-        for name, x, y in zip(("obs", "rewards", "terminated", "truncated", "infos"), r, o):
+    for t, st in enumerate(r["steps"]):
+        o = ov.step(st["actions"])
+        for name, x, y in zip(("obs", "rewards", "terminated", "truncated", "infos"), st["out"], o):
             _same(x, y, "t=%d %s" % (t, name))
-        _same(rv.buf_state, ov.buf_state, "state"), _same(rv.buf_avail_actions, ov.buf_avail_actions, "avail")
-        ends += sum("reset_obs" in i for i in r[4])
+        _same(st["state"], ov.buf_state, "state"), _same(st["avail"], ov.buf_avail_actions, "avail")
+        ends += sum("reset_obs" in i for i in st["out"][4])
     assert ends >= 5                                    # episode ends (death of all agents / truncation) were exercised
-    rv.close(), ov.close()
+    ov.close()
 
 
-def test_qmix_action_mask_variant_against_the_reference_with_its_slice_corrected(ref, monkeypatch):
+def test_qmix_action_mask_variant_against_the_reference_with_its_slice_corrected(ref):
     """use_rnn=True with use_actions_mask=True: the reference slices the AGENT axis of the availability mask
     (iql_learner.py:78, ``[:, 1:]``) and raises; the evidently intended statement slices the time axis (``[:, :, 1:]``).
     The oracle's masked variant (and through it xb_qmix_select_fwd's masked arg-max / target, tests/test_gpu_qmix.py) is pinned
-    here against the LIVE reference learner with that ONE expression corrected at run time - the reference source is read
-    from /root/reference, patched in memory and executed; nothing of it is stored in this repository."""
-    import inspect
-    import textwrap
-    from gymnasium.spaces import Box, Discrete
-    from xuance.common.memory_tools_marl import MARL_OffPolicyBuffer_RNN
-    from xuance.torch.learners.multi_agent_rl import iql_learner as iql
-    torch.manual_seed(1)
-    n, obs_dim, A, S, T = 4, 24, 7, 30, 9
-    keys, model, lrn, om, orc = _qmix_pair(n, obs_dim, A, S, T)
-    lrn.use_actions_mask = lrn.config.use_actions_mask = True
+    here against the reference learner with that ONE expression corrected in memory when the fixture was recorded
+    (tests/golden/make_reference_live.py; nothing of the reference source is stored here), on the samples its replay
+    buffer drew."""
+    r = ref["qmix_action_mask"]
+    assert r["unpatched_raised"]                        # the reference as it is cannot run this configuration
+    n, obs_dim, A, S = 4, 24, 7, 30
+    _, om, orc = _qmix_oracle(n, obs_dim, A, S, r["total_iters"], seed=3)
+    snap = {k: v.clone() for k, v in om.state_dict().items()}
     orc.use_actions_mask = True
-    n_envs, C, Be = 3, 12, 6
-    rb = MARL_OffPolicyBuffer_RNN(agent_keys=keys, state_space=Box(-1, 1, (S,)),
-                                  obs_space={k: Box(-1, 1, (obs_dim,)) for k in keys},
-                                  act_space={k: Discrete(A) for k in keys}, n_envs=n_envs, buffer_size=C,
-                                  batch_size=Be, max_episode_steps=T, use_actions_mask=True,
-                                  avail_actions_shape={k: (A,) for k in keys})
-    rng = np.random.default_rng(4)
-
-    def avail(shape_prefix):
-        a = rng.random(shape_prefix + (A,)) < 0.6
-        a[..., 0] = True                                    # never an all-unavailable row
-        return a
-    for ev in qmix_episode_stream(np.random.default_rng(3), keys, n_envs, T, obs_dim, A, S, 5):
-        if ev[0] == 'store':
-            rb.store(avail_actions={k: avail((n_envs,)) for k in keys}, **ev[1])
-        else:
-            rb.finish_path(ev[1], avail_actions={k: avail(()) for k in keys}, **ev[2])
-    np.random.seed(0)
-    sample = rb.sample()
-    assert sample['avail_actions'][keys[0]].shape == (Be, T + 1, A)
-    # 1. the reference as it is cannot run this configuration
-    snap = {k: v.clone() for k, v in model.state_dict().items()}
-    with pytest.raises((RuntimeError, IndexError)):
-        lrn.update(sample)
-    model.load_state_dict(snap)
-    lrn.iterations = 0
-    # 2. the same learner with the one slice corrected
-    src = textwrap.dedent(inspect.getsource(iql.IQL_Learner._forward_transitions))
-    bad = "batch.avail_actions.group(group)[:, 1:]"
-    assert src.count(bad) == 1, "the reference's masked RNN branch changed - re-read iql_learner.py:60-81"
-    scope = {}
-    exec(compile(src.replace(bad, "batch.avail_actions.group(group)[:, :, 1:]"), "iql_learner.py (slice corrected)", "exec"),
-         vars(iql), scope)
-    monkeypatch.setattr(iql.IQL_Learner, "_forward_transitions", scope["_forward_transitions"])
     for it in range(3):
-        np.random.seed(10 + it)
-        s = rb.sample()
-        i1, i2 = lrn.update(s), orc.update(s)
+        s = r["samples"][it]
+        assert s['avail_actions'][f"agent_0"].shape[-1] == A
+        i2, i1 = orc.update(s), r["updates"][it]
         np.testing.assert_allclose(i1['loss_Q'], i2['loss_Q'], rtol=1e-5)
         np.testing.assert_allclose(i1['predictQ'], i2['predictQ'], rtol=1e-5, atol=1e-7)
-    sd1, sd2 = model.state_dict(), om.state_dict()
-    for k in sd1:
-        np.testing.assert_allclose(sd2[k].numpy(), sd1[k].numpy(), rtol=1e-5, atol=1e-6, err_msg=k)
+    _close_params(om.state_dict(), r["final"])
     # the masks mattered: the same first update without them has a different loss
-    _, _, _, om_m, orc_m = _qmix_pair(n, obs_dim, A, S, T)
-    _, _, _, om_u, orc_u = _qmix_pair(n, obs_dim, A, S, T)
+    _, om_m, orc_m = _qmix_oracle(n, obs_dim, A, S, r["total_iters"], seed=3)
+    _, om_u, orc_u = _qmix_oracle(n, obs_dim, A, S, r["total_iters"], seed=3)
     om_m.load_state_dict(snap, strict=True), om_u.load_state_dict(snap, strict=True)
     om_m.copy_target(), om_u.copy_target()
     orc_m.use_actions_mask = True
-    np.random.seed(10)
-    s = rb.sample()
+    s = r["samples"][0]
     assert abs(orc_m.update(s)['loss_Q'] - orc_u.update(s)['loss_Q']) > 1e-6

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Secondary measurements for BASELINE configs 3-5 (parity-test cases, not the headline): sample + update throughput of
 DQN+PER (2^20-transition HBM replay, B=512), SAC (1M replay, B=1024) and QMIX (5 agents x 72-d, T=60, 32 episodes)
-on one B200, next to the oracle port of the reference's torch-CPU path on the host.  Prints one JSON object.
+on one GPU, next to the oracle port of the reference's torch-CPU path on the host.  Prints one JSON object.
 
     python tools/algo_bench.py [--iters 200] [--cpu-iters 5] [--no-cpu] [--graph]
     torchrun --nnodes=1 --nproc-per-node G --master-addr 127.0.0.1 tools/algo_bench.py --no-cpu --graph    (G GPUs)

@@ -14,15 +14,15 @@ def report(label, fn):
         fn()
     torch.cuda.synchronize()
     fn()
-    buf = (ctypes.c_ulonglong * (12 * 148))()
+    buf = (ctypes.c_ulonglong * (12 * 132))()
     lib = _lib.load()
-    rc = lib.xb_debug_k12_timing(ctypes.addressof(buf), 148)
+    rc = lib.xb_debug_k12_timing(ctypes.addressof(buf), 132)
     assert rc == 0, rc
-    t = np.frombuffer(buf, dtype=np.uint64).reshape(148, 12).astype(np.float64)
+    t = np.frombuffer(buf, dtype=np.uint64).reshape(132, 12).astype(np.float64)
     m = t.mean(0)
-    print("%-34s MMA %8.0f clk: wait operands %4.1f%%  epilogue %4.1f%%  tile %4.1f%% | producer: wait ring %4.1f%%  tile buf %4.1f%% | "
-          "epilogue: wait acc %4.1f%%" % (label, m[0], 100 * m[1] / m[0], 100 * m[2] / m[0], 100 * m[3] / m[0],
-                                          100 * m[5] / max(m[4], 1), 100 * m[6] / max(m[4], 1), 100 * m[8] / max(m[7], 1)))
+    # consumer warpgroups (wgmma issue + epilogue): slots 0-1, 3; producer warpgroup: slots 4-6 (conv_tc.cu, xb_k12_timing)
+    print("%-34s consumer %8.0f clk: wait operands %4.1f%%  wait halo tile %4.1f%% | producer: wait ring %4.1f%%  wait tile buf %4.1f%%"
+          % (label, m[0], 100 * m[1] / max(m[0], 1), 100 * m[3] / max(m[0], 1), 100 * m[5] / max(m[4], 1), 100 * m[6] / max(m[4], 1)))
 
 
 def main():

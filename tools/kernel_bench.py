@@ -2,7 +2,7 @@
 """Per-kernel roofline numbers for every entry point of include/xb200.h, at the BASELINE shapes and at HBM-sized
 shapes (SURVEY.md section 7 "hard parts": at the named PPO shape K2/K4/K5 move < 1 MB and are launch-bound, so the
 bandwidth fraction is also reported at a scaled shape).  CUDA events on the launching stream, >= 3 warm-ups, L2
-flushed between timed launches (256 MB memset).  Prints one JSON object; profiles/rNN_kernels.json keeps a copy.
+flushed between timed launches (256 MB memset).  Prints one JSON object.
 
     python tools/kernel_bench.py [--only k2,k4] [--reps 20]      (k12 / k12box / k3p: the tensor-core encoder layers, gathered and TMA-box / halo variants)
 """
@@ -210,7 +210,7 @@ def main():
                 us_tc = timeit(lambda: mixer(q, st), R)
                 mixer.use_tensor_core_forward = False
                 us_lib = timeit(lambda: mixer(q, st), R)
-            e = entry("K9-TC xb_qmix_mix_fused_fwd (tcgen05, incl. torch.cat of weights)", f"{Rr} rows, S=98, n=5", us_tc,
+            e = entry("K9-TC xb_qmix_mix_fused_fwd (wgmma, incl. torch.cat of weights)", f"{Rr} rows, S=98, n=5", us_tc,
                       Rr * (S + n + 1) * 4, hbm, flops, tpk)
             e["vs_cublas_plus_epilogue_us"] = round(us_lib, 2)
             add(e)

@@ -1,7 +1,7 @@
-"""xuance_b200 - B200-native rollout->update hot path behind the xuance.torch Agent / Learner / buffer API.
+"""xuance_b200 - H100-native rollout->update hot path behind the xuance.torch Agent / Learner / buffer API.
 
 Host code is Python/PyTorch (device memory, streams, torch.distributed); every hot operation is a hand-written
-sm_100a kernel reached through the C-ABI in include/xb200.h (libxb200.so, built in-tree by xuance_b200.build)."""
+sm_90a kernel reached through the C-ABI in include/xb200.h (libxb200.so, built in-tree by xuance_b200.build)."""
 __version__ = "0.1.0"
 
 

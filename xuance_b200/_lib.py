@@ -86,7 +86,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            "xuance_b200: %s is missing - build it with `python -m xuance_b200.build` (nvcc, sm_100a). "
+            "xuance_b200: %s is missing - build it with `python -m xuance_b200.build` (nvcc, sm_90a). "
             "There is no CPU fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, sig in list(_SIGNATURES.items()) + list(_OPTIONAL.items()):

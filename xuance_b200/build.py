@@ -1,9 +1,9 @@
-"""In-tree build of the xb200 C-ABI shared library (nvcc, sm_100a only).
+"""In-tree build of the xb200 C-ABI shared library (nvcc, sm_90a only: H100).
 
     python -m xuance_b200.build [--force]
 
-Produces xuance_b200/libxb200.so next to this file.  The .so is git-ignored but travels to the GPU box with the
-gpurun snapshot.  No torch headers are involved: the library is plain CUDA runtime + extern "C"."""
+Produces xuance_b200/libxb200.so next to this file (git-ignored, rebuilt when a source or a flag changes).  No torch
+headers are involved: the library is plain CUDA runtime + extern "C"."""
 import hashlib
 import os
 import subprocess
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libxb200.so")
 STAMP = os.path.join(HERE, ".libxb200.stamp")
 SOURCES = ["api.cu", "rollout.cu", "losses.cu", "per_tree.cu", "optim.cu", "sac.cu", "qmix_mix.cu", "qmix_tc.cu", "act.cu", "conv_tc.cu", "obs_planes.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--use_fast_math=false", "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v",
               "--expt-relaxed-constexpr", "--expt-extended-lambda"]
 

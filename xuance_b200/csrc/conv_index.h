@@ -1,7 +1,7 @@
 // Index arithmetic of the gathered-operand tensor-core GEMM (conv_tc.cu), kept free of CUDA so that the SAME functions
 // are compiled into the kernel and into the host-side layout test (tests/csrc/conv_index_test.cpp, run by
 // tests/test_conv_index.py): the test stages operands with these functions into an emulated shared-memory image, reads
-// them back the way the tcgen05 shared-memory descriptors do (validated on hardware by K9-TC) and compares with a direct
+// them back the way the wgmma shared-memory descriptors do and compares with a direct
 // convolution.
 //
 // The GEMM:  D[m, n] = sum_k A[m, k] * W[n, k]
@@ -25,7 +25,7 @@
 
 #define XB_CONV_MAX_TAPS 64
 #define XB_CONV_KC 64           // K elements per pipeline stage (8 core matrices, 128 B per operand row)
-#define XB_CONV_TILE_M 128      // rows per CTA tile = TMEM lanes
+#define XB_CONV_TILE_M 128      // rows per CTA tile (two warpgroups of 64)
 
 #define XB_CONV_MAX_UNITS 1024  // 16-byte K units per GEMM row the tap table holds: K = T * C <= 8192
 #define XB_CONV_PRODUCERS 256   // producer threads per CTA (8 warps)
@@ -117,7 +117,7 @@ XB_HD int64_t xb_wgrad_sites_per_split(int64_t M, int splits) {
 // element offset relative to the site's un-shifted pixel) and everything that does not depend on the chunk once per tile
 // (XbSite per row): a unit then costs two adds, two unsigned compares and a select.  (The first version recomputed
 // tap = k / C and the site by integer division for every unit; with ONE producer warp per scheduler those dependent
-// instruction chains, not the loads, set the pace: ~4.5k cycles per chunk on B200 whatever the byte count.)
+// instruction chains, not the loads, set the pace whatever the byte count.)
 //
 // Mapping (row-coalesced): in the canonical no-swizzle layouts the shared-memory bank of a 16-byte unit depends only on
 // (row & 7) [K-major] / (site & 7) [MN-major], so a warp instruction is conflict-free as soon as its 32 lanes hold each of

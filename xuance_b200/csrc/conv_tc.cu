@@ -1,33 +1,33 @@
-// K12: gathered-operand GEMM on the 5th-generation tensor cores (tcgen05.mma, TMEM accumulators) for the NatureCNN layers
+// K12: gathered-operand GEMM on the Hopper tensor cores (wgmma, accumulators in registers) for the NatureCNN layers
 // (cnn.py:45-50, 84-101) - forward, data gradient, weight gradient and bias gradient of the three convolutions and the hidden
-// layer, the 85 % of the fp32 PPO step that cuDNN's CUDA-core fp32 convolutions took (DESIGN.md sections 3, 3a, 7).
+// layer, the bulk of the fp32 PPO step that cuDNN's CUDA-core fp32 convolutions took (DESIGN.md sections 3, 3a, 7).
 //
 //   D[m, n] = sum_{t, c} in[b, y*sy + dy[t], x*sx + dx[t], c] * W[n, t*C + c]  (+ bias[n], ReLU)      conv_index.h
 //
 // Numerics: every fp32 operand travels as 1-3 bf16 planes (x = sum of its planes); the kept plane products are accumulated
-// in fp32 in TMEM, one accumulator per order of magnitude, and added smallest first in the epilogue (see the kernel).
+// in fp32, one accumulator per order of magnitude, and added smallest first in the epilogue (see the kernel).
 //
-// Structure (one CTA per SM, persistent over work items = (128-row tile, column tile[, split]), 13 warps):
-//   warps 5-12 producers : four ways to fill a stage, chosen per operand by the host entry point:
+// Structure (one CTA per SM, persistent over work items = (128-row tile, column tile[, split]), 12 warps):
+//   warps 8-11 producers : four ways to fill a stage, chosen per operand by the host entry point:
 //                          * TMA tiles with the 128-byte swizzle for plain matrices (packed weights, output gradients, the
 //                            Linear layer's inputs), all planes of an operand in one cp.async.bulk.tensor;
 //                          * TMA boxes over padded-row activations (a_box: xb_gemm_box_tc / xb_wgrad_box_tc), rank-5 view
 //                            {channel, pixel, row phase, row / stride, plane};
 //                          * a RESIDENT activation tile (a_halo: xb_gemm_halo_tc) - one box per plane and M tile, taps are
 //                            descriptor offsets, only the weights stream through the ring;
-//                          * 16-byte cp.async gathers into the no-swizzle canonical layout (conv1's raw pixels), 256
-//                            threads, row-coalesced mapping (conv_index.h), zero-fill for padding taps, ASYNCHRONOUS
-//                            arrival on the stage's full barrier (cp.async.mbarrier.arrive.noinc).
+//                          * 16-byte cp.async gathers into the no-swizzle canonical layout (conv1's raw pixels): each of the
+//                            128 threads plays producers pt and pt + 128 of the 256-thread mapping of conv_index.h,
+//                            row-coalesced, zero-fill for padding taps, ASYNCHRONOUS arrival on the stage's full barrier
+//                            (cp.async.mbarrier.arrive.noinc).
 //                          One elected thread arms the barrier with the TMA byte count; no producer waits for a load.
-//   warp 4     MMA       : the warp runs the loop on uniform values, the tcgen05 instructions are predicated on lane 0:
-//                          wait full[stage], PA tcgen05.mma per K step of 16 (A plane pa x the first PB - pa B planes,
-//                          adjacent in the stage = ONE operand of (PB - pa) * N rows; descriptor = per-launch template +
-//                          start address), commit onto empty[stage]; after the last chunk commit onto acc_full[a].  Two
-//                          accumulator sets in TMEM.
-//   warps 0-3  epilogue  : thread = row = TMEM lane.  tcgen05.ld 32 columns at a time from each accumulator group, added
-//                          smallest first, bias + ReLU / ReLU-derivative mask, the row written as fp32 and / or as the bf16
-//                          planes the next layer consumes (into its padded layout), and the column sums of the tile
-//                          (the bias-gradient partials of the layer below).
+//   warps 0-7  consumers : two warpgroups, rows 0-63 and 64-127 of the tile (M = 64 per wgmma).  Per K step of 16 and A plane
+//                          pa, wgmmas of 64 / 32 columns multiply it with the first PB - pa B planes (adjacent in the stage =
+//                          ONE operand of (PB - pa) * N rows) into the register accumulator blocks of groups pa .. PB-1; a
+//                          stage is released when the wgmma group after it was issued has retired the one that read it.
+//                          The epilogue runs on the fragments: accumulator groups added smallest first, bias + ReLU /
+//                          ReLU-derivative mask, the rows written as fp32 and / or as the bf16 planes the next layer consumes
+//                          (into its padded layout), and the column sums of the tile (the bias-gradient partials of the layer
+//                          below).
 #include <cstdlib>
 
 #include <cuda.h>      // CUtensorMap + the cuTensorMapEncodeTiled prototype (resolved at run time through the runtime API)
@@ -39,16 +39,16 @@ namespace {
 using namespace xbtc;
 
 constexpr int KC = XB_CONV_KC, TILE_M = XB_CONV_TILE_M;
-constexpr int EPI_WARPS = 4, PROD_WARPS = XB_CONV_PRODUCERS / 32;
-constexpr int MMA_WARP = EPI_WARPS;
-constexpr int THREADS = (EPI_WARPS + 1 + PROD_WARPS) * 32;
+constexpr int CONS_WARPS = 8;                              // two consumer warpgroups
+constexpr int PROD_THREADS = XB_CONV_PRODUCERS / 2;        // one producer warpgroup, two conv_index.h producers per thread
+constexpr int THREADS = CONS_WARPS * 32 + PROD_THREADS;
 constexpr int MAX_STAGES = 6;
 constexpr int XB_HALO_MAX_CHUNKS = 16;
-constexpr int XB_K12_MAX_DYN_SMEM = 212 * 1024;      // + ~14 KB static (barriers, bias, column sums, tap table) <= 227 KB
+constexpr int XB_K12_MAX_DYN_SMEM = 208 * 1024;      // + ~18 KB static (barriers, bias, column sums, tap table) <= 227 KB
 
 // Optional role timing (XB_K12_TIMING=1): clock64 cycles each role of CTA b spent inside its barrier waits, written at kernel
-// exit to xb_k12_timing[b][..]: 0 MMA total, 1 MMA wait full (operands), 2 MMA wait acc_empty (epilogue), 3 MMA wait a_full (halo
-// tile), 4 producer total, 5 producer wait empty (ring), 6 producer wait a_empty, 7 epilogue total, 8 epilogue wait acc_full
+// exit to xb_k12_timing[b][..]: 0 consumer total, 1 consumer wait full (operands), 3 consumer wait a_full (halo tile),
+// 4 producer total, 5 producer wait empty (ring), 6 producer wait a_empty (tools/k12_timing.py); the other slots are unused
 __device__ unsigned long long xb_k12_timing[160][12];
 
 struct ConvParams {
@@ -74,7 +74,7 @@ struct ConvParams {
     // descriptor offset, not a new load.  Only the weights stream through the ring.  The n tiles of an M tile (stride phases
     // of a data gradient: own weights rows nt*N.., own output placement sub_oy0 / sub_ox0 and valid extent sub_y1 / sub_x1)
     // run back to back on the same tile.
-    int a_halo, halo_w, halo_w0, halo_rows, halo_lo, halo_chunks, halo_same_cols, halo_bo;
+    int a_halo, halo_w, halo_w0, halo_rows, halo_lo, halo_chunks, halo_same_cols;
     int64_t halo_positions;                // B * hp * halo_w
     XbDiv halo_div_w;
     int16_t halo_shift[XB_HALO_MAX_CHUNKS];
@@ -109,7 +109,7 @@ struct ConvParams {
 };
 
 // 16-byte cp.async with zero-fill.  CA = through L1 (sector sharing between the lanes of a request and reuse of the
-// overlapping windows of the raw-pixel first layer: 1080 -> 774 us on B200); otherwise L2 only (better for the wider layers).
+// overlapping windows of the raw-pixel first layer); otherwise L2 only (better for the wider layers).
 template <bool CA>
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, uint32_t src_bytes) {
     if (CA) asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
@@ -124,8 +124,8 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap *tm,
 }
 // one box of a padded-row activation tensor viewed as {channels, pixels, row phase (row mod S), row / S, plane}: row `r` of
 // the tensor is (phase r mod S, index r / S), so a convolution of stride S reads CONSECUTIVE indices of ONE phase - no
-// traversal stride is needed (measured: a 64-byte inner box under the 128-byte swizzle pads every pixel to a 128-byte
-// row, so 32-channel tensors are described as 64-channel pixel pairs instead, see BoxNatureCNN)
+// traversal stride is needed (a 64-byte inner box under the 128-byte swizzle pads every pixel to a 128-byte row, so
+// 32-channel tensors are described as 64-channel pixel pairs instead, see BoxNatureCNN)
 __device__ __forceinline__ void tma_load_box(uint32_t dst, const CUtensorMap *tm, int c, int w, int row, int S, int plane,
                                              uint64_t *bar) {
     const int idx = S == 1 ? row : (row >= 0 ? row / S : -((-row + S - 1) / S));      // floor(row / S)
@@ -133,46 +133,6 @@ __device__ __forceinline__ void tma_load_box(uint32_t dst, const CUtensorMap *tm
     asm volatile(
         "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
         ::"r"(dst), "l"(tm), "r"(c), "r"(w), "r"(ph), "r"(idx), "r"(plane), "r"(smem_u32(bar))
-        : "memory");
-}
-// shared-memory matrix descriptor of a 128-byte-swizzled operand (the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B):
-// K-major:  rows of 64 elements = 128 B, 8-row groups 1024 B apart (SBO), leading offset unused (16 B);
-// MN-major: rows of 64 MN elements = 128 B per K index, 8-K groups 1024 B apart (SBO), 64-element MN blocks LBO apart
-// (cute/atom/mma_traits_sm100.hpp: K  B128 ((8,n),2):((8,SBO),1);  MN B128 ((8,n),(8,k)):((1,LBO),(8,SBO)), 16-byte units)
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-    d |= (uint64_t)1 << 46;                                   // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                                   // layout type SWIZZLE_128B
-    return d;
-}
-// the same for a start address that is NOT a multiple of the 1024-byte swizzle pattern (a window of a larger tile that starts
-// at an arbitrary 128-byte row); with_offset sets the matrix base offset, bits 49-51 = (start address >> 7) & 7 - NOT needed
-// on B200: the swizzle follows the absolute address bits (see xb_gemm_halo_tc)
-__device__ __forceinline__ uint64_t make_desc_sw128_at(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, int with_offset) {
-    uint64_t d = make_desc_sw128(smem_addr, lbo_bytes, sbo_bytes);
-    if (with_offset) d |= (uint64_t)((smem_addr >> 7) & 7u) << 49;
-    return d;
-}
-// tcgen05.mma / tcgen05.commit predicated on `leader` (1 in exactly one lane): the warp stays converged around them
-__device__ __forceinline__ void mma_bf16_if(uint32_t leader, uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "setp.ne.b32 q, %5, 0;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, {%6, %6, %6, %6}, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(leader), "r"(0u)
-        : "memory");
-}
-__device__ __forceinline__ void mma_commit_if(uint32_t leader, uint64_t *bar) {
-    asm volatile(
-        "{\n\t.reg .pred q;\n\t"
-        "setp.ne.b32 q, %1, 0;\n\t"
-        "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}"
-        ::"r"(smem_u32(bar)), "r"(leader)
         : "memory");
 }
 template <int N>
@@ -187,33 +147,46 @@ __device__ __forceinline__ void split3_bf16(float x, __nv_bfloat16 &hi, __nv_bfl
     lo = __float2bfloat16_rn(r1 - __bfloat162float(mid));
 }
 
-// kind::f16 instruction descriptor with both operands MN-major (bits 15 / 16; cute/arch/mma_sm100_desc.hpp)
-__device__ __forceinline__ uint32_t make_idesc_mn(int M, int N) { return make_idesc(M, N) | (1u << 15) | (1u << 16); }
+// A plane x the first PB - pa B planes for one K step: the accumulator blocks pa*NC .. PB*NC-1 (32 columns each).  Block j
+// reads B rows 32 (j - pa*NC) .. +31 of the stage: 4096 bytes per block in every operand layout the kernel uses (128 bytes
+// per row or per MN index).  In-flight wgmmas are ordered on their accumulator registers only when they have the same shape
+// and register set, so every block is always written by the same instruction form: pairs (2i, 2i+1) as one n64 wgmma when
+// NC is even (then every plane's range starts at an even block), single n32 wgmmas when NC is odd.
+template <int T, int PB, int NC, int PA_>
+__device__ __forceinline__ void mma_plane(float (&acc)[PB * NC][16], uint64_t da, uint64_t db, uint32_t scale_d) {
+    constexpr int J0 = PA_ * NC, J1 = PB * NC, STEP = NC % 2 == 0 ? 2 : 1;
+#pragma unroll
+    for (int j = J0; j < J1; j += STEP) {
+        const uint64_t b = db + (uint64_t)(((j - J0) * 4096) >> 4);
+        if (STEP == 2) wgmma_n64<T, T>(acc[j], acc[j + 1 < J1 ? j + 1 : j], da, b, scale_d);
+        else wgmma_n32<T, T>(acc[j], da, b, scale_d);
+    }
+}
 
 // WGRAD = false:  D[site, n]  = sum_k A[site, k] W[n, k]            work item = (128-site tile, n tile),        K-major operands
 // WGRAD = true :  D[kcol, n]  = sum_site A[site, kcol] G[site, n]   work item = (128-kcol tile, n tile, split), MN-major operands
 // PA / PB: bf16 planes of the A / B operand (x = sum of its planes, plane q = bf16 of the residual left by planes < q),
-// PA <= PB.  The products kept are those whose plane indices sum to < PB; they are accumulated in PB SEPARATE float32
-// accumulators D_g, g = pa + pb, which the epilogue adds smallest first: the tensor core truncates (rounds toward zero)
-// when it adds a product block into the accumulator, so keeping the 2^-8 / 2^-16 sized correction terms out of the
-// hi.hi accumulator both shortens its chain of truncating additions by the number of products and keeps the corrections'
-// own truncation error at 2^-8 / 2^-16 of an ulp of the result.  The B planes of a stage are adjacent in shared memory, so
-// in the canonical layouts they ARE one operand of PB*N rows: ONE tcgen05.mma per A plane multiplies it with the first
-// (PB - pa) B planes and lands in the accumulator columns of groups pa .. PB-1 - every A plane is read from shared memory
-// once per K step instead of once per product (shared-memory operand reads, not the tensor pipe, bound N <= 64 tiles).
-template <bool WGRAD, int PA, int PB>
+// PA <= PB.  NC: the tile width N = 32 NC.  The products kept are those whose plane indices sum to < PB; they are accumulated
+// in PB SEPARATE float32 accumulators D_g, g = pa + pb, which the epilogue adds smallest first: the tensor core truncates
+// (rounds toward zero) when it adds a product block into the accumulator, so keeping the 2^-8 / 2^-16 sized correction terms
+// out of the hi.hi accumulator both shortens its chain of truncating additions by the number of products and keeps the
+// corrections' own truncation error at 2^-8 / 2^-16 of an ulp of the result.  The B planes of a stage are adjacent in shared
+// memory, so in the canonical layouts they ARE one operand of PB*N rows: the wgmmas of one A plane multiply it with the
+// first (PB - pa) B planes and land in the accumulator columns of groups pa .. PB-1.
+template <bool WGRAD, int PA, int PB, int NC>
 __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_constant__ ConvParams p) {
-    static_assert(PA >= 1 && PA <= PB && PB <= 3, "plane counts");
+    static_assert(PA >= 1 && PA <= PB && PB <= 3 && PB * NC <= 8, "plane counts / tile width");
+    constexpr int N = 32 * NC;
+    constexpr int TR = WGRAD ? 1 : 0;                 // both operands MN-major in the weight gradient
     extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ __align__(8) uint64_t full_bar[MAX_STAGES], empty_bar[MAX_STAGES], acc_full[2], acc_empty[2], a_full[2], a_empty[2];
-    __shared__ uint32_t tmem_slot;
-    __shared__ float s_bias[256];
-    __shared__ float s_colsum[4][256];                // per epilogue warp: column sums of its 32 rows (ConvParams.colsum)
+    __shared__ __align__(8) uint64_t full_bar[MAX_STAGES], empty_bar[MAX_STAGES], a_full[2], a_empty[2];
+    __shared__ float s_bias[N];
+    __shared__ float s_colsum[CONS_WARPS][N];         // per consumer warp: column sums of its 16 rows (ConvParams.colsum)
     __shared__ XbUnit s_units[XB_CONV_MAX_UNITS];     // per 16-byte K unit: tap offsets + element offset (conv_index.h)
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const XbConvGeom &g = p.g;
-    const int N = g.N, K = g.T * g.C, S = p.stages;
+    const int K = g.T * g.C, S = p.stages;
     const uint32_t a_plane = xb_conv_a_plane_bytes(), w_plane = xb_conv_w_plane_bytes(N);
     const bool halo = !WGRAD && p.a_halo;
     const uint32_t halo_plane = halo ? (((uint32_t)(p.halo_rows * p.halo_w) * 128u + 1023u) & ~1023u) : 0u;   // one plane of a tile
@@ -241,28 +214,18 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
         // a_box: the reduction runs over merged grid rows (p.M of them), box_h rows = box_h * box_w <= 64 sites per chunk
         return p.a_box ? (int)((cnt + p.box_h - 1) / p.box_h) : (int)((cnt + KC - 1) / KC);
     };
-    const uint32_t acc_cols = (uint32_t)(PB * N);           // one accumulator = PB groups of N columns
-    uint32_t tmem_cols = 32;
-    while (tmem_cols < 2 * acc_cols) tmem_cols <<= 1;
 
     if (tid == 0) {
         for (int s = 0; s < S; ++s) {
             // one asynchronous arrival per producer thread (+ the expect_tx arrival of the thread that issues the TMA copies)
-            mbar_init(&full_bar[s], halo ? 1 : PROD_WARPS * 32 + ((p.a_tma || p.b_tma) ? 1 : 0));
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&full_bar[s], halo ? 1 : PROD_THREADS + ((p.a_tma || p.b_tma) ? 1 : 0));
+            mbar_init(&empty_bar[s], CONS_WARPS);
         }
         for (int a = 0; a < 2; ++a) {
-            mbar_init(&acc_full[a], 1);
-            mbar_init(&acc_empty[a], EPI_WARPS);
             mbar_init(&a_full[a], 1);
-            mbar_init(&a_empty[a], 1);
+            mbar_init(&a_empty[a], CONS_WARPS);
         }
         mbar_fence_init();
-    }
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)),
-                     "r"(tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
     }
     if (!p.a_box && !halo)
         for (int i = tid; i < K / 8; i += THREADS) s_units[i] = xb_unit(g, i);
@@ -272,10 +235,7 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
         for (uint32_t i = tid * 16u; i < total; i += THREADS * 16u) *reinterpret_cast<uint4 *>(smem + i) = make_uint4(0, 0, 0, 0);
         fence_proxy_async();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
     const uint32_t smem_base = smem_u32(smem);
     unsigned long long t_wait[3] = {0, 0, 0};
     const unsigned long long t_begin = p.timing ? clock64() : 0ull;
@@ -290,11 +250,11 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
     };
     if ((p.a_tma || p.b_tma) && (smem_base & 1023u)) __trap();     // the 128-byte swizzle pattern repeats every 1024 B
 
-    if (warp > MMA_WARP) {
-        // ------------------------------------------------------------------ producers (256 threads)
-        const int pt = tid - (MMA_WARP + 1) * 32;
+    if (warp >= CONS_WARPS) {
+        // ------------------------------------------------------------------ producers (128 threads)
+        const int ptb = tid - CONS_WARPS * 32;
         uint32_t it = 0, tile_it = 0;
-        if (!(halo && pt != 0))                                // halo: both operands by TMA, one thread drives them
+        if (!(halo && ptb != 0))                               // halo: both operands by TMA, one thread drives them
         for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
           if (halo) {
               // the activation tile of this M tile: one box per plane into the buffer the tile before the last one used
@@ -313,10 +273,10 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
             const int64_t rem = WGRAD ? w - sp * mn_tiles : w;
             const int64_t mt = halo ? w : rem / p.n_tiles;
             const int nt = halo ? sub : (int)(rem - mt * p.n_tiles);
-            XbSite sites[4];                                   // forward: the four rows this thread feeds, fixed for the tile
+            XbSite sites[4];                                   // forward: the four rows this thread feeds (both of its producers)
             if (!WGRAD && !p.a_tma && !halo) {
 #pragma unroll
-                for (int gi = 0; gi < 4; ++gi) sites[gi] = xb_site(g, mt * TILE_M + xb_fwd_row(pt, gi), p.M);
+                for (int gi = 0; gi < 4; ++gi) sites[gi] = xb_site(g, mt * TILE_M + xb_fwd_row(ptb, gi), p.M);
             }
             const int64_t w_off = WGRAD ? 0 : (int64_t)nt * N * K;        // forward: first weight row of this n tile
             const int64_t site_end = WGRAD ? ((sp + 1) * p.sites_per_split < p.M ? (sp + 1) * p.sites_per_split : p.M) : 0;
@@ -340,7 +300,7 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
                     for (int q = 0; q < PB; ++q) cp_async16<false>(wbase + q * w_plane + dst_off, p.w[q] + o, nbytes);
                 };
                 const int64_t site0 = sp * p.sites_per_split + (int64_t)kc * KC;     // weight gradient: first site of the chunk
-                if (pt == 0 && (p.a_tma || p.b_tma)) {
+                if (ptb == 0 && (p.a_tma || p.b_tma)) {
                     // plain-matrix operands: one elected thread arms the barrier with the byte count and issues the tile
                     // copies; every plane of an operand travels in ONE box (planes are the outermost tensor dimension)
                     uint32_t bytes = (p.a_tma ? PA * (p.a_box ? (uint32_t)box_rows * 128u : a_plane) : 0u) + (p.b_tma ? PB * w_plane : 0u);
@@ -383,8 +343,12 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
                     }
                 }
                 if (!halo) {
-                    if (!WGRAD) xb_stage_fwd(g, s_units, pt, sites, kc, emit_a, emit_w);
-                    else xb_stage_wgrad(g, s_units, pt, mt, site0, site_end, p.M, p.w_ld, nt * N, emit_a, emit_w);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int pt = ptb + PROD_THREADS * h;
+                        if (!WGRAD) xb_stage_fwd(g, s_units, pt, sites, kc, emit_a, emit_w);
+                        else xb_stage_wgrad(g, s_units, pt, mt, site0, site_end, p.M, p.w_ld, nt * N, emit_a, emit_w);
+                    }
                     // asynchronous publication: the barrier receives this thread's arrival when the copies issued above have
                     // landed - the producer never waits for its own loads, so up to `stages` chunks of loads are in flight
                     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&full_bar[stage])) : "memory");
@@ -393,241 +357,207 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
             }
           }
         }
-    } else if (warp == MMA_WARP) {
-        // ------------------------------------------------------------------ MMA issue
-        // The whole warp runs the loop on warp-uniform values and only the tcgen05 instructions are predicated on lane 0:
-        // under a divergent `if (lane == 0)` the compiler wraps every tcgen05.mma in a register -> uniform-register broadcast
-        // loop and rebuilds both 64-bit descriptors per instruction (~35 dependent instructions, ~180 clk per MMA measured -
-        // the issuing thread, not the tensor pipe or the loads, bounded every forward launch: tools/k12_timing.py).  Here a
-        // descriptor is a per-launch TEMPLATE (layout, LBO, SBO) plus a start address in 16-byte units: one add per MMA.
-        const uint32_t leader = lane == 0 ? 1u : 0u;
+    } else {
+        // ------------------------------------------------------------------ consumers: wgmma issue + epilogue
         //  A: halo     128-byte swizzle K-major window of the resident tile, K step 32 B, planes halo_plane apart
         //     cp.async no-swizzle canonical layout (conv_index.h), K step = two core matrices = 256 B
         //     TMA      128-byte swizzle.  K-major: rows of 128 B, K step 32 B.  MN-major (weight gradient): two blocks of 64
         //              columns, each [planes][64 sites][128 B]: plane stride a_plane/2, block stride PA*a_plane/2, K step 2048 B
         //  B: the first (PB - pa) planes, adjacent in the stage, are ONE operand of (PB - pa) * N rows (same three layouts;
         //     MN-major: one 64-column block per plane, blocks w_plane apart)
+        // A descriptor = per-launch template (layout, LBO, SBO) + start address in 16-byte units; warpgroup wg reads rows
+        // 64 wg .. 64 wg + 63 of the tile: 8192 bytes further in every layout but the MN-major TMA tile (the next 64-column block)
+        const int wg = warp >> 2;
         uint64_t a_tmpl, b_tmpl;
-        uint32_t a_ks, a_pl, b_ks;                           // steps in 16-byte units: per K step of 16, per A plane
-        if (halo) a_tmpl = make_desc_sw128_at(0, 16, 1024, 0), a_ks = 32 >> 4, a_pl = halo_plane >> 4;
+        uint32_t a_ks, a_pl, b_ks, a_wg;                     // steps in 16-byte units: per K step of 16, per A plane; bytes per warpgroup
+        if (halo) a_tmpl = make_desc_sw128(0, 16, 1024), a_ks = 32 >> 4, a_pl = halo_plane >> 4;
         else if (!p.a_tma) a_tmpl = make_desc(0, KC), a_ks = 256 >> 4, a_pl = a_plane >> 4;
         else if (!WGRAD) a_tmpl = make_desc_sw128(0, 16, 1024), a_ks = 32 >> 4, a_pl = a_plane >> 4;
         else a_tmpl = make_desc_sw128(0, PA * (a_plane / 2), 1024), a_ks = 2048 >> 4, a_pl = (a_plane / 2) >> 4;
+        a_wg = (WGRAD && p.a_tma) ? (uint32_t)wg * PA * (a_plane / 2) : (uint32_t)wg * 8192u;
         if (!p.b_tma) b_tmpl = make_desc(0, KC), b_ks = 256 >> 4;
         else if (!WGRAD) b_tmpl = make_desc_sw128(0, 16, 1024), b_ks = 32 >> 4;
         else b_tmpl = make_desc_sw128(0, w_plane, 1024), b_ks = 2048 >> 4;
-        uint32_t idesc[PA];
-#pragma unroll
-        for (int pa = 0; pa < PA; ++pa) idesc[pa] = WGRAD ? make_idesc_mn(TILE_M, (PB - pa) * N) : make_idesc(TILE_M, (PB - pa) * N);
-        uint32_t it = 0, tcount = 0, tile_it = 0;
+        // this thread's two rows of the tile and the first column of each 8-column block of its fragments
+        const int rbase = 64 * wg + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+        float acc[PB * NC][16];
+        uint32_t it = 0, tile_it = 0;
         for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
           uint32_t halo_base = 0;
           int halo_s0 = 0;
           if (halo) {
               const uint32_t buf = tile_it & 1u;
               timed_wait(&a_full[buf], (tile_it >> 1) & 1u, 2);
-              tc_fence_after();
               halo_base = smem_base + buf * a_buf_bytes;
               halo_s0 = (int)(w * TILE_M) - halo_row_lo(w) * p.halo_w;        // tile row of the site of MMA row 0
           }
           for (int sub = 0; sub < n_inner; ++sub) {
             const int n_chunks = chunks_of(w);
-            const uint32_t a = tcount & 1u;
-            timed_wait(&acc_empty[a], ((tcount >> 1) & 1u) ^ 1u, 1);     // epilogue drained this accumulator
-            tc_fence_after();
-            const uint32_t d_tmem = tmem + a * acc_cols;
-            uint32_t acc = 0;
-            for (int kc = 0; kc < n_chunks; ++kc) {
-                const int stage = (int)(it % (uint32_t)S);
-                timed_wait(&full_bar[stage], (it / (uint32_t)S) & 1u, 0);
-                fence_proxy_async();       // the stage was written by cp.async (generic proxy); the MMA reads it through the async proxy
-                tc_fence_after();
-                const uint32_t base = smem_base + ring_off + (uint32_t)stage * stage_bytes;
-                const uint32_t w_addr = base + (halo ? 0u : PA * a_plane);
-                const uint32_t a_addr = halo ? halo_base + (uint32_t)(halo_s0 + p.halo_shift[sub * p.halo_chunks + kc]) * 128u : base;
-                // start addresses stay below 2^18 bytes: adding 16-byte units to the template never carries out of the field
-                const uint64_t a0 = a_tmpl + (uint64_t)(a_addr >> 4), b0 = b_tmpl + (uint64_t)(w_addr >> 4);
-#pragma unroll
-                for (int ks = 0; ks < KC / 16; ++ks) {
-#pragma unroll
-                    for (int pa = 0; pa < PA; ++pa) {
-                        // A plane pa x B planes 0 .. PB-1-pa -> accumulator groups pa .. PB-1.
-                        // pa = 0 covers every group, so its first instruction of a work item (acc = 0) initialises them all.
-                        mma_bf16_if(leader, d_tmem + (uint32_t)(pa * N), a0 + (uint64_t)(ks * a_ks + pa * a_pl), b0 + (uint64_t)(ks * b_ks),
-                                    idesc[pa], pa == 0 ? acc : 1u);
-                    }
-                    acc = 1;
-                }
-                mma_commit_if(leader, &empty_bar[stage]);     // the stage is free once these MMAs have read it
-                ++it;
-            }
-            mma_commit_if(leader, &acc_full[a]);
-            ++tcount;
-          }
-          if (halo) {
-              mma_commit_if(leader, &a_empty[tile_it & 1u]);         // the tile is free once every MMA issued so far has read it
-              ++tile_it;
-          }
-        }
-        __syncwarp();
-    } else {
-        // ------------------------------------------------------------------ epilogue: thread = row = TMEM lane
-        const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);
-        uint32_t tcount = 0;
-        for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
-          for (int sub = 0; sub < n_inner; ++sub) {
-            const uint32_t a = tcount & 1u;
             const int64_t sp = WGRAD ? w / mn_tiles : 0;
             const int64_t rem = WGRAD ? w - sp * mn_tiles : w;
             const int64_t mt = halo ? w : rem / p.n_tiles;
             const int nt = halo ? sub : (int)(rem - mt * p.n_tiles);
             const int ncol = (halo && p.halo_same_cols) ? 0 : nt;             // column block of the output this item writes
-            bool live;
-            int64_t orow = 0, mrow = 0;                                   // element offsets of the output row / of its mask row
-            if (halo) {
-                const int64_t P = mt * TILE_M + tid;                       // position in the haloed raster
-                const uint32_t R = xb_div((uint32_t)P, p.halo_div_w);      // merged (image, padded row) index
-                const int x = (int)((uint32_t)P - R * (uint32_t)p.halo_w) + p.halo_w0;
-                const int b = (int)xb_div(R, p.box_div_hp), y = (int)(R - (uint32_t)b * (uint32_t)p.box_hp);
-                live = P < p.halo_positions && x >= 0 && x <= p.sub_x1[nt] && y >= p.box_y0 && y <= p.sub_y1[nt];
-                if (live) {
-                    const int64_t orw = (int64_t)b * p.out_H + ((y - p.box_y0) * p.oys + p.sub_oy0[nt]);
-                    const int ox = x * p.oxs + p.sub_ox0[nt];
-                    orow = (orw * p.out_W + ox) * p.out_ld + p.out_c0 + (int64_t)ncol * N;
-                    mrow = (orw * p.mask_W + ox + p.mask_x0) * p.mask_ld + p.mask_c0 + (int64_t)ncol * N;
-                }
-            } else if (!WGRAD && p.a_box) {
-                const int gr = (int)xb_div((uint32_t)tid, p.box_div_w), x = tid - gr * p.box_w;
-                const int64_t R = mt * p.box_h + gr;                       // merged (image, padded row) index
-                const int b = (int)xb_div((uint32_t)R, p.box_div_hp), y = (int)(R - (int64_t)b * p.box_hp);
-                live = tid < box_rows && b < g.B && y >= p.box_y0 && y <= p.box_y1;
-                if (live) {
-                    const int64_t orw = (int64_t)b * p.out_H + ((y - p.box_y0) * p.oys + p.oy0);
-                    const int ox = x * p.oxs + p.ox0;
-                    orow = (orw * p.out_W + ox) * p.out_ld + p.out_c0 + (int64_t)nt * N;
-                    mrow = (orw * p.mask_W + ox + p.mask_x0) * p.mask_ld + p.mask_c0 + (int64_t)nt * N;
-                }
-            } else if (!WGRAD) {
-                const int64_t m = mt * TILE_M + tid;
-                live = m < p.M;
-                if (live) {
-                    int b, y, x;
-                    xb_conv_site(g, m, b, y, x);
-                    const int64_t opix = ((int64_t)b * p.out_H + (y * p.oys + p.oy0)) * p.out_W + (x * p.oxs + p.ox0);
-                    orow = opix * p.out_ld + p.out_c0 + (int64_t)nt * N;
-                    mrow = opix * p.mask_ld + p.mask_c0 + (int64_t)nt * N;
-                }
-            } else {
-                const int64_t kcol = mt * TILE_M + tid;
-                live = kcol < K;
-                orow = ((sp * K + kcol) * p.n_tiles + nt) * (int64_t)N;       // partials [splits, K, N_total]
-            }
             if (!WGRAD) {
-                // the bias slice of this n tile (only the epilogue warps read / write s_bias; named barrier 1, 128 threads)
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                for (int i = tid; i < N; i += EPI_WARPS * 32) s_bias[i] = p.bias ? p.bias[ncol * N + i] : 0.f;
-                asm volatile("bar.sync 1, 128;" ::: "memory");
+                // the bias slice of this n tile (only the consumer warps read / write s_bias; named barrier 1)
+                asm volatile("bar.sync 1, %0;" ::"n"(CONS_WARPS * 32) : "memory");
+                for (int i = tid; i < N; i += CONS_WARPS * 32) s_bias[i] = p.bias ? p.bias[ncol * N + i] : 0.f;
             }
-            timed_wait(&acc_full[a], (tcount >> 1) & 1u, 0);
-            tc_fence_after();
-            for (int c0 = 0; c0 < N; c0 += 32) {
-                float v[32];
-                tmem_ld32(lane_addr + a * acc_cols + (uint32_t)((PB - 1) * N + c0), v);      // smallest group first
+            uint32_t scale_d = 0;
+            int prev_stage = -1;
+            for (int kc = 0; kc < n_chunks; ++kc) {
+                const int stage = (int)(it % (uint32_t)S);
+                timed_wait(&full_bar[stage], (it / (uint32_t)S) & 1u, 0);
+                fence_proxy_async();       // the stage was written by cp.async (generic proxy); the MMA reads it through the async proxy
+                const uint32_t base = smem_base + ring_off + (uint32_t)stage * stage_bytes;
+                const uint32_t w_addr = base + (halo ? 0u : PA * a_plane);
+                const uint32_t a_addr = a_wg + (halo ? halo_base + (uint32_t)(halo_s0 + p.halo_shift[sub * p.halo_chunks + kc]) * 128u : base);
+                // start addresses stay below 2^18 bytes: adding 16-byte units to the template never carries out of the field
+                const uint64_t a0 = a_tmpl + (uint64_t)(a_addr >> 4), b0 = b_tmpl + (uint64_t)(w_addr >> 4);
+                wgmma_fence();
 #pragma unroll
-                for (int gq = PB - 2; gq >= 0; --gq) {
-                    float u[32];
-                    tmem_ld32(lane_addr + a * acc_cols + (uint32_t)(gq * N + c0), u);
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] += u[j];
+                for (int ks = 0; ks < KC / 16; ++ks) {
+                    // A plane pa x B planes 0 .. PB-1-pa -> accumulator groups pa .. PB-1.
+                    // pa = 0 covers every group, so its first instruction of a work item (scale_d = 0) initialises them all.
+                    const uint64_t da = a0 + (uint64_t)(ks * a_ks), db = b0 + (uint64_t)(ks * b_ks);
+                    mma_plane<TR, PB, NC, 0>(acc, da, db, scale_d);
+                    if (PA > 1) mma_plane<TR, PB, NC, (PA > 1 ? 1 : 0)>(acc, da + a_pl, db, 1u);
+                    if (PA > 2) mma_plane<TR, PB, NC, (PA > 2 ? 2 : 0)>(acc, da + 2 * a_pl, db, 1u);
+                    scale_d = 1;
                 }
-                if (!WGRAD) {
+                wgmma_commit();
+                // the group before this one has retired: its stage is free
+                wgmma_wait<1>();
+                if (prev_stage >= 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+                }
+                prev_stage = stage;
+                ++it;
+            }
+            wgmma_wait<0>();
+            if (prev_stage >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+            }
+            if (!WGRAD) asm volatile("bar.sync 1, %0;" ::"n"(CONS_WARPS * 32) : "memory");     // s_bias written
+            // ---- epilogue on the fragments: rows rbase (h = 0) and rbase + 8 (h = 1)
+            bool live[2];
+            int64_t orow[2] = {0, 0}, mrow[2] = {0, 0};                       // element offsets of the output row / of its mask row
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        v[j] += s_bias[c0 + j];
-                        if (p.relu) v[j] = fmaxf(v[j], 0.f);
+            for (int h = 0; h < 2; ++h) {
+                const int r = rbase + 8 * h;
+                if (halo) {
+                    const int64_t P = mt * TILE_M + r;                         // position in the haloed raster
+                    const uint32_t R = xb_div((uint32_t)P, p.halo_div_w);      // merged (image, padded row) index
+                    const int x = (int)((uint32_t)P - R * (uint32_t)p.halo_w) + p.halo_w0;
+                    const int b = (int)xb_div(R, p.box_div_hp), y = (int)(R - (uint32_t)b * (uint32_t)p.box_hp);
+                    live[h] = P < p.halo_positions && x >= 0 && x <= p.sub_x1[nt] && y >= p.box_y0 && y <= p.sub_y1[nt];
+                    if (live[h]) {
+                        const int64_t orw = (int64_t)b * p.out_H + ((y - p.box_y0) * p.oys + p.sub_oy0[nt]);
+                        const int ox = x * p.oxs + p.sub_ox0[nt];
+                        orow[h] = (orw * p.out_W + ox) * p.out_ld + p.out_c0 + (int64_t)ncol * N;
+                        mrow[h] = (orw * p.mask_W + ox + p.mask_x0) * p.mask_ld + p.mask_c0 + (int64_t)ncol * N;
                     }
+                } else if (!WGRAD && p.a_box) {
+                    const int gr = (int)xb_div((uint32_t)r, p.box_div_w), x = r - gr * p.box_w;
+                    const int64_t R = mt * p.box_h + gr;                       // merged (image, padded row) index
+                    const int b = (int)xb_div((uint32_t)R, p.box_div_hp), y = (int)(R - (int64_t)b * p.box_hp);
+                    live[h] = r < box_rows && b < g.B && y >= p.box_y0 && y <= p.box_y1;
+                    if (live[h]) {
+                        const int64_t orw = (int64_t)b * p.out_H + ((y - p.box_y0) * p.oys + p.oy0);
+                        const int ox = x * p.oxs + p.ox0;
+                        orow[h] = (orw * p.out_W + ox) * p.out_ld + p.out_c0 + (int64_t)nt * N;
+                        mrow[h] = (orw * p.mask_W + ox + p.mask_x0) * p.mask_ld + p.mask_c0 + (int64_t)nt * N;
+                    }
+                } else if (!WGRAD) {
+                    const int64_t m = mt * TILE_M + r;
+                    live[h] = m < p.M;
+                    if (live[h]) {
+                        int b, y, x;
+                        xb_conv_site(g, m, b, y, x);
+                        const int64_t opix = ((int64_t)b * p.out_H + (y * p.oys + p.oy0)) * p.out_W + (x * p.oxs + p.ox0);
+                        orow[h] = opix * p.out_ld + p.out_c0 + (int64_t)nt * N;
+                        mrow[h] = opix * p.mask_ld + p.mask_c0 + (int64_t)nt * N;
+                    }
+                } else {
+                    const int64_t kcol = mt * TILE_M + r;
+                    live[h] = kcol < K;
+                    orow[h] = ((sp * K + kcol) * p.n_tiles + nt) * (int64_t)N;       // partials [splits, K, N_total]
                 }
-                if (!WGRAD && p.mask && live) {
-                    const uint4 *mk = reinterpret_cast<const uint4 *>(p.mask + mrow + c0);
+            }
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const uint4 q = mk[j];
-                        const uint32_t ws[4] = {q.x, q.y, q.z, q.w};
+            for (int cc = 0; cc < NC; ++cc) {
 #pragma unroll
-                        for (int i = 0; i < 4; ++i) {
+                for (int i = 0; i < 4; ++i) {
+                    const int c = 32 * cc + 8 * i + cq;                        // columns c, c + 1
+                    float cs[2] = {0.f, 0.f};
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        float v[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            v[e] = acc[(PB - 1) * NC + cc][4 * i + 2 * h + e];     // smallest group first
+#pragma unroll
+                            for (int gq = PB - 2; gq >= 0; --gq) v[e] += acc[gq * NC + cc][4 * i + 2 * h + e];
+                            if (!WGRAD) {
+                                v[e] += s_bias[c + e];
+                                if (p.relu) v[e] = fmaxf(v[e], 0.f);
+                            }
+                        }
+                        if (!WGRAD && p.mask && live[h]) {
                             // bf16 > 0  <=>  sign bit clear and not (+)zero
-                            const uint32_t lo16 = ws[i] & 0xffffu, hi16 = ws[i] >> 16;
-                            if (!(lo16 != 0u && lo16 < 0x8000u)) v[8 * j + 2 * i] = 0.f;
-                            if (!(hi16 != 0u && hi16 < 0x8000u)) v[8 * j + 2 * i + 1] = 0.f;
+                            const uint32_t mw = *reinterpret_cast<const uint32_t *>(p.mask + mrow[h] + c);
+                            const uint32_t lo16 = mw & 0xffffu, hi16 = mw >> 16;
+                            if (!(lo16 != 0u && lo16 < 0x8000u)) v[0] = 0.f;
+                            if (!(hi16 != 0u && hi16 < 0x8000u)) v[1] = 0.f;
+                        }
+                        if (live[h]) {
+                            if (p.out_f32) *reinterpret_cast<float2 *>(p.out_f32 + orow[h] + c) = make_float2(v[0], v[1]);
+                            if (!WGRAD && p.p_out > 0) {
+                                __nv_bfloat16 q0[3], q1[3];
+                                split3_bf16(v[0], q0[0], q0[1], q0[2]);
+                                split3_bf16(v[1], q1[0], q1[1], q1[2]);
+#pragma unroll
+                                for (int q = 0; q < 3; ++q)
+                                    if (q < p.p_out) *reinterpret_cast<uint32_t *>(p.out[q] + orow[h] + c) = pack2(q0[q], q1[q]);
+                            }
+                            cs[0] += v[0], cs[1] += v[1];
                         }
                     }
-                }
-                if (live) {
-                    if (p.out_f32) {
-                        float4 *o = reinterpret_cast<float4 *>(p.out_f32 + orow + c0);
+                    if (!WGRAD && p.colsum) {
+                        // column sums over the warp's 16 rows: the 8 lanes that share (lane & 3) hold the same columns
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) o[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                    }
-                    if (!WGRAD && p.p_out > 0) {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            __nv_bfloat16 h[3][8];
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) split3_bf16(v[8 * j + i], h[0][i], h[1][i], h[2][i]);
-#pragma unroll
-                            for (int q = 0; q < 3; ++q)
-                                if (q < p.p_out)
-                                    reinterpret_cast<uint4 *>(p.out[q] + orow + c0)[j] =
-                                        make_uint4(pack2(h[q][0], h[q][1]), pack2(h[q][2], h[q][3]), pack2(h[q][4], h[q][5]),
-                                                   pack2(h[q][6], h[q][7]));
+                        for (int off = 4; off <= 16; off <<= 1) {
+                            cs[0] += __shfl_xor_sync(0xffffffffu, cs[0], off);
+                            cs[1] += __shfl_xor_sync(0xffffffffu, cs[1], off);
                         }
+                        if (lane < 4) s_colsum[warp][c] = cs[0], s_colsum[warp][c + 1] = cs[1];
                     }
-                }
-                if (!WGRAD && p.colsum) {
-                    // column sums over this warp's 32 rows by a transposing butterfly: after the step with offset `off` a lane
-                    // keeps the half of its columns selected by that bit of its index, so lane j ends with column c0 + j
-                    if (!live) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) v[j] = 0.f;
-                    }
-#pragma unroll
-                    for (int off = 16; off >= 1; off >>= 1) {
-                        const bool upper = (lane & off) != 0;
-#pragma unroll
-                        for (int i = 0; i < off; ++i) {
-                            const float send = upper ? v[i] : v[i + off];
-                            const float keep = upper ? v[i + off] : v[i];
-                            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-                        }
-                    }
-                    s_colsum[tid >> 5][c0 + lane] = v[0];
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[a]);
             if (!WGRAD && p.colsum) {
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                for (int i = tid; i < N; i += EPI_WARPS * 32)            // fixed order: deterministic
-                    p.colsum[(mt * p.n_tiles + nt) * (int64_t)N + i] =
-                        ((s_colsum[0][i] + s_colsum[1][i]) + s_colsum[2][i]) + s_colsum[3][i];
+                asm volatile("bar.sync 1, %0;" ::"n"(CONS_WARPS * 32) : "memory");
+                for (int i = tid; i < N; i += CONS_WARPS * 32) {          // fixed order: deterministic
+                    float s = s_colsum[0][i];
+#pragma unroll
+                    for (int q = 1; q < CONS_WARPS; ++q) s += s_colsum[q][i];
+                    p.colsum[(mt * p.n_tiles + nt) * (int64_t)N + i] = s;
+                }
             }
-            ++tcount;
+          }
+          if (halo) {
+              __syncwarp();                                   // every MMA of this tile has retired (wait above)
+              if (lane == 0) mbar_arrive(&a_empty[tile_it & 1u]);
+              ++tile_it;
           }
         }
     }
     if (p.timing && blockIdx.x < 160) {
         const unsigned long long tot = clock64() - t_begin;
         unsigned long long *o = xb_k12_timing[blockIdx.x];
-        if (warp == MMA_WARP && lane == 0) o[0] = tot, o[1] = t_wait[0], o[2] = t_wait[1], o[3] = t_wait[2];
-        if (warp == MMA_WARP + 1 && lane == 0) o[4] = tot, o[5] = t_wait[0], o[6] = t_wait[1];
-        if (tid == 0) o[7] = tot, o[8] = t_wait[0];
-    }
-    // ---- teardown
-    tc_fence_before();
-    __syncthreads();
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tmem_cols));
+        if (tid == 0) o[0] = tot, o[1] = t_wait[0], o[3] = t_wait[2];
+        if (warp == CONS_WARPS && lane == 0) o[4] = tot, o[5] = t_wait[0], o[6] = t_wait[1];
     }
 }
 
@@ -755,7 +685,7 @@ struct PackJobs {
     int n;
 };
 // [N, C, HW] <-> [N, (hw, c)] is a C x HW transpose per n with strides of HW elements: element-wise it touches one 32-byte
-// sector per 4-byte value on one side (69 us to pack, 109 us to reduce the 512 x 6400 layer on B200).  Tiles through shared
+// sector per 4-byte value on one side (the 512 x 6400 Linear layer is the case that matters).  Tiles through shared
 // memory make both sides coalesced: mode 0 one n (C*HW values) per block; mode 1 / the weight-gradient reduction a tile of
 // 32 n x 2 c x HW values (rows of 32 n on the (hw, c)-major side, runs of HW on torch's side).
 constexpr int PACK_TILE_MAX = 8192;        // floats of shared memory per block
@@ -904,7 +834,7 @@ int fill_params(ConvParams &p, int pa, int pb, const void *in, int64_t in_plane,
     if (!in || !w || !dy || !dx) return XB_EINVAL;
     if (B <= 0 || IH <= 0 || IW <= 0 || OY <= 0 || OX <= 0 || sy <= 0 || sx <= 0 || T <= 0 || N <= 0 || n_tile <= 0)
         return XB_EINVAL;
-    // one tcgen05.mma spans pb * n_tile columns (<= 256, a multiple of 16); two accumulators of pb * n_tile columns in TMEM
+    // the register accumulators of one consumer thread: pb * n_tile / 2 floats (pb * n_tile <= 256, n_tile a multiple of 32)
     if (T > XB_CONV_MAX_TAPS || n_tile % 32 != 0 || N % n_tile != 0 || pb * n_tile > 256 || C % 8 != 0) return XB_ERANGE;
     if ((int64_t)T * C > 8 * XB_CONV_MAX_UNITS || (int64_t)B * OY * OX >= (int64_t)1 << 31) return XB_ERANGE;   // tap table, 32-bit sites
     if (!xb_aligned(in, 16) || !xb_aligned(w, 16) || in_plane % 8 != 0 || w_plane % 8 != 0) return XB_EALIGN;
@@ -934,27 +864,38 @@ int fill_params(ConvParams &p, int pa, int pb, const void *in, int64_t in_plane,
     return XB_OK;
 }
 
-template <bool WGRAD, int PA, int PB>
+template <bool WGRAD, int PA, int PB, int NC>
 int launch_pp(const ConvParams &p, int64_t work, void *stream) {
     static bool attr = false;
     if (!attr) {
-        cudaFuncSetAttribute(conv_tc_kernel<WGRAD, PA, PB>, cudaFuncAttributeMaxDynamicSharedMemorySize, XB_K12_MAX_DYN_SMEM);
+        cudaFuncSetAttribute(conv_tc_kernel<WGRAD, PA, PB, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, XB_K12_MAX_DYN_SMEM);
         attr = true;
     }
     const int grid = (int)(work < xb_sm_count() ? work : xb_sm_count());
     const size_t smem = p.dyn_smem ? p.dyn_smem : (size_t)p.stages * (PA * xb_conv_a_plane_bytes() + PB * xb_conv_w_plane_bytes(p.g.N));
-    conv_tc_kernel<WGRAD, PA, PB><<<grid, THREADS, smem, (cudaStream_t)stream>>>(p);
+    conv_tc_kernel<WGRAD, PA, PB, NC><<<grid, THREADS, smem, (cudaStream_t)stream>>>(p);
     return xb_launch_status();
+}
+
+// the tile width N = 32 NC is a template parameter: the accumulators are registers (PB * NC blocks of 32 columns, at most 8)
+template <bool WGRAD, int PA, int PB, int NC = 1>
+int launch_n(const ConvParams &p, int64_t work, void *stream) {
+    if constexpr (PB * NC > 8) {
+        return XB_ERANGE;
+    } else {
+        if (p.g.N == 32 * NC) return launch_pp<WGRAD, PA, PB, NC>(p, work, stream);
+        return launch_n<WGRAD, PA, PB, NC + 1>(p, work, stream);
+    }
 }
 
 template <bool WGRAD>
 int launch(int pa, int pb, const ConvParams &p, int64_t work, void *stream) {
-    if (pa == 1 && pb == 1) return launch_pp<WGRAD, 1, 1>(p, work, stream);
-    if (pa == 1 && pb == 2) return launch_pp<WGRAD, 1, 2>(p, work, stream);
-    if (pa == 1 && pb == 3) return launch_pp<WGRAD, 1, 3>(p, work, stream);
-    if (pa == 2 && pb == 2) return launch_pp<WGRAD, 2, 2>(p, work, stream);
-    if (pa == 2 && pb == 3) return launch_pp<WGRAD, 2, 3>(p, work, stream);
-    if (pa == 3 && pb == 3) return launch_pp<WGRAD, 3, 3>(p, work, stream);
+    if (pa == 1 && pb == 1) return launch_n<WGRAD, 1, 1>(p, work, stream);
+    if (pa == 1 && pb == 2) return launch_n<WGRAD, 1, 2>(p, work, stream);
+    if (pa == 1 && pb == 3) return launch_n<WGRAD, 1, 3>(p, work, stream);
+    if (pa == 2 && pb == 2) return launch_n<WGRAD, 2, 2>(p, work, stream);
+    if (pa == 2 && pb == 3) return launch_n<WGRAD, 2, 3>(p, work, stream);
+    if (pa == 3 && pb == 3) return launch_n<WGRAD, 3, 3>(p, work, stream);
     return XB_EINVAL;
 }
 
@@ -1163,11 +1104,8 @@ extern "C" int xb_gemm_halo_tc(int planes_a, int planes_b, const void *in, int64
     p.a_halo = 1, p.b_tma = 1;
     p.halo_w = halo_w, p.halo_w0 = halo_w0, p.halo_rows = halo_rows, p.halo_lo = lo, p.halo_chunks = n_chunks;
     p.halo_same_cols = same_cols ? 1 : 0;
-    // measured on B200 (tests/test_gpu_tc_conv.py, halo test): the 128-byte swizzle of a descriptor whose start is an
-    // arbitrary 128-byte row of a 1024-byte-aligned tile is a function of the ABSOLUTE shared-memory address, exactly as TMA
-    // wrote it - the matrix-base-offset field must stay 0 (XB_K12_HALO_BO=1 sets it to (addr >> 7) & 7: wrong results)
-    const char *bo = getenv("XB_K12_HALO_BO");
-    p.halo_bo = bo ? atoi(bo) : 0;
+    // the 128-byte swizzle of a descriptor whose start is an arbitrary 128-byte row of a 1024-byte-aligned tile is a function
+    // of the ABSOLUTE shared-memory address, exactly as TMA wrote it: the descriptors leave the matrix-base-offset field 0
     p.halo_positions = (int64_t)B * hp * halo_w;
     if (p.halo_positions + 4 * halo_w + TILE_M >= ((int64_t)1 << 31)) return XB_ERANGE;
     p.halo_div_w = xb_div_make((uint32_t)halo_w);

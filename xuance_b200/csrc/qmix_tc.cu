@@ -1,18 +1,19 @@
-// K9-TC: the QMIX mixing network forward as ONE tensor-core kernel (tcgen05.mma, accumulators in TMEM).
+// K9-TC: the QMIX mixing network forward as ONE tensor-core kernel (wgmma, accumulators in registers).
 //
 //   Z      = X[rows x S] . W1cat^T[S x 128]              (first layers of hyper_w_1 | hyper_b_1 | hyper_w_2 | hyper_b_2)
 //   W1raw  = relu(Z[:,  0: 32] + c) . Wb1^T [32 x n*32]  (second layer of hyper_w_1)
 //   W2raw  = relu(Z[:, 64: 96] + c) . Wb2^T [32 x 32]    (second layer of hyper_w_2)
 //   b2     = relu(Z[:, 96:128] + c) . wb2^T [32 x 1]     (second layer of hyper_b_2)
 //   q_tot  = elu(q . |W1raw + c| + (Z[:,32:64] + c)) . |W2raw + c| + b2 + c         per row
-// (xuance/torch/rl_models/heads/q_mix_head.py:52-95).  One CTA (128 threads) owns a tile of 128 rows: M = 128,
-// thread i <-> TMEM lane i <-> row i.  All GEMM operands sit in shared memory in the K-major no-swizzle canonical
+// (xuance/torch/rl_models/heads/q_mix_head.py:52-95).  One CTA (two warpgroups) owns a tile of 128 rows, each
+// warpgroup 64 of them (M = 64 per wgmma); the epilogues work on the accumulator fragments (tc_common.cuh).  All GEMM
+// operands sit in shared memory in the K-major no-swizzle canonical
 // layout (8-row x 16-byte core matrices), written by the threads themselves; the weights are staged once per CTA,
 // the CTA then loops over its tiles (persistent grid = SM count).
 //
 // Numerics: the reference computes these layers in fp32.  The tensor pipe takes bf16 here, so every fp32 operand is
 // split x = hi + lo (two bf16 values, |x - hi - lo| <= 2^-16 |x|) and each product is the sum of the three MMAs
-// hi.hi + hi.lo + lo.hi (lo.lo <= 2^-16 relative, the size of the split residual itself) accumulated in fp32 in TMEM: relative error ~1e-5 per layer (a plain bf16 or TF32
+// hi.hi + hi.lo + lo.hi (lo.lo <= 2^-16 relative, the size of the split residual itself) accumulated in fp32: relative error ~1e-5 per layer (a plain bf16 or TF32
 // pass would be ~4e-3 / ~5e-4).  tests/test_gpu_qmix.py pins it against the fp32 oracle.
 #include "tc_common.cuh"
 
@@ -22,8 +23,7 @@ using namespace xbtc;
 constexpr int TC_ROWS = 128;   // M
 constexpr int TC_HH = 32;      // hypernet hidden = mixing hidden = 32 (the shipped QMIX configs)
 constexpr int TC_N1 = 128;     // 4 x 32 first-layer outputs
-constexpr int TC_TMEM_COLS = 512;
-constexpr int COL_Z = 0, COL_W1 = 128, COL_W2 = 384, COL_B2 = 416;   // W1raw may take up to 256 columns (n <= 8)
+constexpr int TC_THREADS = 256;  // two warpgroups, 64 rows each
 
 // stage a [rows x K] fp32 row-major matrix (leading dimension ld; global OR shared memory) as hi/lo bf16 canonical
 // operands, zero padded; one thread-iteration = 8 consecutive k of one row (two 16-byte shared-memory stores);
@@ -54,23 +54,6 @@ __device__ __forceinline__ void stage_operand(const float *__restrict__ g, int r
     }
 }
 
-// issue the three split products of one GEMM: D[128 x N] (+)= A[128 x KP] . B[N x KP]^T
-__device__ __forceinline__ void issue_gemm(uint32_t d_tmem, const uint8_t *a_hi, const uint8_t *a_lo,
-                                           const uint8_t *b_hi, const uint8_t *b_lo, int KP, int N) {
-    const uint32_t idesc = make_idesc(TC_ROWS, N);
-    const uint8_t *as[2] = {a_hi, a_lo};
-    const uint8_t *bs[2] = {b_hi, b_lo};
-    uint32_t acc = 0;
-    for (int pa = 0; pa < 2; ++pa)
-        for (int pb = 0; pb < 2 - pa; ++pb)   // (hi,hi) (hi,lo) (lo,hi); lo.lo <= 2^-16 relative is dropped
-            for (int ks = 0; ks < KP / 16; ++ks) {  // one MMA = K 16 = two core matrices = 256 B along K
-                const uint64_t da = make_desc(smem_u32(as[pa]) + ks * 256, KP);
-                const uint64_t db = make_desc(smem_u32(bs[pb]) + ks * 256, KP);
-                mma_bf16(d_tmem, da, db, idesc, acc);
-                acc = 1;
-            }
-}
-
 struct TcParams {
     const float *states, *q;                 // [R,S], [R,n]
     const float *w_l1[4], *b_l1[4];          // first layers of hyper_w_1 | hyper_b_1 | hyper_w_2 | hyper_b_2: [32,S], [32]
@@ -82,13 +65,13 @@ struct TcParams {
     int S, n;
 };
 
-__global__ void __launch_bounds__(128, 1) qmix_mix_tc_kernel(TcParams p) {
+__global__ void __launch_bounds__(TC_THREADS, 1) qmix_mix_tc_kernel(TcParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ __align__(8) uint64_t mma_bar, x_bar;
-    __shared__ uint32_t tmem_base_slot;
+    __shared__ __align__(8) uint64_t x_bar;
     __shared__ float s_bias1[TC_N1], s_bias_wb1[256], s_bias_wb2[TC_HH], s_bias_b2;
 
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int wg = warp >> 2;                                         // warpgroup: rows 64 wg .. 64 wg + 63 of a tile
     const int S = p.S, n = p.n, KP1 = (S + 15) & ~15, N2A = n * TC_HH;
     // ---- shared memory carve-up (every operand base 128-B aligned)
     const int szA1 = TC_ROWS * KP1 * 2, szB1 = TC_N1 * KP1 * 2, szA2 = TC_ROWS * TC_HH * 2;
@@ -103,7 +86,7 @@ __global__ void __launch_bounds__(128, 1) qmix_mix_tc_kernel(TcParams p) {
     uint8_t *B2ah = B1l + szB1, *B2al = B2ah + szB2a, *B2bh = B2al + szB2a, *B2bl = B2bh + szB2b;
     uint8_t *B2ch = B2bl + szB2b, *B2cl = B2ch + szB2c;
     float *Xraw = reinterpret_cast<float *>(B2cl + szB2c);   // [128 x S] fp32: the NEXT tile, fetched by the TMA unit
-    // ---- one-time setup: mbarrier, TMEM, weights
+    // ---- one-time setup: mbarrier, weights
     const int64_t n_tiles = (p.R + TC_ROWS - 1) / TC_ROWS;
     // a tile is one contiguous run of rows_valid*S*4 bytes; the bulk copy needs a multiple of 16 bytes
     auto tile_copy_bytes = [&](int64_t t) -> uint32_t {
@@ -111,19 +94,12 @@ __global__ void __launch_bounds__(128, 1) qmix_mix_tc_kernel(TcParams p) {
         return (uint32_t)(rows * S * 4);
     };
     if (tid == 0) {
-        mbar_init(&mma_bar, 1);
         mbar_init(&x_bar, 1);
         mbar_fence_init();
         if ((int64_t)blockIdx.x < n_tiles && (tile_copy_bytes(blockIdx.x) & 15) == 0) {   // prefetch the first tile
             mbar_expect_tx(&x_bar, tile_copy_bytes(blockIdx.x));
             bulk_g2s(Xraw, p.states + (int64_t)blockIdx.x * TC_ROWS * S, tile_copy_bytes(blockIdx.x), &x_bar);
         }
-    }
-    __syncwarp();
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)),
-                     "r"(TC_TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
     }
     for (int blk = 0; blk < 4; ++blk)   // rows 32*blk .. 32*blk+31 of the concatenated first-layer weight
         stage_operand(p.w_l1[blk], TC_HH, TC_HH, S, S, KP1, B1h + (size_t)blk * (TC_HH / 8) * (KP1 / 8) * 128,
@@ -135,20 +111,22 @@ __global__ void __launch_bounds__(128, 1) qmix_mix_tc_kernel(TcParams p) {
     for (int i = tid; i < N2A; i += blockDim.x) s_bias_wb1[i] = p.bias_wb1[i];
     if (tid < TC_HH) s_bias_wb2[tid] = p.bias_wb2[tid];
     if (tid == 0) s_bias_b2 = p.bias_wb2c[0];
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_slot;
-    const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);   // this warp's 32 TMEM lanes
-    uint32_t phase = 0, xphase = 0;
+    uint32_t xphase = 0;
+    // this thread's rows (tile-relative) and first column of every 8-column block of a fragment
+    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+    // A operands: this warpgroup's 64 rows; B operands: row offsets of 8-row groups (KP * 2 bytes per row)
+    const uint32_t a1h = smem_u32(A1h) + (uint32_t)(64 * wg * KP1 * 2), a1l = smem_u32(A1l) + (uint32_t)(64 * wg * KP1 * 2);
 
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int64_t row0 = tile * TC_ROWS;
         const int rows_valid = (int)((p.R - row0) < TC_ROWS ? (p.R - row0) : TC_ROWS);
-        // ---- this row's agent utilities (latency hidden behind the staging + first GEMM)
-        float qv[8];
+        // ---- the agent utilities of this thread's two rows (latency hidden behind the staging + first GEMM)
+        float qv[2][8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) qv[i] = (i < n && tid < rows_valid) ? p.q[(row0 + tid) * n + i] : 0.f;
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < 8; ++i) qv[h][i] = (i < n && r0 + 8 * h < rows_valid) ? p.q[(row0 + r0 + 8 * h) * n + i] : 0.f;
         // ---- stage X tile (split to bf16 hi/lo) from the prefetched raw copy (or from global for an unaligned tail)
         if ((tile_copy_bytes(tile) & 15) == 0) {
             mbar_wait(&x_bar, xphase);
@@ -158,12 +136,8 @@ __global__ void __launch_bounds__(128, 1) qmix_mix_tc_kernel(TcParams p) {
             stage_operand(p.states + row0 * S, rows_valid, TC_ROWS, S, S, KP1, A1h, A1l);
         }
         fence_proxy_async();   // generic-proxy smem writes -> visible to the tensor core (async proxy)
-        tc_fence_before();
-        __syncthreads();       // also orders the previous tile's TMEM reads before this tile's MMAs
-        tc_fence_after();
+        __syncthreads();       // the whole X tile is staged (and Xraw consumed) before GEMM1 and the next prefetch
         if (tid == 0) {
-            issue_gemm(tmem + COL_Z, A1h, A1l, B1h, B1l, KP1, TC_N1);
-            mma_commit(&mma_bar);
             // Xraw was consumed by every thread (barrier above): fetch the next tile while this one computes
             const int64_t nt = tile + gridDim.x;
             if (nt < n_tiles && (tile_copy_bytes(nt) & 15) == 0) {
@@ -171,72 +145,103 @@ __global__ void __launch_bounds__(128, 1) qmix_mix_tc_kernel(TcParams p) {
                 bulk_g2s(Xraw, p.states + nt * TC_ROWS * S, tile_copy_bytes(nt), &x_bar);
             }
         }
-        mbar_wait(&mma_bar, phase);
-        phase ^= 1;
-        tc_fence_after();
-        // ---- layer-1 epilogue: thread = row.  relu(Z + bias) of the three hidden blocks -> GEMM2 A operands
-        float b1v[TC_HH];
+        // ---- GEMM1: Z[64 x 128] per warpgroup, products (hi,hi) (hi,lo) (lo,hi); lo.lo <= 2^-16 relative is dropped
+        float z[4][16];
+        wgmma_fence();
         {
-            float z[32];
-            const int blocks[3] = {0, 64, 96};
+            const uint32_t as[2] = {a1h, a1l}, bs[2] = {smem_u32(B1h), smem_u32(B1l)};
+            uint32_t acc = 0;
+            for (int pa = 0; pa < 2; ++pa)
+                for (int pb = 0; pb < 2 - pa; ++pb)
+                    for (int ks = 0; ks < KP1 / 16; ++ks) {   // one MMA = K 16 = two core matrices = 256 B along K
+                        const uint64_t da = make_desc(as[pa] + ks * 256, KP1);
+                        wgmma_n64<0, 0>(z[0], z[1], da, make_desc(bs[pb] + ks * 256, KP1), acc);
+                        wgmma_n64<0, 0>(z[2], z[3], da, make_desc(bs[pb] + 64 * KP1 * 2 + ks * 256, KP1), acc);
+                        acc = 1;
+                    }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncthreads();       // both warpgroups are done reading A1: the A2 operands overwrite it
+        // ---- layer-1 epilogue: relu(Z + bias) of the three hidden blocks -> GEMM2 A operands; b1v = Z[:, 32:64] + bias
+        float b1v[16];
+        {
+            const int blocks[3] = {0, 2, 3};
 #pragma unroll
-            for (int g = 0; g < 3; ++g) {
-                tmem_ld32(lane_addr + COL_Z + blocks[g], z);
+            for (int gi = 0; gi < 3; ++gi)
 #pragma unroll
-                for (int k0 = 0; k0 < 32; k0 += 8) {
-                    float x[8];
+                for (int i = 0; i < 4; ++i)
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) x[i] = fmaxf(z[k0 + i] + s_bias1[blocks[g] + k0 + i], 0.f);
-                    store_unit(x, tid, k0, TC_HH, A2h[g], A2l[g]);
-                }
-            }
-            tmem_ld32(lane_addr + COL_Z + 32, z);
+                    for (int h = 0; h < 2; ++h) {
+                        const int c = 8 * i + cq, bc = 32 * blocks[gi] + c;
+                        store_pair(fmaxf(z[blocks[gi]][4 * i + 2 * h] + s_bias1[bc], 0.f),
+                                   fmaxf(z[blocks[gi]][4 * i + 2 * h + 1] + s_bias1[bc + 1], 0.f), r0 + 8 * h, c, TC_HH, A2h[gi],
+                                   A2l[gi]);
+                    }
 #pragma unroll
-            for (int k = 0; k < 32; ++k) b1v[k] = z[k] + s_bias1[32 + k];
+            for (int j = 0; j < 16; ++j) b1v[j] = z[1][j] + s_bias1[32 + 8 * (j >> 2) + cq + (j & 1)];
         }
         fence_proxy_async();
-        tc_fence_before();
         __syncthreads();
-        tc_fence_after();
-        if (tid == 0) {
-            issue_gemm(tmem + COL_W1, A2h[0], A2l[0], B2ah, B2al, TC_HH, N2A);
-            issue_gemm(tmem + COL_W2, A2h[1], A2l[1], B2bh, B2bl, TC_HH, TC_HH);
-            issue_gemm(tmem + COL_B2, A2h[2], A2l[2], B2ch, B2cl, TC_HH, 16);
-            mma_commit(&mma_bar);
-        }
-        mbar_wait(&mma_bar, phase);
-        phase ^= 1;
-        tc_fence_after();
-        // ---- mixing epilogue (q_mix_head.py:81-94), thread = row
-        const bool live = tid < rows_valid;
-        float pre[TC_HH];
+        // ---- GEMM2: W1raw (one 32-column block per agent), W2raw, b2
+        float w1[8][16], w2[16], b2[8];
+        wgmma_fence();
+        {
+            const uint32_t off = (uint32_t)(64 * wg * TC_HH * 2);
+            uint32_t acc = 0;
+            for (int pa = 0; pa < 2; ++pa)
+                for (int pb = 0; pb < 2 - pa; ++pb) {
+                    const uint32_t ba = smem_u32(pb ? B2al : B2ah), bb = smem_u32(pb ? B2bl : B2bh), bc = smem_u32(pb ? B2cl : B2ch);
 #pragma unroll
-        for (int j = 0; j < TC_HH; ++j) pre[j] = b1v[j];
-        float w[32];
+                    for (int ks = 0; ks < TC_HH / 16; ++ks) {
+                        const uint32_t a0 = smem_u32(pa ? A2l[0] : A2h[0]) + off + ks * 256;
+                        const uint32_t a1 = smem_u32(pa ? A2l[1] : A2h[1]) + off + ks * 256;
+                        const uint32_t a2 = smem_u32(pa ? A2l[2] : A2h[2]) + off + ks * 256;
+#pragma unroll
+                        for (int i = 0; i < 8; ++i)
+                            if (i < n)
+                                wgmma_n32<0, 0>(w1[i], make_desc(a0, TC_HH), make_desc(ba + i * TC_HH * TC_HH * 2 + ks * 256, TC_HH), acc);
+                        wgmma_n32<0, 0>(w2, make_desc(a1, TC_HH), make_desc(bb + ks * 256, TC_HH), acc);
+                        wgmma_n16<0, 0>(b2, make_desc(a2, TC_HH), make_desc(bc + ks * 256, TC_HH), acc);
+                        acc = 1;
+                    }
+                }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        // each warpgroup waited for its own wgmmas only: the next tile's staging overwrites A1, which the A2 operands alias,
+        // so no thread may get there before BOTH warpgroups' GEMM2 has read them
+        __syncthreads();
+        // ---- mixing epilogue (q_mix_head.py:81-94) on the fragments: this thread holds 8 of the 32 hidden columns of
+        // its two rows; the row sums over the hidden units are finished across the 4 lanes that share a row
+        float pre[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) pre[j] = b1v[j];
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
             if (i < n) {
-                tmem_ld32(lane_addr + COL_W1 + i * TC_HH, w);
-                const float qi = qv[i];
 #pragma unroll
-                for (int j = 0; j < TC_HH; ++j) pre[j] += qi * fabsf(w[j] + s_bias_wb1[i * TC_HH + j]);
+                for (int j = 0; j < 16; ++j)
+                    pre[j] += qv[(j >> 1) & 1][i] * fabsf(w1[i][j] + s_bias_wb1[i * TC_HH + 8 * (j >> 2) + cq + (j & 1)]);
             }
         }
-        tmem_ld32(lane_addr + COL_W2, w);
-        float y = 0.f;
+        float y[2] = {0.f, 0.f};
 #pragma unroll
-        for (int j = 0; j < TC_HH; ++j) {
-            const float h = pre[j] > 0.f ? pre[j] : (expf(pre[j]) - 1.f);
-            y += h * fabsf(w[j] + s_bias_wb2[j]);
+        for (int j = 0; j < 16; ++j) {
+            const float hv = pre[j] > 0.f ? pre[j] : (expf(pre[j]) - 1.f);
+            y[(j >> 1) & 1] += hv * fabsf(w2[j] + s_bias_wb2[8 * (j >> 2) + cq + (j & 1)]);
         }
-        tmem_ld32(lane_addr + COL_B2, w);
-        if (live) p.q_tot[row0 + tid] = y + w[0] + s_bias_b2;
-    }
-    // ---- teardown
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TC_TMEM_COLS));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            y[h] += __shfl_xor_sync(0xffffffffu, y[h], 1);
+            y[h] += __shfl_xor_sync(0xffffffffu, y[h], 2);
+        }
+        // b2 is column 0 of its fragment: registers 0 (row r0) and 2 (row r0 + 8) of the lane with lane % 4 == 0
+        if ((lane & 3) == 0) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                if (r0 + 8 * h < rows_valid) p.q_tot[row0 + r0 + 8 * h] = y[h] + b2[2 * h] + s_bias_b2;
+        }
     }
 }
 
@@ -267,6 +272,6 @@ extern "C" int xb_qmix_mix_fused_fwd(const float *states, const float *q, const 
                wb1, bias_wb1, wb2, bias_wb2, wb2c, bias_wb2c, q_tot, R, S, n};
     int64_t tiles = (R + TC_ROWS - 1) / TC_ROWS;
     int grid = (int)(tiles < xb_sm_count() ? tiles : xb_sm_count());
-    qmix_mix_tc_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>(p);
+    qmix_mix_tc_kernel<<<grid, TC_THREADS, smem, (cudaStream_t)stream>>>(p);
     return xb_launch_status();
 }

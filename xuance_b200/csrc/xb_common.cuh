@@ -1,4 +1,4 @@
-// Shared device/host helpers for the xb200 kernels (sm_100a only).
+// Shared device/host helpers for the xb200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -6,7 +6,7 @@
 #include <stdint.h>
 #include "../../include/xb200.h"
 
-#define XB_SM_COUNT_FALLBACK 148
+#define XB_SM_COUNT_FALLBACK 132               // H100 SXM
 #define XB_MAX_PARTIALS 2048               // scratch doubles (per reduction slot group)
 #define XB_SCRATCH_DOUBLES (XB_MAX_PARTIALS * 8 + 8)
 

@@ -34,11 +34,9 @@ class PPO_Learner(Learner):
         """Optional (XB_EARLY_ALLREDUCE=1): the bulk of the gradient (the 6400->512 layer and the heads, 98 % of the parameters) is
         final before the convolution backward starts, so its all-reduce can be issued there (async, on NCCL's stream) and
         what remains - [statistics | convolution gradients], the front of the bucket - is one small all-reduce at the end.
-        Measured on B200: no difference at 2 GPUs (65.4 ms per step either way); at 8 GPUs the early piece does NOT hide - the
-        K12 launches are 148 persistent CTAs that hold every SM, NCCL's CTAs only run at launch boundaries, and the final piece
-        then waits for it: 0.20 ms of collectives exposed per update against 0.09 ms for ONE all-reduce of the whole bucket
-        issued at the end (profiles/r02_scale_n8.json: phases.nccl_all_reduce vs parity_vs_1gpu.allreduce_ms).  The default
-        is therefore the single collective.  Needs an encoder that reports when those gradients are in place
+        The early piece cannot hide behind the convolution backward: the K12 launches are persistent CTAs that hold every
+        SM, NCCL's CTAs only run at launch boundaries, and the final piece then waits for it.  The default is therefore the
+        single collective issued at the end.  Needs an encoder that reports when those gradients are in place
         (BoxNatureCNN.grads_ready) and the bucket laid out in parameter order."""
         import os
         enc = getattr(getattr(self.model, "representation", None), "_tc", None)       # set by _PixelEncoder.set_compute("tc")

@@ -123,7 +123,7 @@ class QMIX_Mixer(nn.Module):
         self.hyper_b_2 = nn.Sequential(nn.Linear(dim_state, dim_hypernet_hidden), nn.ReLU(),
                                        nn.Linear(dim_hypernet_hidden, 1)).to(device)
 
-    use_tensor_core_forward = True   # no-grad forwards (target mixer, inference) take the fused tcgen05 kernel
+    use_tensor_core_forward = True   # no-grad forwards (target mixer, inference) take the fused wgmma kernel
 
     def _fusable(self):
         kp1 = (self.dim_state + 15) // 16 * 16

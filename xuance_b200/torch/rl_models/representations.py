@@ -67,7 +67,7 @@ class _PixelEncoder(nn.Module):
         return {"fp32": _lib.OBS_F32_NCHW, "fp32_cl": _lib.OBS_F32_NHWC, "tf32": _lib.OBS_F32_NHWC,
                 "bf16": _lib.OBS_BF16_NHWC}[self.compute]
 
-    # ---- "tc" mode: the conv stack + hidden layer as K12 launches (split-bf16 tcgen05 GEMMs, float32 accumulation in TMEM,
+    # ---- "tc" mode: the conv stack + hidden layer as K12 launches (split-bf16 wgmma GEMMs, float32 accumulation,
     # utils/tc_conv.py): forward, data gradients and weight gradients; pinned against float64 in tests/test_gpu_tc_conv.py.
     def _build_tc(self):
         import os

@@ -5,7 +5,7 @@ gradients and weight gradients as the gathered-operand GEMM of ``xuance_b200/csr
 
 The geometry and the kernel's index arithmetic are verified on the host (tests/test_conv_index.py emulates the
 shared-memory staging, the descriptor reads and the per-plane MMA issue and compares with ``torch.nn.functional.conv2d`` /
-autograd); tests/test_gpu_tc_conv.py pins every mode against float64 on B200.
+autograd); tests/test_gpu_tc_conv.py pins every mode against float64 on the GPU.
 """
 from dataclasses import dataclass, field
 from typing import List
@@ -177,8 +177,8 @@ def pack_conv_weight(w, planes=2, scale=1.0):
 
 
 def n_tile_for(N, planes_b):
-    """Columns per work item: the largest multiple of 32 that divides N with planes_b * n_tile <= 256 (one tcgen05.mma
-    spans the planes_b adjacent weight planes of a tile)."""
+    """Columns per work item: the largest multiple of 32 that divides N with planes_b * n_tile <= 256 (the register
+    accumulators of a consumer thread hold planes_b * n_tile / 2 floats)."""
     t = (256 // planes_b) // 32 * 32
     while t >= 32:
         if N % t == 0:
@@ -275,7 +275,7 @@ def wgrad_reduce(partials, N, C, KH, KW, out=None, accumulate=False, scale=1.0):
     return out
 
 
-def wgrad_splits(M, K, n_tiles=1, sm_count=148):
+def wgrad_splits(M, K, n_tiles=1, sm_count=132):
     """Split count for the weight gradient: about two work items per SM, at least 8 chunks of 64 sites per split, at most
     4096 sites per split (the tensor core truncates on every addition into the accumulator: a chain of n K-steps carries a
     bias of up to n * 2^-24 relative, so long reductions are cut and the pieces added in float32 by xb_wgrad_reduce), and
@@ -594,7 +594,7 @@ def wgrad_box(x_pl, g_pl, bg, box_h, splits):
     return partials
 
 
-def wgrad_box_splits(g_rows, box_h, K, N, sm_count=148):
+def wgrad_box_splits(g_rows, box_h, K, N, sm_count=132):
     """Splits for the box weight gradient: about two work items per SM, chains of at most 4096 sites (truncating adds)."""
     tiles = -(-K // 128) * (N // 64)
     s = max(1, (2 * sm_count) // tiles, -(-g_rows * 10 // 4096))
@@ -610,7 +610,7 @@ def wgrad_box_splits(g_rows, box_h, K, N, sm_count=148):
 class BoxNatureCNN(TensorCoreNatureCNN):
     """``TensorCoreNatureCNN`` with the activations between the convolutions kept in PADDED-ROW layouts so that the A
     operands of every convolution after the first (forward and data gradient) are plain TMA boxes instead of 16-byte
-    cp.async gathers - on B200 a CTA's cp.async stream tops out near 13 B/clk (L1 miss tracking), a quarter of what the
+    cp.async gathers - a CTA's cp.async stream is limited by L1 miss tracking, well below what the
     tensor pipe needs for these 64-column layers.
 
     Layout of an activation with H real rows: [P, B, hp, W, C], real row i at row i + off, every other row zero (written once
