@@ -146,7 +146,9 @@ int xb_dqn_td_fwd_bwd(const float *q_eval, const float *q_next, const float *q_s
  * mix     : QMIX_Mixer.forward epilogue (q_mix_head.py:81-94) on precomputed hypernet outputs:
  *           hidden = elu(q . |w1_raw|[n,H] + b1) ; q_tot = hidden . |w2_raw| + b2   (n <= 16), and its backward
  *           (abs' = sign, elu' = exp) producing dq, dw1_raw, db1, dw2_raw (db2 = dq_tot).
- * td      : qmix_learner.py:34-35,76-84 masked TD loss; writes dq_tot and stats[2] = {loss_Q, mean(q_tot)}. */
+ * td      : qmix_learner.py:34-35,76-84 masked TD loss; writes dq_tot and stats[2] = {loss_Q, mean(q_tot)}.
+ *           filled_sum[0] and rows_total >= B*T are the GLOBAL sum(filled) and row count, so a rank-local shard
+ *           writes its share of the global-minibatch gradient and statistics (sums over local rows / global count). */
 int xb_qmix_select_fwd(const float *q_all, const float *q_tgt, const float *actions, const float *agent_mask,
                        const float *filled, const uint8_t *avail, int avail_ld, int B, int n, int T, int A,
                        int double_q, float *q_eval_taken, float *q_next_taken, float *filled_sum, double *scratch,
@@ -158,7 +160,7 @@ int xb_qmix_mix_fwd(const float *q, const float *w1_raw, const float *b1, const 
 int xb_qmix_mix_bwd(const float *dq_tot, const float *q, const float *w1_raw, const float *b1, const float *w2_raw,
                     int64_t R, int n, int H, float *dq, float *dw1_raw, float *db1, float *dw2_raw, void *stream);
 int xb_qmix_td(const float *q_tot, const float *q_tot_next, const float *rewards, const float *terminals,
-               const float *filled, const float *filled_sum, int B, int n, int T, float gamma, float grad_scale,
+               const float *filled, const float *filled_sum, int B, int n, int T, float gamma, int64_t rows_total,
                float *dq_tot, float *stats, double *scratch, void *stream);
 
 /* Tensor-core forward of the whole mixer (hypernet GEMMs + epilogue in ONE kernel; wgmma with register

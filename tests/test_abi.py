@@ -92,6 +92,9 @@ def test_every_entry_point_validates_before_touching_the_device():
     assert lib.xb_sac_actor_loss(junk, junk, junk, None, 8, 8, junk, junk, junk, junk, junk, None) == EINVAL
     assert lib.xb_qmix_mix_fwd(junk, junk, junk, junk, junk, 8, 17, 32, junk, None) == ERANGE   # n > 16
     assert lib.xb_qmix_select_fwd(junk, junk, junk, junk, junk, None, 0, 0, 5, 60, 12, 1, junk, junk, junk, junk, None) == EINVAL
+    td = lambda rows_total: lib.xb_qmix_td(junk, junk, junk, junk, junk, junk, 4, 5, 6, 0.99, rows_total, junk, junk, junk, None)
+    assert td(4 * 6 - 1) == EINVAL                     # rows_total is the global B*T: never below the local one
+    assert td(0) == EINVAL
     four = (P * 4)(junk, junk, junk, junk)
     assert lib.xb_qmix_mix_fused_fwd(junk, junk, four, four, junk, junk, junk, junk, junk, junk, 128, 98, 5, 64, 32, junk, None) == ERANGE
     assert lib.xb_qmix_mix_fused_fwd(junk, junk, four, four, junk, junk, junk, junk, junk, junk, 128, 160, 5, 32, 32, junk, None) == ERANGE  # smem

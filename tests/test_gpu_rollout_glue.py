@@ -15,7 +15,7 @@ DEV = "cuda:0"
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-@pytest.mark.parametrize("N,A", [(300, 4), (256, 2), (64, 6), (1000, 18), (33, 40), (7, 64)])
+@pytest.mark.parametrize("N,A", [(300, 4), (256, 2), (64, 6), (1000, 18), (129, 19), (64, 32), (33, 40), (7, 64)])
 def test_categorical_act_matches_oracle(N, A):
     from xuance_b200.torch.utils.rollout_glue import categorical_act
     rng = np.random.default_rng(N + A)

@@ -65,7 +65,7 @@ _SIGNATURES = {
     "xb_qmix_select_bwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
     "xb_qmix_mix_fwd": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int, c_int, _P, _P]),
     "xb_qmix_mix_bwd": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int, c_int, _P, _P, _P, _P, _P]),
-    "xb_qmix_td": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, c_float, _P, _P, _P, _P]),
+    "xb_qmix_td": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, c_int64, _P, _P, _P, _P]),
     "xb_qmix_mix_fused_fwd": (c_int, [_P] * 10 + [c_int64, c_int, c_int, c_int, c_int, _P, _P]),
     "xb_powf_libm": (c_int, [_P, c_float, _P, c_int64, _P]),
 }

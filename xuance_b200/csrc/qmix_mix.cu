@@ -314,13 +314,15 @@ extern "C" int xb_qmix_mix_bwd(const float *dq_tot, const float *q, const float 
 // =====================================================================================================
 // (c) masked TD loss (qmix_learner.py:34-35, 76-84): team reward = mean over agents, team terminal = all agents,
 //     y = r + (1-d)*gamma*Qtot' ; td = (Qtot - y)*filled ; loss = sum(td^2)/sum(filled) ; dQtot = 2*td*filled/sum(filled)
+// Both denominators are global (filled_sum all-reduced, rows_total = B*T over all ranks), so a rank-local shard writes
+// its share of the global sums, like K4/K6/K8.
 // =====================================================================================================
 __global__ void __launch_bounds__(256) qmix_td_kernel(const float *__restrict__ q_tot, const float *__restrict__ q_tot_next,
                                                       const float *__restrict__ rewards,
                                                       const float *__restrict__ terminals,
                                                       const float *__restrict__ filled,
                                                       const float *__restrict__ filled_sum, int B, int n, int T,
-                                                      float gamma, float inv_world, float *__restrict__ dq_tot,
+                                                      float gamma, int64_t rows_total, float *__restrict__ dq_tot,
                                                       float *__restrict__ stats, double *__restrict__ scratch) {
     __shared__ double red[2 * 32];
     double acc[2] = {0, 0};
@@ -340,25 +342,26 @@ __global__ void __launch_bounds__(256) qmix_td_kernel(const float *__restrict__ 
         const float y = r_tot + (1.f - d_tot) * gamma * q_tot_next[row];
         const float f = filled[row];
         const float td = (q_tot[row] - y) * f;
-        dq_tot[row] = 2.f * td * f / fs * inv_world;
+        dq_tot[row] = 2.f * td * f / fs;
         acc[0] += (double)td * td;
         acc[1] += (double)q_tot[row];
     }
     grid_sum_finalize<2>(acc, scratch, red, [&](double(&tsum)[2]) {
-        stats[0] = (float)(tsum[0] / (double)fs);   // loss_Q
-        stats[1] = (float)(tsum[1] / (double)R);    // predictQ = mean(q_tot_eval)
+        stats[0] = (float)(tsum[0] / (double)fs);            // loss_Q
+        stats[1] = (float)(tsum[1] / (double)rows_total);    // predictQ = mean(q_tot_eval)
     });
 }
 
 extern "C" int xb_qmix_td(const float *q_tot, const float *q_tot_next, const float *rewards, const float *terminals,
                           const float *filled, const float *filled_sum, int B, int n, int T, float gamma,
-                          float inv_world, float *dq_tot, float *stats, double *scratch, void *stream) {
+                          int64_t rows_total, float *dq_tot, float *stats, double *scratch, void *stream) {
     if (!q_tot || !q_tot_next || !rewards || !terminals || !filled || !filled_sum || !dq_tot || !stats || !scratch)
         return XB_EINVAL;
     if (B <= 0 || n <= 0 || T <= 0) return XB_EINVAL;
     int64_t R = (int64_t)B * T, want = (R + 255) / 256;
+    if (rows_total < R) return XB_EINVAL;
     int grid = (int)(want < XB_MAX_PARTIALS ? want : XB_MAX_PARTIALS);
     qmix_td_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(q_tot, q_tot_next, rewards, terminals, filled, filled_sum, B, n,
-                                                           T, gamma, inv_world, dq_tot, stats, scratch);
+                                                           T, gamma, rows_total, dq_tot, stats, scratch);
     return xb_launch_status();
 }

@@ -121,7 +121,8 @@ class QMIX_Learner(Learner):
             q_tot_next = self.model.Qtarget_tot(q_next_taken, state[:, 1:]).reshape(-1).contiguous()
         dq_tot = torch.empty_like(q_tot_eval)
         _lib.call("xb_qmix_td", _lib.ptr(q_tot_eval), _lib.ptr(q_tot_next), _lib.ptr(rewards), _lib.ptr(terminals),
-                  _lib.ptr(filled), _lib.ptr(self._filled_sum), B, n, T, float(self.gamma), 1.0, _lib.ptr(dq_tot),
+                  _lib.ptr(filled), _lib.ptr(self._filled_sum), B, n, T, float(self.gamma), B * T * self.world_size,
+                  _lib.ptr(dq_tot),
                   _lib.ptr(self._stats), _lib.ptr(self._scratch))
         self.optimizer.zero_grad()
         torch.autograd.backward([q_tot_eval], [dq_tot])
