@@ -103,6 +103,24 @@ int xb_ppo_loss_fwd_bwd(const float *logits, const float *value, const float *ac
                         int64_t B, int A, int64_t B_total, float clip_range, float vf_coef, float ent_coef,
                         int loss_kind, float *dlogits, float *dvalue, float *stats, double *scratch, void *stream);
 
+/* ---------------------------------------------------------------- K4G: fused Gaussian PPO loss fwd+bwd -
+ * ppo_learner.py:46-60 (and a2c_learner.py:46-52, pg_learner.py:44-47 with loss_kind 1) for a DiagGaussianDistribution
+ * (modules/distributions.py:165-197): Normal(mu, exp(log_std)), log_prob and entropy summed over the D components:
+ *   logp_b = sum_j [-(x-mu)^2/(2 sigma^2) - log_std_j - log sqrt(2 pi)]  (j in index order)
+ *   H_b    = sum_j [1/2 + log(2 pi)/2 + log_std_j]
+ * ratio, clamp, minimum, tie split, clamp boundary, loss_kind, B_total scaling and stats[8] exactly as K4.
+ * Writes dmu[B,D], dvalue[B] and dlog_std[D] = the sum over the local rows divided by B_total (a SUM all-reduce of
+ * the shards gives the global gradient).  mu / actions [B,D] float32, log_std [D]; 1 <= D <= 64 (else XB_ERANGE).
+ * ws: caller workspace of >= xb_ppo_gauss_ws_doubles(B, D) doubles (D * min(ceil(B/256), 2048); 64 * 2048 doubles
+ * always suffice) for the per-block column partials of dlog_std, which are added in block order: dlog_std is
+ * bit-identical from launch to launch.  ws_doubles is its size (XB_EINVAL if too small); scratch as for K4. */
+int64_t xb_ppo_gauss_ws_doubles(int64_t B, int D);
+int xb_ppo_gauss_loss_fwd_bwd(const float *mu, const float *log_std, const float *value, const float *actions,
+                              const float *old_logp, const float *adv, const float *ret, int64_t B, int D,
+                              int64_t B_total, float clip_range, float vf_coef, float ent_coef, int loss_kind,
+                              float *dmu, float *dlog_std, float *dvalue, float *stats, double *scratch, double *ws,
+                              int64_t ws_doubles, void *stream);
+
 /* ---------------------------------------------------------------- K5: prioritized-replay trees -------
  * Replaces SumSegmentTree/MinSegmentTree (xuance/common/segtree_tool.py:4-220) and their use in
  * PerOffPolicyBuffer (memory_tools.py:505-598).  One (sum,min) pair PER ENV, float32 nodes, heap layout
@@ -220,6 +238,12 @@ int xb_soft_update(float *target, const float *source, int64_t n, float tau, voi
  *   else                   : a_n = first argmax_i p_i               (deterministic_sample)
  *   outputs (each nullable, at least one): actions_f32[N] (the float32 the buffers store), actions_i32[N] (for the
  *   host-side env step), logp[N] = log_softmax(logits)[a], entropy[N] = -sum p log p.
+ * xb_gaussian_act: DiagGaussianDistribution(mu[N,D], exp(log_std[D])) (modules/distributions.py:165-197).
+ *   forced_actions != NULL : x = forced_actions[N,D]; actions_f32 is not written (log_prob / entropy of given actions)
+ *   else noise != NULL     : x = mu + exp(log_std) * noise, noise[N,D] standard normals (stochastic_sample)
+ *   else                   : x = mu                                   (deterministic_sample)
+ *   outputs (each nullable, at least one): actions_f32[N,D] (e.g. the rollout buffer's staging rows),
+ *   logp[N] = sum_j log N(x_j; mu_j, sigma_j), entropy[N] = sum_j (1/2 + log(2 pi)/2 + log_std_j).
  * xb_rms_update_normalize: x[N,D] float32.
  *   update != 0: (mean, var)[D] <- parallel-variance merge with the batch moments, float32 in the reference's operation
  *                order; `count` is the running count BEFORE the merge (host state, Python float in the reference).
@@ -228,6 +252,8 @@ int xb_soft_update(float *target, const float *source, int64_t n, float tau, voi
  */
 int xb_categorical_act(const float *logits, const float *uniforms, const float *forced_actions, int N, int A,
                        float *actions_f32, int32_t *actions_i32, float *logp, float *entropy, void *stream);
+int xb_gaussian_act(const float *mu, const float *log_std, const float *noise, const float *forced_actions, int N, int D,
+                    float *actions_f32, float *logp, float *entropy, void *stream);
 int xb_rms_update_normalize(const float *x, int N, int64_t D, float *mean, float *var, double count, int update,
                             float *out, float clip_range, float eps, void *stream);
 

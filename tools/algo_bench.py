@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Secondary measurements for BASELINE configs 3-5 (parity-test cases, not the headline): sample + update throughput of
 DQN+PER (2^20-transition HBM replay, B=512), SAC (1M replay, B=1024) and QMIX (5 agents x 72-d, T=60, 32 episodes)
-on one GPU, next to the oracle port of the reference's torch-CPU path on the host.  Prints one JSON object.
+on one GPU, next to the oracle port of the reference's torch-CPU path on the host; and ``ppo_gauss``, continuous-control
+PPO in the shape of the reference's ppo/mujoco.yaml (train_epochs env-steps/s).  Prints one JSON object.
 
     python tools/algo_bench.py [--iters 200] [--cpu-iters 5] [--no-cpu] [--graph]
     torchrun --nnodes=1 --nproc-per-node G --master-addr 127.0.0.1 tools/algo_bench.py --no-cpu --graph    (G GPUs)
@@ -184,6 +185,51 @@ def bench_qmix(args, Be=32):
     return out
 
 
+def bench_ppo_gauss(args):
+    """PPO with a Gaussian policy in the shape of the reference's ppo/mujoco.yaml (Ant-v4: 27-d obs, 8-d action): 16 envs x
+    256 steps, 16 epochs x 8 minibatches of 512, Basic_Identical + actor / critic [256, 256].  The measured unit is
+    ``train_epochs`` over one stored rollout (128 minibatch updates); env-steps/s = 4096 / its time."""
+    from xuance_b200.common import Box
+    from xuance_b200.torch.agents import PPO_Agent
+    N, T, od, ad, epochs, mb = 16, 256, 27, 8, 16, 8
+    cfg = Namespace(agent="PPO", learner="PPO_Learner", representation="Basic_Identical", env_name="MuJoCo",
+                    distributed_training=False, device=DEV, seed=1, parallels=N, running_steps=10**6, horizon_size=T,
+                    n_epochs=epochs, n_minibatch=mb, learning_rate=4e-4, vf_coef=0.25, ent_coef=0.0, clip_range=0.2,
+                    gamma=0.99, use_gae=True, gae_lambda=0.95, use_advnorm=True, use_grad_clip=True, grad_clip_norm=0.5,
+                    use_obsnorm=False, use_rewnorm=False, activation="leaky_relu", activation_action="tanh",
+                    actor_hidden_size=[256, 256], critic_hidden_size=[256, 256], model_dir="/tmp/x", logger=None,
+                    episode_length=None, use_cuda_graph=args.graph)
+    agent = PPO_Agent(cfg, None, Box(-np.inf, np.inf, (od,), np.float32), Box(-1, 1, (ad,), np.float32))
+    rng = np.random.default_rng(0)
+    ro = dict(obs=rng.normal(size=(T, N, od)).astype(np.float32), acts=np.clip(rng.normal(size=(T, N, ad)), -1, 1).astype(np.float32),
+              rews=rng.normal(size=(T, N)).astype(np.float32), vals=rng.normal(size=(T, N)).astype(np.float32),
+              terms=rng.random((T, N)) < 0.005, logp=(rng.normal(size=(T, N)) * 0.3 - 7.0).astype(np.float32))
+    for t in range(T):
+        agent.memory.store(ro["obs"][t], ro["acts"][t], ro["rews"][t], ro["vals"][t], ro["terms"][t], {"old_logp": ro["logp"][t]})
+    for i in range(N):
+        agent.memory.finish_path(0.0, i)
+    iters = max(2, args.iters // 40)
+    dt = timed(lambda: agent.train_epochs(epochs), iters, warm=1)
+    out = {"config": "PPO Gaussian policy, Ant-v4 shape (27-d obs, 8-d action), 16 envs x 256, 16 epochs x 8 minibatches "
+                     "of 512, Basic_Identical + actor/critic MLP 256-256", "gpu_env_steps_per_s": N * T / dt,
+           "gpu_ms_per_train_epochs": dt * 1e3, "gpu_ms_per_update": dt * 1e3 / (epochs * mb)}
+    if not args.no_cpu:
+        from oracle.onpolicy import OnPolicyBufferOracle
+        from oracle_gauss import GaussianActorCriticOracle, PPOGaussLearnerOracle
+        ob = OnPolicyBufferOracle((od,), (ad,), {"old_logp": ()}, N, T)
+        for t in range(T):
+            ob.store(ro["obs"][t], ro["acts"][t], ro["rews"][t], ro["vals"][t], ro["terms"][t], {"old_logp": ro["logp"][t]})
+        for i in range(N):
+            ob.finish_path(0.0, i)
+        ol = PPOGaussLearnerOracle(GaussianActorCriticOracle(od, ad, rep_hidden=(), actor_hidden=(256, 256),
+                                                             critic_hidden=(256, 256)), learning_rate=4e-4, ent_coef=0.0)
+        idx = np.arange(N * T)
+        cdt = cpu_timed(lambda: ol.update(**ob.sample(np.random.permutation(idx)[:N * T // mb])), max(args.cpu_iters, 20))
+        out.update(cpu_ms_per_update=cdt * 1e3, cpu_env_steps_per_s=N * T / (cdt * epochs * mb),
+                   cpu_threads=torch.get_num_threads(), speedup=cdt * epochs * mb / dt)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=200)
@@ -211,6 +257,8 @@ def main():
     if not only or "qmix" in only:
         res["qmix"] = bench_qmix(args)
         res["qmix_4096"] = bench_qmix(Namespace(**{**vars(args), "iters": 20, "no_cpu": True}), Be=1024)
+    if (not only and WORLD == 1) or "ppo_gauss" in only:
+        res["ppo_gauss"] = bench_ppo_gauss(args)
     res["cuda_graph"] = bool(args.graph)
     res["n_gpus"] = WORLD
     if RANK == 0:

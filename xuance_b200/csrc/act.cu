@@ -97,6 +97,56 @@ extern "C" int xb_categorical_act(const float *logits, const float *uniforms, co
 }
 
 // =====================================================================================================
+// K10G  xb_gaussian_act
+// =====================================================================================================
+// DiagGaussianDistribution(mu, exp(log_std)) (modules/distributions.py:165-197) over mu[N,D], log_std[D]:
+//   forced:        x = forced_actions[n]            (log_prob of given actions; no action is written)
+//   stochastic:    x = mu + sigma * noise[n]        (stochastic_sample on the caller's standard normals)
+//   deterministic: x = mu                           (deterministic_sample)
+//   logp = sum_j (-z_j^2/2 - log_std_j - log sqrt(2 pi)), z_j = (x_j - mu_j) / sigma_j (j in index order)
+//   entropy = sum_j (1/2 + log(2 pi)/2 + log_std_j)
+// As for K10, torch's Normal.sample stream cannot be reproduced by a fused kernel: parity of the draw is defined on the
+// supplied noise, parity of logp / entropy on the action taken.
+#define XB_ACT_LOG_SQRT_2PI 0.91893853320467274178f
+__global__ void __launch_bounds__(128) gaussian_act_kernel(const float *__restrict__ mu,
+                                                           const float *__restrict__ log_std,
+                                                           const float *__restrict__ noise,
+                                                           const float *__restrict__ forced, int N, int D,
+                                                           float *__restrict__ act_f, float *__restrict__ logp,
+                                                           float *__restrict__ entropy) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= N) return;
+    const float *mr = mu + (int64_t)n * D;
+    float lp = 0.f, ent = 0.f;
+    for (int j = 0; j < D; ++j) {
+        const float ls = log_std[j], m = mr[j];
+        const float sig = expf(ls);
+        float x;
+        if (forced) {
+            x = forced[(int64_t)n * D + j];
+        } else {
+            x = noise ? m + sig * noise[(int64_t)n * D + j] : m;
+            if (act_f) act_f[(int64_t)n * D + j] = x;
+        }
+        const float z = (x - m) * (1.f / sig);  // K4G's arithmetic: its forced log-prob is the loss kernel's
+        lp += -0.5f * z * z - ls - XB_ACT_LOG_SQRT_2PI;
+        ent += 0.5f + XB_ACT_LOG_SQRT_2PI + ls;
+    }
+    if (logp) logp[n] = lp;
+    if (entropy) entropy[n] = ent;
+}
+
+extern "C" int xb_gaussian_act(const float *mu, const float *log_std, const float *noise, const float *forced_actions,
+                               int N, int D, float *actions_f32, float *logp, float *entropy, void *stream) {
+    if (!mu || !log_std || N <= 0 || D <= 0) return XB_EINVAL;
+    if (!actions_f32 && !logp && !entropy) return XB_EINVAL;
+    const int grid = (N + 127) / 128;
+    gaussian_act_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(mu, log_std, noise, forced_actions, N, D, actions_f32,
+                                                                logp, entropy);
+    return xb_launch_status();
+}
+
+// =====================================================================================================
 // K11  xb_rms_update_normalize
 // =====================================================================================================
 // RunningMeanStd.update + Agent._process_observation for a float32 batch x[N,D] (common/statistic_tools.py:117-185,

@@ -164,6 +164,163 @@ extern "C" int xb_ppo_loss_fwd_bwd(const float *logits, const float *value, cons
 }
 
 // =====================================================================================================
+// K4G  xb_ppo_gauss_loss_fwd_bwd
+// =====================================================================================================
+// The same loss for a diagonal Gaussian policy: torch.distributions.Normal(mu, exp(log_std)) as the reference's
+// DiagGaussianDistribution uses it (modules/distributions.py:165-197), log_prob and entropy summed over the D action
+// components.  Per row, with z_j = (x_j - mu_j) / sigma_j:
+//   logp = sum_j (-z_j^2/2 - log_std_j - log sqrt(2 pi))   (j in index order)   H = sum_j (1/2 + log(2 pi)/2 + log_std_j)
+//   dmu_j = d_logp * z_j / sigma_j ;  d log_std_j (this row) = d_logp * (z_j^2 - 1) + dent
+// log_std is shared by every row: each thread accumulates its rows' terms per column in float, each block adds its
+// threads' sums in double in a fixed order and deposits one partial per column into ws[D][grid]; the last block to
+// arrive adds the partials in block order.  No float atomics: dlog_std is bit-identical from launch to launch.
+#define XB_LOG_SQRT_2PI 0.91893853320467274178f
+template <int D_MAX>
+__global__ void __launch_bounds__(256, 1) ppo_gauss_loss_kernel(
+    const float *__restrict__ mu, const float *__restrict__ log_std, const float *__restrict__ value,
+    const float *__restrict__ actions, const float *__restrict__ old_logp, const float *__restrict__ adv,
+    const float *__restrict__ ret, int64_t B, int D, float inv_bt, float clip, float vf_coef, float ent_coef,
+    int loss_kind, float *__restrict__ dmu, float *__restrict__ dlog_std, float *__restrict__ dvalue,
+    float *__restrict__ stats, double *__restrict__ scratch, double *__restrict__ ws) {
+    __shared__ double red[6 * 32];
+    __shared__ double cred[D_MAX * 8];  // [column][warp] partials of the block (256 threads = 8 warps)
+    __shared__ float s_ls[D_MAX], s_isig[D_MAX];
+    for (int j = threadIdx.x; j < D; j += blockDim.x) {
+        const float ls = log_std[j];
+        s_ls[j] = ls;
+        s_isig[j] = 1.f / expf(ls);
+    }
+    __syncthreads();
+    float ent = 0.f;  // the same for every row
+#pragma unroll
+    for (int j = 0; j < D_MAX; ++j)
+        if (j < D) ent += 0.5f + XB_LOG_SQRT_2PI + s_ls[j];
+    double acc[6] = {0, 0, 0, 0, 0, 0};  // a_loss, c_loss, entropy, v, clipped count, (unused)
+    double col_lo = 0.0, col_hi = 0.0;    // this warp's sums of the columns lane and lane + 32
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const float lo = 1.0f - clip, hi = 1.0f + clip;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    // block-uniform trip count: every lane takes part in the column shuffles, rows past B contribute zero
+    for (int64_t base = (int64_t)blockIdx.x * blockDim.x; base < B; base += stride) {
+        const int64_t b = base + threadIdx.x;
+        const bool active = b < B;
+        const int64_t bb = active ? b : 0;
+        const float *mr = mu + bb * D, *xr = actions + bb * D;
+        float logp = 0.f;
+#pragma unroll
+        for (int j = 0; j < D_MAX; ++j) {
+            if (j < D) {
+                const float z = (xr[j] - mr[j]) * s_isig[j];
+                logp += -0.5f * z * z - s_ls[j] - XB_LOG_SQRT_2PI;
+            }
+        }
+        const float ad = adv[bb];
+        float ratio = 1.f, smin, d_logp;
+        if (loss_kind == 0) {  // PPO-Clip surrogate: K4's rules for ratio, clamp, min and their ties
+            ratio = expf(logp - old_logp[bb]);
+            const float rc = fminf(fmaxf(ratio, lo), hi);
+            const float s1 = rc * ad, s2 = ad * ratio;
+            smin = fminf(s1, s2);
+            float g1 = s1 < s2 ? 1.f : (s1 == s2 ? 0.5f : 0.f);
+            float g2 = s2 < s1 ? 1.f : (s1 == s2 ? 0.5f : 0.f);
+            const bool inside = ratio >= lo && ratio <= hi;
+            d_logp = -inv_bt * ad * ((inside ? g1 : 0.f) + g2) * ratio;
+        } else {  // plain policy gradient (A2C / PG)
+            smin = ad * logp;
+            d_logp = -inv_bt * ad;
+        }
+        float *gr = dmu + b * D;
+#pragma unroll
+        for (int j = 0; j < D_MAX; ++j) {
+            if (j < D) {
+                const float z = (xr[j] - mr[j]) * s_isig[j];
+                if (active) gr[j] = d_logp * z * s_isig[j];
+                const double s = warp_sum_d(active ? (double)(d_logp * (z * z - 1.f)) : 0.0);
+                if (j < 32) col_lo += (lane == j) ? s : 0.0;
+                else col_hi += (lane == j - 32) ? s : 0.0;
+            }
+        }
+        if (active) {
+            const float v = value[b];
+            const float dv = v - ret[b];
+            dvalue[b] = vf_coef * 2.f * dv * inv_bt;
+            acc[0] += (double)(-smin);
+            acc[1] += (double)dv * (double)dv;
+            acc[2] += (double)ent;
+            acc[3] += (double)v;
+            acc[4] += (ratio < lo || ratio > hi) ? 1.0 : 0.0;
+        }
+    }
+    // column partials of this block: the 8 warps' sums in warp order
+    if (lane < D) cred[lane * 8 + warp] = col_lo;
+    if (lane + 32 < D) cred[(lane + 32) * 8 + warp] = col_hi;
+    __syncthreads();
+    if (threadIdx.x < D) {
+        double s = 0.0;
+        for (int w = 0; w < 8; ++w) s += cred[threadIdx.x * 8 + w];
+        ws[(int64_t)threadIdx.x * gridDim.x + blockIdx.x] = s;
+        __threadfence();
+    }
+    const bool last = grid_sum_finalize<6>(acc, scratch, red, [&](double(&t)[6]) {
+        const double ib = (double)inv_bt;
+        float a_loss = (float)(t[0] * ib), c_loss = (float)(t[1] * ib), e = (float)(t[2] * ib);
+        stats[0] = a_loss;
+        stats[1] = c_loss;
+        stats[2] = e;
+        stats[3] = (float)(t[3] * ib);
+        stats[4] = (float)(t[4] * ib);
+        stats[5] = a_loss - ent_coef * e + vf_coef * c_loss;
+        stats[6] = 0.f;
+        stats[7] = 0.f;
+    });
+    if (last && threadIdx.x < D) {
+        const double *p = ws + (int64_t)threadIdx.x * gridDim.x;
+        double s = 0.0;
+        for (int k = 0; k < (int)gridDim.x; ++k) s += __ldcg(&p[k]);
+        // the entropy term: d(-ent_coef * mean H)/d log_std_j = -ent_coef / B_total for each local row
+        s += (double)B * (-(double)ent_coef * (double)inv_bt);
+        dlog_std[threadIdx.x] = (float)s;
+    }
+}
+
+extern "C" int64_t xb_ppo_gauss_ws_doubles(int64_t B, int D) {
+    if (B <= 0 || D <= 0) return 0;
+    const int64_t want = (B + 255) / 256;
+    return (int64_t)D * (want < XB_MAX_PARTIALS ? want : XB_MAX_PARTIALS);
+}
+
+extern "C" int xb_ppo_gauss_loss_fwd_bwd(const float *mu, const float *log_std, const float *value,
+                                         const float *actions, const float *old_logp, const float *adv,
+                                         const float *ret, int64_t B, int D, int64_t B_total, float clip_range,
+                                         float vf_coef, float ent_coef, int loss_kind, float *dmu, float *dlog_std,
+                                         float *dvalue, float *stats, double *scratch, double *ws,
+                                         int64_t ws_doubles, void *stream) {
+    if (!mu || !log_std || !value || !actions || !adv || !ret || !dmu || !dlog_std || !dvalue || !stats || !scratch ||
+        !ws)
+        return XB_EINVAL;
+    if (loss_kind != 0 && loss_kind != 1) return XB_EINVAL;
+    if (loss_kind == 0 && !old_logp) return XB_EINVAL;
+    if (B <= 0 || B_total < B || D <= 0) return XB_EINVAL;
+    if (D > 64) return XB_ERANGE;
+    if (ws_doubles < xb_ppo_gauss_ws_doubles(B, D)) return XB_EINVAL;
+    cudaStream_t s = (cudaStream_t)stream;
+    int64_t want = (B + 255) / 256;
+    int grid = (int)(want < XB_MAX_PARTIALS ? want : XB_MAX_PARTIALS);
+    const float inv_bt = 1.0f / (float)B_total;
+#define XB_PPOG(DM)                                                                                                  \
+    ppo_gauss_loss_kernel<DM><<<grid, 256, 0, s>>>(mu, log_std, value, actions, old_logp, adv, ret, B, D, inv_bt,    \
+                                                   clip_range, vf_coef, ent_coef, loss_kind, dmu, dlog_std, dvalue,  \
+                                                   stats, scratch, ws)
+    if (D <= 4) XB_PPOG(4);
+    else if (D <= 8) XB_PPOG(8);
+    else if (D <= 16) XB_PPOG(16);
+    else if (D <= 32) XB_PPOG(32);
+    else XB_PPOG(64);
+#undef XB_PPOG
+    return xb_launch_status();
+}
+
+// =====================================================================================================
 // K6  xb_dqn_td_fwd_bwd
 // =====================================================================================================
 __global__ void __launch_bounds__(256) dqn_td_kernel(const float *__restrict__ q_eval, const float *__restrict__ q_next,

@@ -65,8 +65,10 @@ __device__ __forceinline__ void block_sum_d(double (&v)[K], double *smem) {
 // Deterministic grid reduction: every block deposits K partial sums, the last block to arrive (ticket counter)
 // adds them in block order and calls fin(total[K]).  scratch layout: [K][XB_MAX_PARTIALS] doubles then the
 // int32 ticket at scratch[K_MAX*XB_MAX_PARTIALS] (K_MAX = 8).  gridDim.x <= XB_MAX_PARTIALS.
+// Returns, in every thread, whether this block was the last to arrive: global writes the block's threads fenced
+// before the call are then visible to it (K4G sums its column partials there).
 template <int K, typename Fin>
-__device__ __forceinline__ void grid_sum_finalize(double (&v)[K], double *scratch, double *smem, Fin fin) {
+__device__ __forceinline__ bool grid_sum_finalize(double (&v)[K], double *scratch, double *smem, Fin fin) {
     __shared__ bool is_last;
     int *ticket = reinterpret_cast<int *>(scratch + 8 * XB_MAX_PARTIALS);
     block_sum_d<K>(v, smem);
@@ -95,6 +97,7 @@ __device__ __forceinline__ void grid_sum_finalize(double (&v)[K], double *scratc
             fin(acc);
         }
     }
+    return is_last;
 }
 
 // ---------------------------------------------------------------- mbarrier + 1-D bulk async copy (TMA unit)

@@ -1,6 +1,7 @@
 """Raw environments available without third-party simulators (no gymnasium / ALE / SMAC in this image):
-``CartPoleEnv`` - CartPole-v1 dynamics restated from the classic-control equations (BASELINE config 1 plumbing) -
-and ``SyntheticAtariEnv`` - Atari-SHAPED frames (84x84x4 uint8), sign-clipped rewards, rare terminals (the
+``CartPoleEnv`` - CartPole-v1 dynamics restated from the classic-control equations (BASELINE config 1 plumbing),
+``PendulumEnv`` - Pendulum-v1 restated the same way (a continuous-control task for PPO's Gaussian policy) - and
+``SyntheticAtariEnv`` - Atari-SHAPED frames (84x84x4 uint8), sign-clipped rewards, rare terminals (the
 synthetic workload of BASELINE config 2; SURVEY.md section 8d).  ``XuanCeEnvWrapper`` adds the episode_step /
 episode_score bookkeeping of xuance/environment/utils/wrapper.py:76-97 (actions are NOT rescaled: appendix B #17)."""
 import math
@@ -51,6 +52,55 @@ class CartPoleEnv:
                           or theta > self.theta_threshold)
         truncated = self.steps >= self.max_episode_steps
         return self.state.astype(np.float32), 1.0, terminated, truncated, {}
+
+    def close(self):
+        pass
+
+    def render(self, *a, **k):
+        return None
+
+
+def _angle_normalize(x):
+    return ((x + math.pi) % (2 * math.pi)) - math.pi
+
+
+class PendulumEnv:
+    """Pendulum-v1 of the classic-control suite: swing a frictionless pendulum up and hold it upright.  Observation
+    (cos th, sin th, th_dot); action a torque in [-2, 2] (the step clips it there, as Pendulum does - the agent's actions
+    are not rescaled); reward -(th^2 + 0.1 th_dot^2 + 0.001 u^2) with th normalised to [-pi, pi); never terminates,
+    truncated after 200 steps (the registered TimeLimit)."""
+    max_episode_steps = 200
+
+    def __init__(self, seed=None, g=10.0):
+        self.max_speed, self.max_torque, self.dt = 8.0, 2.0, 0.05
+        self.g, self.m, self.l = g, 1.0, 1.0
+        high = np.array([1.0, 1.0, self.max_speed], dtype=np.float32)
+        self.observation_space = Box(-high, high, dtype=np.float32)
+        self.action_space = Box(-self.max_torque, self.max_torque, (1,), np.float32)
+        self.rng = np.random.default_rng(seed)
+        self.state, self.steps, self.last_u = None, 0, None
+
+    def _obs(self):
+        th, thdot = self.state
+        return np.array([math.cos(th), math.sin(th), thdot], dtype=np.float32)
+
+    def reset(self, seed=None, **kwargs):
+        if seed is not None:
+            self.rng = np.random.default_rng(seed)
+        self.state = self.rng.uniform(low=[-math.pi, -1.0], high=[math.pi, 1.0])
+        self.steps, self.last_u = 0, None
+        return self._obs(), {}
+
+    def step(self, action):
+        th, thdot = self.state
+        u = float(np.clip(np.asarray(action, dtype=np.float64).reshape(-1)[0], -self.max_torque, self.max_torque))
+        self.last_u = u
+        cost = _angle_normalize(th) ** 2 + 0.1 * thdot ** 2 + 0.001 * u ** 2
+        newthdot = thdot + (3 * self.g / (2 * self.l) * math.sin(th) + 3.0 / (self.m * self.l ** 2) * u) * self.dt
+        newthdot = float(np.clip(newthdot, -self.max_speed, self.max_speed))
+        self.state = np.array([th + newthdot * self.dt, newthdot])
+        self.steps += 1
+        return self._obs(), -float(cost), False, self.steps >= self.max_episode_steps, {}
 
     def close(self):
         pass
@@ -119,4 +169,4 @@ class XuanCeEnvWrapper:
         return self.env.close()
 
 
-REGISTRY_ENV = {"CartPole-v1": CartPoleEnv, "SyntheticAtari": SyntheticAtariEnv}
+REGISTRY_ENV = {"CartPole-v1": CartPoleEnv, "Pendulum-v1": PendulumEnv, "SyntheticAtari": SyntheticAtariEnv}

@@ -5,8 +5,8 @@ import numpy as np
 import torch
 
 from ...common.spaces import is_discrete, space2shape
-from ..utils.rollout_glue import categorical_act, DeviceRunningMeanStd, ActionReadback
-from ..rl_models import CategoricalActorHead, ValueHead, SharedActorCritic
+from ..utils.rollout_glue import categorical_act, gaussian_act, DeviceRunningMeanStd, ActionReadback
+from ..rl_models import CategoricalActorHead, GaussianActorHead, ValueHead, SharedActorCritic, ActivationFunctions
 from .on_policy import OnPolicyAgent
 
 
@@ -18,19 +18,35 @@ class PPO_Agent(OnPolicyAgent):
         self.learner = self._build_learner(self.config, self.model, self.callback)
 
     def _build_model(self):
-        """ppo_agent.py:40-93 (shared representation + categorical actor head + value head)."""
+        """ppo_agent.py:40-93 (shared representation + categorical (Discrete) or Gaussian (Box) actor head + value
+        head)."""
         if not getattr(self.config, "shared_representation", True):
             raise NotImplementedError("separate actor/critic representations are outside the hot path scope")
+        gaussian = self._gaussian_policy
+        if not (is_discrete(self.action_space) or gaussian):
+            raise NotImplementedError("PPO supports Discrete and one-dimensional Box action spaces, got %r"
+                                      % (self.action_space,))
+        if gaussian and self.action_space.shape[0] > 64:
+            raise NotImplementedError("PPO with a Box action space: the fused K4G loss takes at most 64 action "
+                                      "components, this space has %d" % self.action_space.shape[0])
         rep = self._build_representation(self.config.representation, self.observation_space, self.config)
-        if not is_discrete(self.action_space):
-            raise NotImplementedError("PPO with a Box action space (Gaussian head) is listed as 'next' in DESIGN.md; "
-                                      "the fused K4 loss covers the categorical policy of BASELINE configs 1-2")
         kw = dict(normalizer=self.normalize_fn, initializer=self.initializer, activation=self.activation,
                   device=self.device)
-        actor = CategoricalActorHead(feature_dim=rep.output_shapes['state'][0], hidden_size=self.config.actor_hidden_size,
-                                     action_dim=self.action_space.n, **kw)
+        if gaussian:
+            actor = GaussianActorHead(feature_dim=rep.output_shapes['state'][0],
+                                      hidden_size=self.config.actor_hidden_size, action_dim=self.action_space.shape[0],
+                                      activation_action=ActivationFunctions[self.config.activation_action], **kw)
+        else:
+            actor = CategoricalActorHead(feature_dim=rep.output_shapes['state'][0],
+                                         hidden_size=self.config.actor_hidden_size, action_dim=self.action_space.n, **kw)
         critic = ValueHead(feature_dim=rep.output_shapes['state'][0], hidden_size=self.config.critic_hidden_size, **kw)
         return SharedActorCritic(representation=rep, actor=actor, critic=critic).to(self.device)
+
+    @property
+    def _gaussian_policy(self):
+        """A Box action space (anything with ``low`` / ``high`` and a one-dimensional shape, gymnasium's included)."""
+        space = self.action_space
+        return hasattr(space, "low") and len(tuple(getattr(space, "shape", ()) or ())) == 1
 
     @property
     def auxiliary_info_shape(self):
@@ -46,8 +62,10 @@ class PPO_Agent(OnPolicyAgent):
             shape = tuple(space2shape(self.observation_space))
             dt = torch.uint8 if np.dtype(getattr(self.observation_space, "dtype", np.float32)) == np.uint8 \
                 else torch.float32
+            rb = ActionReadback(self.n_envs, self.device, torch.float32, self.action_space.shape) \
+                if self._gaussian_policy else ActionReadback(self.n_envs, self.device)
             self._dr = {"stage": torch.zeros((self.n_envs,) + shape, dtype=dt).pin_memory(),
-                        "readback": ActionReadback(self.n_envs, self.device),
+                        "readback": rb,
                         "rms": DeviceRunningMeanStd(shape, self.device) if self.use_obsnorm else None}
             if self.use_obsnorm:      # continue from whatever the host statistics hold (fresh, or a loaded checkpoint)
                 self._dr["rms"].load_state({'count': self.obs_rms.count, 'mean': self.obs_rms.mean,
@@ -78,13 +96,16 @@ class PPO_Agent(OnPolicyAgent):
         x = torch.as_tensor(np.ascontiguousarray(obs_host)).to(self.device)
         if dr["rms"] is not None:
             x = dr["rms"].normalize(x.float().contiguous(), self.obsnorm_range)
+        if self._gaussian_policy:
+            return self.model.forward_raw_gauss(x)[2].reshape(-1).cpu().numpy()
         return self.model.forward_raw(x)[1].reshape(-1).cpu().numpy()
 
     def _train_device(self, train_steps):
         """The loop of ``train`` with the per-step host work moved to the device: ONE upload of the observations (also
         the copy the buffer stores - the reference uploads them for the forward and stores a second host copy), K11
         running-statistics + normalise, the network, K10 sample + log-prob written into the buffer's K1 staging rows,
-        ONE read-back of N int32 actions, K1.  Episode bookkeeping (rewards, terminals, infos) stays on the host, where
+        ONE read-back of N int32 actions, K1 (a Box action space: K10G ``mu + sigma * noise`` + log-prob on torch's standard
+        normals, ONE read-back of N x D float32 actions).  Episode bookkeeping (rewards, terminals, infos) stays on the host, where
         the environments live.  Random stream: torch's device generator (``torch.rand``) - the reference's
         ``Categorical.sample`` stream cannot be reproduced by any fused kernel; distribution and log-prob are identical."""
         dr = self._device_rollout_state()
@@ -93,17 +114,25 @@ class PPO_Agent(OnPolicyAgent):
         stage_np[...] = self.train_envs.buf_obs
         slots = self.memory.policy_slots()
         N = self.n_envs
+        gaussian = self._gaussian_policy
         train_info = {}
         for _ in range(train_steps):
             obs_d = stage.to(self.device, non_blocking=True)
             obs_in = rms.update_and_normalize(obs_d, self.obsnorm_range) if rms is not None else obs_d
             with torch.no_grad():
-                logits, values = self.model.forward_raw(obs_in)
-                slots["values"].copy_(values.reshape(N))
-                act = categorical_act(logits, uniforms=torch.rand(N, device=self.device), actions_f32=slots["actions"],
-                                      actions_i32=rb.dev, logp=slots["aux:old_logp"])
+                if gaussian:    # K10G writes the [N, D] actions into the staging rows; one D2H of N*D float32
+                    mu, log_std, values = self.model.forward_raw_gauss(obs_in)
+                    slots["values"].copy_(values.reshape(N))
+                    act = gaussian_act(mu, log_std, noise=torch.randn(mu.shape, device=self.device),
+                                       actions_f32=slots["actions"], logp=slots["aux:old_logp"])
+                    rb.dev.copy_(slots["actions"])
+                else:
+                    logits, values = self.model.forward_raw(obs_in)
+                    slots["values"].copy_(values.reshape(N))
+                    act = categorical_act(logits, uniforms=torch.rand(N, device=self.device),
+                                          actions_f32=slots["actions"], actions_i32=rb.dev, logp=slots["aux:old_logp"])
             rb.launch()
-            acts = rb.wait().astype(np.int64)
+            acts = rb.wait().copy() if gaussian else rb.wait().astype(np.int64)
             next_obs, rewards, terminals, truncations, infos = self.train_envs.step(acts)
             self.callback.on_train_step(self.current_step, envs=self.train_envs, policy=self.model, obs=obs_in,
                                         policy_out=act, acts=acts, vals=slots["values"], next_obs=next_obs,

@@ -8,6 +8,7 @@ dvalue and the logged statistics) -> torch backward through the network into the
 import torch
 
 from ... import _lib
+from ..rl_models.heads import GaussianActorHead
 from ..utils import FusedAdam, allreduce_sum_
 from .learner import Learner
 
@@ -27,6 +28,9 @@ class PPO_Learner(Learner):
         self.clip_range = getattr(config, "clip_range", 0.0)
         self._stats = self.optimizer.bucket.tail[:8]      # the logged sums travel in the gradient bucket's tail
         self._scratch = _lib.scratch(self.device)
+        # a GaussianActorHead (Box action space) takes the K4G branch of _device_update
+        self._gaussian = isinstance(getattr(self.model, "actor", None), GaussianActorHead)
+        self._ws = None
         self._early = None
         self._hook_early_allreduce()
 
@@ -69,9 +73,37 @@ class PPO_Learner(Learner):
     def _f32(self, x):
         return torch.as_tensor(x, device=self.device).to(torch.float32).contiguous()
 
+    def _gauss_ws(self, D):
+        """K4G's column-partial workspace, allocated once at the size that fits any row count (D x 2048 doubles, at
+        most 1 MiB): captured graphs keep the pointer they were recorded with, so it is never reallocated."""
+        if self._ws is None:
+            need = int(_lib.load().xb_ppo_gauss_ws_doubles(1 << 40, D))
+            self._ws = torch.empty(need, dtype=torch.float64, device=self.device)
+        return self._ws
+
+    def _device_update_gauss(self, obs, act, ret, adv, old_logp):
+        """The Gaussian-policy branch: K4G gives (dmu, dlog_std, dvalue) and the statistics in one launch."""
+        mu, log_std, v_pred = self.model.forward_raw_gauss(obs)
+        mu_c, v_c = mu.contiguous(), v_pred.contiguous()
+        B, D = mu_c.shape
+        ls_c = log_std.detach().contiguous()
+        dmu, dvalue = torch.empty_like(mu_c), torch.empty_like(v_c)
+        dlog_std = torch.empty_like(ls_c)
+        ws = self._gauss_ws(D)
+        _lib.call("xb_ppo_gauss_loss_fwd_bwd", _lib.ptr(mu_c), _lib.ptr(ls_c), _lib.ptr(v_c), _lib.ptr(act),
+                  _lib.ptr(old_logp), _lib.ptr(adv), _lib.ptr(ret), B, D, B * self.world_size, float(self.clip_range),
+                  float(self.vf_coef), float(self.ent_coef), self.loss_kind, _lib.ptr(dmu), _lib.ptr(dlog_std),
+                  _lib.ptr(dvalue), _lib.ptr(self._stats), _lib.ptr(self._scratch), _lib.ptr(ws), ws.numel())
+        self.optimizer.zero_grad()
+        torch.autograd.backward([mu_c, v_c, log_std], [dmu, dvalue, dlog_std])
+
     def _device_update(self, obs, act, ret, adv, old_logp):
         """ppo_learner.py:43-65 on the device (no host synchronisation, static shapes: CUDA-graph capturable)."""
         B = act.shape[0]
+        if self._gaussian:
+            self._device_update_gauss(obs, act, ret, adv, old_logp)
+            self._reduce_and_step()
+            return
         if hasattr(self.model, "forward_raw"):
             logits, v_pred = self.model.forward_raw(obs)
         else:
@@ -88,6 +120,10 @@ class PPO_Learner(Learner):
                   _lib.ptr(self._scratch))
         self.optimizer.zero_grad()
         torch.autograd.backward([logits_c, v_c], [dlogits, dvalue])
+        self._reduce_and_step()
+
+    def _reduce_and_step(self):
+        """[one all-reduce of gradient + statistics] -> K7."""
         if self.world_size > 1:
             if self._early is not None:                      # the tail end of the bucket is already being reduced
                 off, work = self._early

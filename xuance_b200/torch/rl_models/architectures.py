@@ -46,6 +46,12 @@ class SharedActorCritic(nn.Module):
         z = self.representation(observation).embeddings
         return self.actor.logits(z), self.critic(z)
 
+    def forward_raw_gauss(self, observation):
+        """(mu, log_std, values) of a GaussianActorHead without building a torch.distributions object - the fused K4G
+        loss and K10G act consume these."""
+        z = self.representation(observation).embeddings
+        return self.actor.mu(z), self.actor.log_std, self.critic(z)
+
     def act(self, observation, deterministic=False, **kwargs):
         d = self.actor(self.representation(observation, **kwargs).embeddings, **kwargs)
         return d.deterministic_sample() if deterministic else d.stochastic_sample()

@@ -4,9 +4,12 @@ the host, as single launches that leave their results in HBM.
 * ``categorical_act``        - K10: sample / argmax / log-prob / entropy of a categorical policy from raw logits
                                (``OnPolicyAgent.get_actions``, core/on_policy.py:128-169 +
                                ``CategoricalDistribution``, modules/distributions.py:128-162).
+* ``gaussian_act``           - K10G: the same for a diagonal Gaussian policy from (mu, log_std) on supplied standard
+                               normals (``DiagGaussianDistribution``, modules/distributions.py:165-197).
 * ``DeviceRunningMeanStd``   - K11: ``RunningMeanStd.update`` + ``Agent._process_observation``
                                (common/statistic_tools.py:117-185, agents/base/agent.py:262-279) on device arrays.
-* ``ActionReadback``         - the one device->host transfer a vector-env step needs: N int32 actions into pinned memory.
+* ``ActionReadback``         - the one device->host transfer a vector-env step needs: N int32 actions (or N x D float32
+                               actions of a Box space) into pinned memory.
 """
 import numpy as np
 import torch
@@ -44,6 +47,36 @@ def categorical_act(logits, uniforms=None, forced_actions=None, actions_f32=None
               _lib.ptr(actions_i32) if actions_i32 is not None else None, _lib.ptr(logp),
               _lib.ptr(entropy) if entropy is not None else None)
     return {"actions": actions_f32, "actions_i32": actions_i32, "logp": logp, "entropy": entropy, "_keep": keep}
+
+
+def gaussian_act(mu, log_std, noise=None, forced_actions=None, actions_f32=None, logp=None, entropy=None):
+    """One K10G launch over ``mu [N, D]`` and ``log_std [D]`` (float32, CUDA).  Mode: ``forced_actions`` given -> log-prob
+    of those (no action written); else ``noise`` (standard normals [N, D]) given -> mu + exp(log_std) * noise; else mu.
+    Output tensors may be passed in (e.g. the rollout buffer's staging rows); missing ones among (actions_f32, logp) are
+    allocated.  Returns a dict."""
+    if not (mu.is_cuda and log_std.is_cuda):
+        raise RuntimeError("gaussian_act: mu and log_std must be CUDA tensors (no CPU fallback)")
+    mu = mu.detach().float().contiguous()
+    log_std = log_std.detach().float().contiguous()
+    N, D = mu.shape
+    if log_std.numel() != D:
+        raise ValueError("gaussian_act: log_std has %d entries, mu has %d columns" % (log_std.numel(), D))
+    dev = mu.device
+    if actions_f32 is None and forced_actions is None:
+        actions_f32 = torch.empty((N, D), dtype=torch.float32, device=dev)
+    if logp is None:
+        logp = torch.empty(N, dtype=torch.float32, device=dev)
+    keep = [mu, log_std]
+    if noise is not None:
+        noise = noise.to(device=dev, dtype=torch.float32).contiguous()
+        keep.append(noise)
+    if forced_actions is not None:
+        forced_actions = forced_actions.to(device=dev, dtype=torch.float32).contiguous()
+        keep.append(forced_actions)
+    _lib.call("xb_gaussian_act", _lib.ptr(mu), _lib.ptr(log_std), _lib.ptr(noise), _lib.ptr(forced_actions), N, D,
+              _lib.ptr(actions_f32), _lib.ptr(logp), _lib.ptr(entropy))
+    return {"actions": actions_f32 if forced_actions is None else forced_actions, "logp": logp, "entropy": entropy,
+            "_keep": keep}
 
 
 class DeviceRunningMeanStd:
@@ -104,11 +137,13 @@ class DeviceRunningMeanStd:
 
 class ActionReadback:
     """Double-buffered pinned block for the per-step actions: ``launch`` enqueues the D2H copy and records an event,
-    ``wait`` blocks on that event only (not on the whole device) and hands out the NumPy view."""
+    ``wait`` blocks on that event only (not on the whole device) and hands out the NumPy view.  The default block is
+    int32 [n_envs] (categorical actions); a Box policy passes ``dtype=torch.float32, shape=(D,)`` for [n_envs, D]."""
 
-    def __init__(self, n_envs, device):
-        self.dev = torch.zeros(n_envs, dtype=torch.int32, device=device)
-        self.host = [torch.zeros(n_envs, dtype=torch.int32).pin_memory() for _ in range(2)]
+    def __init__(self, n_envs, device, dtype=torch.int32, shape=()):
+        full = (n_envs,) + tuple(shape)
+        self.dev = torch.zeros(full, dtype=dtype, device=device)
+        self.host = [torch.zeros(full, dtype=dtype).pin_memory() for _ in range(2)]
         self.evt = [torch.cuda.Event(), torch.cuda.Event()]
         self.i = 0
 
