@@ -1,15 +1,21 @@
-"""Where the K12 warp roles wait (XB_K12_TIMING=1): per layer, mean over CTAs of the clock64 cycles each role spent in its
-barrier waits, as a share of the role's lifetime.  Run on a GPU box:  XB_K12_TIMING=1 python tools/k12_timing.py"""
-import ctypes, os, sys
-os.environ.setdefault("XB_K12_TIMING", "1")
+"""K12 on the GPU, two reports.
+
+    XB_K12_TIMING=1 python tools/k12_timing.py             where the warp roles wait (default mode)
+    XB_K12_TIMING=0 python tools/k12_timing.py --launches  CUDA-event time of every K12 launch of one encoder update
+
+Role timing: per layer, mean over CTAs of the clock64 cycles each role spent in its barrier waits, as a share of the
+role's lifetime.  Per-launch table: BoxNatureCNN's real plan at B = 8192 (XB_K12_BATCH), three planes, raw uint8 pixels,
+one forward + backward of conv1-3 and the 6400 -> 512 layer exactly as an update runs them; each launch gets its own label
+(conv3's forward and data gradient have the same GEMM shape), the median over the timed repetitions, and the executed
+bf16 TFLOP/s of tc_conv's FLOP log.  ``--json PATH`` also writes the table."""
+import argparse, ctypes, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import numpy as np, torch, torch.nn as nn
-from xuance_b200 import _lib
-from xuance_b200.torch.utils import tc_conv as tc
 DEV = "cuda:0"
 
 
 def report(label, fn):
+    import numpy as np, torch
+    from xuance_b200 import _lib
     for _ in range(2):
         fn()
     torch.cuda.synchronize()
@@ -25,7 +31,9 @@ def report(label, fn):
           % (label, m[0], 100 * m[1] / max(m[0], 1), 100 * m[3] / max(m[0], 1), 100 * m[5] / max(m[4], 1), 100 * m[6] / max(m[4], 1)))
 
 
-def main():
+def roles():
+    import torch, torch.nn as nn
+    from xuance_b200.torch.utils import tc_conv as tc
     B, Pn = int(os.environ.get("XB_K12_BATCH", "8192")), 3
     g = torch.Generator(device=DEV).manual_seed(0)
     convs = [nn.Conv2d(4, 32, 8, 4, padding=2).to(DEV), nn.Conv2d(32, 64, 4, 2, padding=1).to(DEV), nn.Conv2d(64, 64, 3, 1, padding=1).to(DEV)]
@@ -57,6 +65,79 @@ def main():
     xf, wf = rnd(Pn, B, 6400), rnd(Pn, 512, 6400)
     yf = torch.empty(Pn, B, 512, dtype=torch.bfloat16, device=DEV)
     report("Linear forward (TMA tiles)", lambda: tc.gemm_gather(xf, wf, tc.linear_geometry(B, 6400), relu=True, out_pl=yf))
+
+
+def launch_labels(tc, P):
+    """(ABI name, label) of every K12 launch of BoxNatureCNN.forward + backward, in launch order (tc_conv.py)."""
+    dg = "xb_gemm_halo_tc" if tc.HALO3 else "xb_gemm_box_tc"
+    wg = lambda box: "xb_wgrad_box_tc" if box else "xb_wgrad_gather_tc"
+    seq = [("xb_gemm_gather_tc", "conv1 forward"), ("xb_gemm_box_tc", "conv2 forward"), (dg, "conv3 forward"),
+           ("xb_gemm_gather_tc", "Linear forward"), ("xb_wgrad_gather_tc", "Linear weight gradient"),
+           ("xb_gemm_gather_tc", "Linear data gradient"), (wg(tc.BOX_WGRAD3), "conv3 weight gradient"),
+           (dg, "conv3 data gradient"), (wg(tc.BOX_WGRAD2), "conv2 weight gradient")]
+    if tc.HALO and P["h_dg2"] is not None:
+        seq.append(("xb_gemm_halo_tc", "conv2 data gradient"))
+    else:
+        seq += [("xb_gemm_box_tc", "conv2 data gradient, phase %d" % i) for i in range(len(P["dg2"]))]
+    return seq + [("xb_wgrad_gather_tc", "conv1 weight gradient")]
+
+
+def launches(reps, json_path):
+    import numpy as np, torch, torch.nn as nn
+    from xuance_b200 import _lib
+    from xuance_b200.torch.utils import tc_conv as tc
+    B = int(os.environ.get("XB_K12_BATCH", "8192"))
+    torch.manual_seed(0)
+    convs = [nn.Conv2d(4, 32, 8, 4, padding=2).to(DEV), nn.Conv2d(32, 64, 4, 2, padding=1).to(DEV), nn.Conv2d(64, 64, 3, 1, padding=1).to(DEV)]
+    fc = nn.Linear(6400, 512).to(DEV)
+    enc = tc.BoxNatureCNN(convs, fc, (84, 84, 4), backend=tc.CudaBackend(3))
+    P = enc._plan(B)
+    x = torch.randint(0, 256, (1, B, 84, 84, 4), device=DEV).to(torch.bfloat16)
+    dz = torch.randn(B, 512, device=DEV) * 1e-3
+    names = sorted({n for n, _ in launch_labels(tc, P)})
+
+    def update():
+        enc.forward(x, B)
+        enc.backward(dz)
+    update()
+    torch.cuda.synchronize()
+    times, log = [], None
+    for _ in range(reps):
+        _lib.profile, tc.flop_log = {n: [] for n in names}, []
+        update()
+        torch.cuda.synchronize()
+        prof, log = _lib.profile, tc.flop_log
+        _lib.profile, tc.flop_log = None, None
+        it = {n: iter(prof[n]) for n in names}
+        times.append([(lambda ab: ab[0].elapsed_time(ab[1]))(next(it[nm])) for nm, _, _, _ in log])
+    seq = launch_labels(tc, P)
+    assert [nm for nm, _, _, _ in log] == [n for n, _ in seq], ([nm for nm, *_ in log], seq)
+    ms = np.median(np.array(times), 0)
+    props = torch.cuda.get_device_properties(0)
+    rows = []
+    for (nm, label), (_, tag, fl, _), t in zip(seq, log, ms):
+        rows.append(dict(label=label, abi=nm, shape=tag, ms=float(t), tflops_executed=fl / (t * 1e-3) / 1e12))
+        print("%-34s %-20s %-40s %7.3f ms  %6.1f TFLOP/s" % (label, nm, tag, t, rows[-1]["tflops_executed"]))
+    total = float(ms.sum())
+    print("%-34s %69.3f ms  (B = %d, %s, XB_K12_HALO=%s XB_K12_BOX_WGRAD=%s)" % ("sum", total, B, props.name, tc.HALO_MODE, tc.BOX_WGRAD))
+    if json_path:
+        with open(json_path, "w") as fh:
+            json.dump(dict(device=props.name, batch=B, halo=tc.HALO_MODE, box_wgrad=tc.BOX_WGRAD, reps=reps, sum_ms=total,
+                           launches=rows), fh, indent=1)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--launches", action="store_true", help="per-launch CUDA-event table instead of the role timing")
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--json", default=None)
+    a = ap.parse_args()
+    if a.launches:
+        os.environ["XB_K12_TIMING"] = "0"        # the role clocks cost time inside the kernel
+        launches(a.reps, a.json)
+    else:
+        os.environ.setdefault("XB_K12_TIMING", "1")
+        roles()
 
 
 if __name__ == "__main__":

@@ -21,9 +21,11 @@
 //                            (cp.async.mbarrier.arrive.noinc).
 //                          One elected thread arms the barrier with the TMA byte count; no producer waits for a load.
 //   warps 0-7  consumers : two warpgroups, rows 0-63 and 64-127 of the tile (M = 64 per wgmma).  Per K step of 16 and A plane
-//                          pa, wgmmas of 64 / 32 columns multiply it with the first PB - pa B planes (adjacent in the stage =
-//                          ONE operand of (PB - pa) * N rows) into the register accumulator blocks of groups pa .. PB-1; a
-//                          stage is released when the wgmma group after it was issued has retired the one that read it.
+//                          pa, the A fragment is read ONCE into registers (ldmatrix) and wgmmas of 64 / 32 columns multiply
+//                          it with the first PB - pa B planes (adjacent in the stage = ONE operand of (PB - pa) * N rows, read
+//                          from shared memory) into the register accumulator blocks of groups pa .. PB-1; the wgmmas of a
+//                          chunk form one group, and its stage is released when that group has retired.
+//   Registers: setmaxnreg moves them from the producer warpgroup to the consumers (PROD_REGS / CONS_REGS).
 //                          The epilogue runs on the fragments: accumulator groups added smallest first, bias + ReLU /
 //                          ReLU-derivative mask, the rows written as fp32 and / or as the bf16 planes the next layer consumes
 //                          (into its padded layout), and the column sums of the tile (the bias-gradient partials of the layer
@@ -147,21 +149,29 @@ __device__ __forceinline__ void split3_bf16(float x, __nv_bfloat16 &hi, __nv_bfl
     lo = __float2bfloat16_rn(r1 - __bfloat162float(mid));
 }
 
-// A plane x the first PB - pa B planes for one K step: the accumulator blocks pa*NC .. PB*NC-1 (32 columns each).  Block j
-// reads B rows 32 (j - pa*NC) .. +31 of the stage: 4096 bytes per block in every operand layout the kernel uses (128 bytes
-// per row or per MN index).  In-flight wgmmas are ordered on their accumulator registers only when they have the same shape
-// and register set, so every block is always written by the same instruction form: pairs (2i, 2i+1) as one n64 wgmma when
-// NC is even (then every plane's range starts at an even block), single n32 wgmmas when NC is odd.
-template <int T, int PB, int NC, int PA_>
-__device__ __forceinline__ void mma_plane(float (&acc)[PB * NC][16], uint64_t da, uint64_t db, uint32_t scale_d) {
+// A plane (its fragment in registers) x the first PB - pa B planes for one K step: the accumulator blocks pa*NC .. PB*NC-1
+// (32 columns each).  Block j reads B rows 32 (j - pa*NC) .. +31 of the stage: 4096 bytes per block in every operand layout
+// the kernel uses (128 bytes per row or per MN index).  In-flight wgmmas are ordered on their accumulator registers only
+// when they have the same shape and register set, so every block is always written by the same instruction form: pairs
+// (2i, 2i+1) as one n64 wgmma when NC is even (then every plane's range starts at an even block), single n32 wgmmas when NC
+// is odd.
+template <int TB, int PB, int NC, int PA_>
+__device__ __forceinline__ void mma_plane(float (&acc)[PB * NC][16], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
     constexpr int J0 = PA_ * NC, J1 = PB * NC, STEP = NC % 2 == 0 ? 2 : 1;
 #pragma unroll
     for (int j = J0; j < J1; j += STEP) {
         const uint64_t b = db + (uint64_t)(((j - J0) * 4096) >> 4);
-        if (STEP == 2) wgmma_n64<T, T>(acc[j], acc[j + 1 < J1 ? j + 1 : j], da, b, scale_d);
-        else wgmma_n32<T, T>(acc[j], da, b, scale_d);
+        if (STEP == 2) wgmma_rs_n64<TB>(acc[j], acc[j + 1 < J1 ? j + 1 : j], a, b, scale_d);
+        else wgmma_rs_n32<TB>(acc[j], a, b, scale_d);
     }
 }
+
+// register split between the roles (setmaxnreg): 384 threads at the 168 registers one CTA per SM allows = 64512 per CTA;
+// the producer warpgroup gives back to PROD_REGS and the consumer warpgroups, which hold the accumulators and the double
+// buffered A fragments, take CONS_REGS: 2 * 128 * CONS_REGS + 128 * PROD_REGS must not exceed 128 * 3 * 168, or the
+// consumers' setmaxnreg.inc would wait for registers that never come free
+constexpr int LAUNCH_REGS = 168, PROD_REGS = 104, CONS_REGS = 200;
+static_assert(2 * CONS_REGS + PROD_REGS <= 3 * LAUNCH_REGS && THREADS == 3 * 128, "register split");
 
 // WGRAD = false:  D[site, n]  = sum_k A[site, k] W[n, k]            work item = (128-site tile, n tile),        K-major operands
 // WGRAD = true :  D[kcol, n]  = sum_site A[site, kcol] G[site, n]   work item = (128-kcol tile, n tile, split), MN-major operands
@@ -252,6 +262,7 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
 
     if (warp >= CONS_WARPS) {
         // ------------------------------------------------------------------ producers (128 threads)
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PROD_REGS));
         const int ptb = tid - CONS_WARPS * 32;
         uint32_t it = 0, tile_it = 0;
         if (!(halo && ptb != 0))                               // halo: both operands by TMA, one thread drives them
@@ -359,25 +370,40 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
         }
     } else {
         // ------------------------------------------------------------------ consumers: wgmma issue + epilogue
-        //  A: halo     128-byte swizzle K-major window of the resident tile, K step 32 B, planes halo_plane apart
-        //     cp.async no-swizzle canonical layout (conv_index.h), K step = two core matrices = 256 B
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONS_REGS));
+        //  A (read into registers with ldmatrix, one x4 per K step of 16 and plane; warpgroup wg reads rows 64 wg .. +63):
+        //     halo     128-byte swizzle K-major window of the resident tile, planes halo_plane apart
+        //     cp.async no-swizzle canonical layout (conv_index.h): K-major forward, MN-major weight gradient, K step = two
+        //              core matrices = 256 B, planes a_plane apart
         //     TMA      128-byte swizzle.  K-major: rows of 128 B, K step 32 B.  MN-major (weight gradient): two blocks of 64
         //              columns, each [planes][64 sites][128 B]: plane stride a_plane/2, block stride PA*a_plane/2, K step 2048 B
         //  B: the first (PB - pa) planes, adjacent in the stage, are ONE operand of (PB - pa) * N rows (same three layouts;
-        //     MN-major: one 64-column block per plane, blocks w_plane apart)
-        // A descriptor = per-launch template (layout, LBO, SBO) + start address in 16-byte units; warpgroup wg reads rows
-        // 64 wg .. 64 wg + 63 of the tile: 8192 bytes further in every layout but the MN-major TMA tile (the next 64-column block)
+        //     MN-major: one 64-column block per plane, blocks w_plane apart); descriptor = per-launch template (layout, LBO,
+        //     SBO) + start address in 16-byte units
         const int wg = warp >> 2;
-        uint64_t a_tmpl, b_tmpl;
-        uint32_t a_ks, a_pl, b_ks, a_wg;                     // steps in 16-byte units: per K step of 16, per A plane; bytes per warpgroup
-        if (halo) a_tmpl = make_desc_sw128(0, 16, 1024), a_ks = 32 >> 4, a_pl = halo_plane >> 4;
-        else if (!p.a_tma) a_tmpl = make_desc(0, KC), a_ks = 256 >> 4, a_pl = a_plane >> 4;
-        else if (!WGRAD) a_tmpl = make_desc_sw128(0, 16, 1024), a_ks = 32 >> 4, a_pl = a_plane >> 4;
-        else a_tmpl = make_desc_sw128(0, PA * (a_plane / 2), 1024), a_ks = 2048 >> 4, a_pl = (a_plane / 2) >> 4;
-        a_wg = (WGRAD && p.a_tma) ? (uint32_t)wg * PA * (a_plane / 2) : (uint32_t)wg * 8192u;
+        uint64_t b_tmpl;
+        uint32_t b_ks;                                       // per K step of 16, in 16-byte units
         if (!p.b_tma) b_tmpl = make_desc(0, KC), b_ks = 256 >> 4;
         else if (!WGRAD) b_tmpl = make_desc_sw128(0, 16, 1024), b_ks = 32 >> 4;
         else b_tmpl = make_desc_sw128(0, w_plane, 1024), b_ks = 2048 >> 4;
+        // this lane's ldmatrix row: matrix mi = lane / 8 of the x4 holds rows (m) + 8 (mi & 1), K columns + 8 (mi >> 1) of
+        // the warp's 16 x 16 fragment; lane & 7 is its row of that 8 x 8 matrix (an m row K-major, a k row MN-major)
+        const int mi = lane >> 3, lr = lane & 7, m_l = 16 * (warp & 3) + 8 * (mi & 1);
+        // a_lane: byte offset of the lane's 16-byte row at K step 0 from the stage's A base, a_ks: per K step (linear
+        // layouts), a_pl: per plane (multiples of 1024 B: the swizzle phase is the same for every plane)
+        const bool a_sw_k = !WGRAD && (halo || p.a_tma);     // 128-byte swizzle, K-major: the K step is an XOR on the 16-byte unit
+        uint32_t a_lane, a_ks, a_pl;
+        if (!WGRAD) {
+            if (a_sw_k) a_lane = (uint32_t)wg * 8192u + (uint32_t)(m_l + lr) * 128u, a_ks = 0, a_pl = halo ? halo_plane : a_plane;
+            else a_lane = (uint32_t)wg * 8192u + (uint32_t)((m_l + lr) >> 3) * 1024u + (uint32_t)(mi >> 1) * 128u + lr * 16u,
+                 a_ks = 256, a_pl = a_plane;
+        } else if (p.a_tma) {
+            a_lane = (uint32_t)wg * PA * (a_plane / 2) + (uint32_t)(8 * (mi >> 1) + lr) * 128u + (uint32_t)(((m_l >> 3) ^ lr) << 4);
+            a_ks = 2048, a_pl = a_plane / 2;
+        } else {
+            a_lane = (uint32_t)wg * 8192u + (uint32_t)(m_l >> 3) * 1024u + (uint32_t)(mi >> 1) * 128u + lr * 16u;
+            a_ks = 256, a_pl = a_plane;
+        }
         // this thread's two rows of the tile and the first column of each 8-column block of its fragments
         const int rbase = 64 * wg + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
         float acc[PB * NC][16];
@@ -404,41 +430,44 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
                 for (int i = tid; i < N; i += CONS_WARPS * 32) s_bias[i] = p.bias ? p.bias[ncol * N + i] : 0.f;
             }
             uint32_t scale_d = 0;
-            int prev_stage = -1;
+            uint32_t af[KC / 16][PA][4];                      // A fragments of a chunk, one register set per K step and plane
             for (int kc = 0; kc < n_chunks; ++kc) {
                 const int stage = (int)(it % (uint32_t)S);
                 timed_wait(&full_bar[stage], (it / (uint32_t)S) & 1u, 0);
                 fence_proxy_async();       // the stage was written by cp.async (generic proxy); the MMA reads it through the async proxy
                 const uint32_t base = smem_base + ring_off + (uint32_t)stage * stage_bytes;
                 const uint32_t w_addr = base + (halo ? 0u : PA * a_plane);
-                const uint32_t a_addr = a_wg + (halo ? halo_base + (uint32_t)(halo_s0 + p.halo_shift[sub * p.halo_chunks + kc]) * 128u : base);
+                const uint32_t a_row = a_lane + (halo ? halo_base + (uint32_t)(halo_s0 + p.halo_shift[sub * p.halo_chunks + kc]) * 128u : base);
+                // the 128-byte swizzle XORs the 16-byte unit with bits 7-9 of the ABSOLUTE address, as TMA wrote it (a halo
+                // window starts at any 128-byte row of its 1024-byte-aligned tile)
+                const uint32_t a_sw = (a_row >> 7) & 7u;
                 // start addresses stay below 2^18 bytes: adding 16-byte units to the template never carries out of the field
-                const uint64_t a0 = a_tmpl + (uint64_t)(a_addr >> 4), b0 = b_tmpl + (uint64_t)(w_addr >> 4);
+                const uint64_t b0 = b_tmpl + (uint64_t)(w_addr >> 4);
+                // every fragment of the chunk is loaded while no wgmma is in flight: registers a pending wgmma reads are
+                // never redefined (otherwise ptxas serialises every wgmma of the kernel)
+#pragma unroll
+                for (int ks = 0; ks < KC / 16; ++ks) {
+                    const uint32_t a_addr = a_sw_k ? a_row + (((uint32_t)(2 * ks + (mi >> 1))) ^ a_sw) * 16u : a_row + (uint32_t)ks * a_ks;
+#pragma unroll
+                    for (int q = 0; q < PA; ++q) ldmatrix_x4<TR>(af[ks][q], a_addr + (uint32_t)q * a_pl);
+                }
                 wgmma_fence();
 #pragma unroll
                 for (int ks = 0; ks < KC / 16; ++ks) {
                     // A plane pa x B planes 0 .. PB-1-pa -> accumulator groups pa .. PB-1.
                     // pa = 0 covers every group, so its first instruction of a work item (scale_d = 0) initialises them all.
-                    const uint64_t da = a0 + (uint64_t)(ks * a_ks), db = b0 + (uint64_t)(ks * b_ks);
-                    mma_plane<TR, PB, NC, 0>(acc, da, db, scale_d);
-                    if (PA > 1) mma_plane<TR, PB, NC, (PA > 1 ? 1 : 0)>(acc, da + a_pl, db, 1u);
-                    if (PA > 2) mma_plane<TR, PB, NC, (PA > 2 ? 2 : 0)>(acc, da + 2 * a_pl, db, 1u);
+                    const uint64_t db = b0 + (uint64_t)(ks * b_ks);
+                    mma_plane<TR, PB, NC, 0>(acc, af[ks][0], db, scale_d);
+                    if (PA > 1) mma_plane<TR, PB, NC, (PA > 1 ? 1 : 0)>(acc, af[ks][PA > 1 ? 1 : 0], db, 1u);
+                    if (PA > 2) mma_plane<TR, PB, NC, (PA > 2 ? 2 : 0)>(acc, af[ks][PA > 2 ? 2 : 0], db, 1u);
                     scale_d = 1;
                 }
                 wgmma_commit();
-                // the group before this one has retired: its stage is free
-                wgmma_wait<1>();
-                if (prev_stage >= 0) {
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-                }
-                prev_stage = stage;
-                ++it;
-            }
-            wgmma_wait<0>();
-            if (prev_stage >= 0) {
+                wgmma_wait<0>();
+                // every wgmma that read the stage has retired: it is free
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+                if (lane == 0) mbar_arrive(&empty_bar[stage]);
+                ++it;
             }
             if (!WGRAD) asm volatile("bar.sync 1, %0;" ::"n"(CONS_WARPS * 32) : "memory");     // s_bias written
             // ---- epilogue on the fragments: rows rbase (h = 0) and rbase + 8 (h = 1)

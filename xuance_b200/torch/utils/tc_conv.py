@@ -471,14 +471,15 @@ class BoxGeometry:
 
 _BOXTAB = {}
 import os as _os
-# weight gradients with both operands as TMA boxes, per layer (measured at B = 8192, 3 planes: conv3 785 us box vs 837 us
-# gathered; conv2 947 us box vs 851 us gathered - its 16 pixel-pair chunks re-read G once per pair of chunks)
+# weight gradients with both operands as TMA boxes, per layer (tools/k12_timing.py --launches, B = 8192, 3 planes, H100 80GB
+# HBM3 at a 400 W power limit: conv3 1.12 ms box vs 1.58 ms gathered; conv2 1.50 ms box vs 1.57 ms gathered - about 1 % of
+# bench.py's step, but the box path sums conv2's sites in another order, so "23" does not reproduce the "3" results bit for bit)
 BOX_WGRAD = _os.environ.get("XB_K12_BOX_WGRAD", "3")
 BOX_WGRAD2, BOX_WGRAD3 = "2" in BOX_WGRAD, "3" in BOX_WGRAD
 # xb_gemm_halo_tc (activation tile resident in shared memory, taps = descriptor offsets): "2" = conv2's data gradient (its
-# four stride phases become ONE launch: 868 us vs 892 us as four box launches at B = 8192), "3" = also conv3 forward / data
-# gradient (473 / 479 us vs 461 / 469 us as box launches: no gain - with 64-column tiles the tensor pipe waits for its own
-# shared-memory operand reads, not for the fill of the ring, see DESIGN.md section 3a), "0" = box launches only
+# four stride phases become ONE launch: 2.2-2.5 ms vs 2.59 ms as four box launches, same card and settings as above), "3" =
+# also conv3 forward / data gradient (1.07 / 1.36 ms vs 1.09 / 1.25 ms as box launches: no gain - the consumers of the box
+# launches wait on the ring for under 5 % of their time, see DESIGN.md section 3a), "0" = box launches only
 HALO_MODE = _os.environ.get("XB_K12_HALO", "2")
 HALO, HALO3 = HALO_MODE != "0", HALO_MODE in ("1", "3")
 
