@@ -64,6 +64,24 @@ int xb_gae_scan(const float *rew, const float *val, const float *term,
                 const uint8_t *seg_end, const float *bootstrap, const int32_t *covered,
                 float *adv, float *ret, int N, int T, float gamma, float lam, int use_gae, void *stream);
 
+/* K2 for the multi-agent on-policy buffer (MARL_OnPolicyBuffer.finish_path, memory_tools_marl.py:208-236): rows are
+ * (env, agent) pairs, [N,T] fields as for xb_gae_scan, start[N] / covered[N] (int32, nullable = 0 / T): only steps in
+ * [start, covered) are written.  With a ValueNorm state (running_mean, running_mean_sq, debiasing_term: device
+ * scalars, all or none) the stored values and, for use_gae, the bootstrap are denormalised with the state as it is
+ * when the kernel runs (float32, value_norm.py:65-75); without one they are used as stored.
+ *   use_gae=1: delta_t = r_t + (1-d_t)*gamma*V'_{t+1} - V'_t; A_t = delta_t + (1-d_t)*gamma*lam*A_{t+1} in float64
+ *              (warp scan of affine maps), ret_t = float32(A_t + V'_t)
+ *   use_gae=0: ret_t = float32(r_t + (1-d_t)*gamma*ret_{t+1}) step by step, ret at the segment end's successor = the
+ *              raw bootstrap
+ *   both:      adv_t = ret_t - V'_t in float32.
+ * Every path is float32 as above.  The reference computes a path whose bootstrap is the Python float 0.0 (a terminal
+ * step) in float64 (np.append promotes it): its non-GAE returns are not rounded step by step and its advantages
+ * denormalise in float64 - a few ulp from this (DESIGN.md section 4). */
+int xb_gae_scan_vn(const float *rew, const float *val, const float *term, const uint8_t *seg_end, const float *bootstrap,
+                   const int32_t *start, const int32_t *covered, float *adv, float *ret, int N, int T, double gamma,
+                   double lam, int use_gae, const float *running_mean, const float *running_mean_sq,
+                   const float *debiasing_term, void *stream);
+
 /* ---------------------------------------------------------------- K3: minibatch gather ---------------
  * Replaces sample_batch(): `memory[(env_idx, step_idx)]` (memory_tools.py:64-84) as used by
  * DummyOnPolicyBuffer.sample :267-287 and the replay buffers' sample().  idx[B] are flat slots (env*T+step);
@@ -120,6 +138,38 @@ int xb_ppo_gauss_loss_fwd_bwd(const float *mu, const float *log_std, const float
                               int64_t B_total, float clip_range, float vf_coef, float ent_coef, int loss_kind,
                               float *dmu, float *dlog_std, float *dvalue, float *stats, double *scratch, double *ws,
                               int64_t ws_doubles, void *stream);
+
+/* ---------------------------------------------------------------- K4M: fused MAPPO loss fwd+bwd -------
+ * Replaces mappo_learner.py:55-113 (one parameter-sharing group, feed-forward actor and critic, Discrete actions) plus
+ * the autograd backward of those lines down to (logits, value).  One row = one agent at one env step.
+ * xb_mappo_prepare    : block[4] (float64) = {sum mask, sum ret, sum ret^2, 0} over the R local rows (deterministic
+ *                       two-level reduction); SUM-all-reduce it when the minibatch is sharded.
+ * xb_value_norm_update: ValueNorm.update + running_mean_var (xuance/torch/utils/value_norm.py:29-52) in float32, in
+ *                       torch's operation order: x <- x*beta + m*(1-beta) for running_mean / running_mean_sq with the
+ *                       batch moments m = block[1] / R_total, block[2] / R_total (float64 quotients rounded to float32),
+ *                       debiasing_term <- d*beta + (1-beta); mean = rm / max(d, 1e-5), var = max(rmsq / max(d, 1e-5) -
+ *                       mean^2, 1e-2); writes the state in place and mean_std[2] = {mean, sqrt(var)}.  One thread.
+ * xb_mappo_loss_fwd_bwd: logits[R,A] with avail[R, avail_ld] (uint8, nullable; 0 = unavailable: the logit counts as
+ *                       -1e10 and its gradient is exactly 0, actor_head.py:40); M = prep[0] is the GLOBAL sum of the
+ *                       agent mask:
+ *     a_loss = -sum(min(ratio*adv, clip(ratio, 1-eps, 1+eps)*adv) * mask) / M       (K4's tie and clamp rules)
+ *     target = vn ? (ret - vn[0]) / vn[1] : ret                                        (vn: mean_std, nullable)
+ *     L(d)   = huber_delta > 0 ? HuberLoss(delta)(d) : d^2
+ *     value_clip_range > 0: lc = max(L(v - target), L(v_old + clamp(v - v_old, -c, c) - target))  (ties split 1/2,
+ *                           clamp inclusive);  else lc = L(v - target)
+ *     c_loss = sum(lc * mask) / M;  e = sum(H * mask) / M;  loss = a_loss + vf_coef*c_loss - ent_coef*e
+ * Writes dlogits[R,A], dvalue[R] and stats[8] = {a_loss, c_loss, e, predict_value = sum(v) / R_total (unmasked, as the
+ * reference logs it), loss, 0, 0, 0}, each the local rows' share (a SUM all-reduce of the shards gives the global
+ * value).  M = 0 gives 0/0 = NaN statistics and gradients, as in the reference.  actions are float32; A <= 64 (else
+ * XB_ERANGE); old_value may be NULL when value_clip_range <= 0.  scratch as for K4. */
+int xb_mappo_prepare(const float *mask, const float *ret, int64_t R, double *block, double *scratch, void *stream);
+int xb_value_norm_update(float *running_mean, float *running_mean_sq, float *debiasing_term, const double *block,
+                         int64_t R_total, double beta, float *mean_std, void *stream);
+int xb_mappo_loss_fwd_bwd(const float *logits, const uint8_t *avail, int avail_ld, const float *actions,
+                          const float *old_logp, const float *adv, const float *value, const float *old_value,
+                          const float *ret, const float *mask, const float *vn, const double *prep, int64_t R, int A,
+                          int64_t R_total, float clip_range, float value_clip_range, float huber_delta, float vf_coef,
+                          float ent_coef, float *dlogits, float *dvalue, float *stats, double *scratch, void *stream);
 
 /* ---------------------------------------------------------------- K5: prioritized-replay trees -------
  * Replaces SumSegmentTree/MinSegmentTree (xuance/common/segtree_tool.py:4-220) and their use in

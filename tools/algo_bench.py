@@ -2,7 +2,8 @@
 """Secondary measurements for BASELINE configs 3-5 (parity-test cases, not the headline): sample + update throughput of
 DQN+PER (2^20-transition HBM replay, B=512), SAC (1M replay, B=1024) and QMIX (5 agents x 72-d, T=60, 32 episodes)
 on one GPU, next to the oracle port of the reference's torch-CPU path on the host; and ``ppo_gauss``, continuous-control
-PPO in the shape of the reference's ppo/mujoco.yaml (train_epochs env-steps/s).  Prints one JSON object.
+PPO in the shape of the reference's ppo/mujoco.yaml (train_epochs env-steps/s); ``mappo``, MAPPO in the shape of
+configs/mappo/sc2/5m_vs_6m.yaml (train_epochs env-steps/s).  Prints one JSON object.
 
     python tools/algo_bench.py [--iters 200] [--cpu-iters 5] [--no-cpu] [--graph]
     torchrun --nnodes=1 --nproc-per-node G --master-addr 127.0.0.1 tools/algo_bench.py --no-cpu --graph    (G GPUs)
@@ -230,6 +231,61 @@ def bench_ppo_gauss(args):
     return out
 
 
+def bench_mappo(args):
+    """MAPPO in the shape of configs/mappo/sc2/5m_vs_6m.yaml (feed-forward; SMAC 5m_vs_6m shape: 5 agents, 72-d obs, 12
+    actions with masks): 8 envs x 128 steps x 5 agents = 5120 rows per update, 10 epochs x 1 minibatch.  The measured
+    unit is ``train_epochs`` over one stored rollout (the buffer is kept between repetitions); env-steps/s = 1024 / its
+    time.  The LayerNorm of the config is left out on both sides (the CPU oracle's MLPs have none)."""
+    from xuance_b200.common import Box, Discrete
+    from xuance_b200.common.common_tools import get_arguments
+    from xuance_b200.torch.agents import MAPPO_Agents
+    N, T, n, od, A, epochs = 8, 128, 5, 72, 12, 10
+    cfg = get_arguments("mappo", "sc2", config_path=os.path.join(ROOT, "xuance_b200", "configs", "mappo", "sc2",
+                                                                  "5m_vs_6m.yaml"))
+    for k, v in dict(device=DEV, parallels=N, buffer_size=N * T, n_epochs=epochs, n_minibatch=1, logger=None,
+                     model_dir="/tmp/x", use_cuda_graph=args.graph, distributed_training=False).items():
+        setattr(cfg, k, v)
+    del cfg.normalize
+    keys = ["agent_%d" % i for i in range(n)]
+    agent = MAPPO_Agents(cfg, None, n, keys, None, {k: Box(-1, 1, (od,), np.float32) for k in keys},
+                         {k: Discrete(A) for k in keys})
+    rng = np.random.default_rng(0)
+    for t in range(T):
+        avail = {k: (rng.random((N, A)) > 0.3).astype(np.int64) for k in keys}
+        for k in keys:
+            avail[k][:, 0] = 1
+        agent.memory.store(obs={k: rng.uniform(-1, 1, (N, od)).astype(np.float32) for k in keys},
+                           actions={k: np.zeros(N, np.float32) for k in keys},
+                           log_pi_old={k: np.full(N, -2.3, np.float32) for k in keys},
+                           rewards={k: rng.random(N).astype(np.float32) for k in keys},
+                           values={k: rng.normal(size=N).astype(np.float32) for k in keys},
+                           terminals={k: rng.random(N) < 0.01 for k in keys},
+                           agent_mask={k: rng.random(N) > 0.05 for k in keys}, avail_actions=avail)
+    for i in range(N):
+        agent.memory.finish_path(i, agent.agent_grouping, {k: np.float32(0.1) for k in keys},
+                                 agent.learner.value_normalizer)
+    agent.memory.clear = lambda: None          # keep the stored rollout for every repetition
+    iters = max(2, args.iters // 40)
+    dt = timed(lambda: agent.train_epochs(epochs), iters, warm=1)
+    R = N * T * n
+    out = {"config": "MAPPO 5m_vs_6m shape (5 agents, 72-d obs, 12 masked actions), 8 envs x 128 steps, 10 epochs x 1 "
+                     "minibatch of 5120 rows, Basic_MLP 64 + actor / critic MLP 64-64, value clip + ValueNorm + Huber",
+           "gpu_env_steps_per_s": N * T / dt, "gpu_ms_per_train_epochs": dt * 1e3, "gpu_ms_per_update": dt * 1e3 / epochs}
+    if not args.no_cpu:
+        from oracle_mappo import MAPPOModelOracle, MAPPOLearnerOracle
+        ol = MAPPOLearnerOracle(MAPPOModelOracle(od, A, (64,), (64, 64), (64, 64)), cfg)
+        av = torch.from_numpy(rng.random((R, A)) > 0.3)
+        av[:, 0] = True
+        b = [torch.from_numpy(x) for x in (rng.uniform(-1, 1, (R, od)).astype(np.float32), np.zeros(R, np.float32),
+                                           np.full(R, -2.3, np.float32), rng.normal(size=R).astype(np.float32),
+                                           rng.normal(size=R).astype(np.float32), rng.normal(size=R).astype(np.float32),
+                                           (rng.random(R) > 0.05).astype(np.float32))]
+        cdt = cpu_timed(lambda: ol.update(*b, av), max(args.cpu_iters, 10))
+        out.update(cpu_ms_per_update=cdt * 1e3, cpu_env_steps_per_s=N * T / (cdt * epochs),
+                   cpu_threads=torch.get_num_threads(), speedup=cdt * epochs / dt)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=200)
@@ -259,6 +315,8 @@ def main():
         res["qmix_4096"] = bench_qmix(Namespace(**{**vars(args), "iters": 20, "no_cpu": True}), Be=1024)
     if (not only and WORLD == 1) or "ppo_gauss" in only:
         res["ppo_gauss"] = bench_ppo_gauss(args)
+    if (not only and WORLD == 1) or "mappo" in only:
+        res["mappo"] = bench_mappo(args)
     res["cuda_graph"] = bool(args.graph)
     res["n_gpus"] = WORLD
     if RANK == 0:

@@ -23,6 +23,8 @@ _SIGNATURES = {
     "xb_device_info": (c_int, [POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     "xb_rollout_store": (c_int, [_P, _P, c_int64, _P, _P, c_int, c_int, c_int, c_int, _P]),
     "xb_gae_scan": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_float, c_float, c_int, _P]),
+    "xb_gae_scan_vn": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_double, c_double, c_int, _P, _P,
+                                _P, _P]),
     "xb_gather_rows": (c_int, [_P, _P, c_int64, c_int64, _P, _P]),
     "xb_gather_obs": (c_int, [_P, _P, c_int64, c_int, c_int, c_int, _P, c_int, _P]),
     "xb_scratch_doubles": (c_int64, []),
@@ -33,6 +35,10 @@ _SIGNATURES = {
     "xb_ppo_gauss_ws_doubles": (c_int64, [c_int64, c_int]),
     "xb_ppo_gauss_loss_fwd_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int64, c_int, c_int64, c_float, c_float,
                                           c_float, c_int, _P, _P, _P, _P, _P, _P, c_int64, _P]),
+    "xb_mappo_prepare": (c_int, [_P, _P, c_int64, _P, _P, _P]),
+    "xb_value_norm_update": (c_int, [_P, _P, _P, _P, c_int64, c_double, _P, _P]),
+    "xb_mappo_loss_fwd_bwd": (c_int, [_P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, c_int64,
+                                      c_float, c_float, c_float, c_float, c_float, _P, _P, _P, _P, _P]),
     "xb_per_insert": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_float, _P]),
     "xb_per_sample": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int64, c_float, _P, _P, _P, _P]),
     "xb_per_update": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, _P]),

@@ -7,7 +7,9 @@ vector env loop - while the replay ring (``data``) lives in HBM, agent-stacked `
 so that one K1 row-store per field ingests a finished episode and one K3 row-gather per field builds a batch
 already in the ``[B, n_agents, T(+1), dim]`` layout the learner consumes (the reference re-stacks per-agent
 dicts on every update, marl_learner.py:336-394).  ``sample()`` returns per-agent views of those stacked tensors
-under the reference's keys, plus the stacked tensors themselves under ``'_stacked'``."""
+under the reference's keys, plus the stacked tensors themselves under ``'_stacked'``.
+
+``MARL_OnPolicyBuffer`` mirrors memory_tools_marl.py:63-270 for feed-forward MAPPO (see its docstring)."""
 import numpy as np
 import torch
 
@@ -171,3 +173,209 @@ class MARL_OffPolicyBuffer_RNN:
         out['sequence_length'] = T
         out['_stacked'] = st
         return out
+
+
+class MARL_OnPolicyBuffer:
+    """On-policy multi-agent rollout - mirror of MARL_OnPolicyBuffer (xuance/common/memory_tools_marl.py:63-270):
+    ``store(**step_data)``, ``finish_path(i_env, agent_grouping, value_next, value_normalizer)``, ``sample(indexes)``,
+    ``clear``, ``full``, ``ptr / size / start_ids``, same constructor arguments and sample keys.
+
+    The rollout lives in HBM.  Rows are (env, agent) pairs, row = env * n_agents + agent, so the scalar fields
+    ``[F, n_envs * n_agents, n_size]`` are K2's layout with the agents as extra envs, and one K1 launch stores a vector
+    step.  ``finish_path`` runs ``xb_gae_scan_vn`` over the finished env's rows at once, denormalising with the
+    ValueNorm state as it is at that moment (the reference's per-step Python loop, :208-236).  ``sample`` gathers the
+    minibatch agent-major (row k * B + b is agent k of sample b) with K3 and normalises the advantages per agent over
+    the minibatch, as the reference does per agent key (:255-258)."""
+    FIELDS = ('actions', 'rewards', 'values', 'log_pi_old', 'terminals', 'agent_mask', 'returns', 'advantages')
+    STORED = 6   # the fields store() writes; returns / advantages come from finish_path
+
+    def __init__(self, agent_keys, state_space=None, obs_space=None, act_space=None, n_envs=1, buffer_size=1,
+                 use_gae=False, use_advnorm=False, gamma=None, gae_lam=None, device="cuda:0", **kwargs):
+        assert buffer_size % n_envs == 0, "buffer_size must be divisible by the number of envs (parallels)"
+        self.agent_keys = list(agent_keys)
+        self.n_agents = len(self.agent_keys)
+        self.n_envs, self.buffer_size = n_envs, buffer_size
+        self.n_size = buffer_size // n_envs
+        self.state_space = state_space
+        self.store_global_state = state_space is not None
+        self.use_actions_mask = kwargs.get("use_actions_mask", False)
+        self.avail_actions_shape = kwargs.get("avail_actions_shape", None)
+        self.use_gae, self.use_advantage_norm = use_gae, use_advnorm
+        self.gamma, self.gae_lambda = gamma, gae_lam
+        k0 = self.agent_keys[0]
+        obs_shape = {k: tuple(space2shape(obs_space[k])) for k in self.agent_keys}
+        act_shape = {k: tuple(space2shape(act_space[k])) for k in self.agent_keys}
+        if any(obs_shape[k] != obs_shape[k0] or act_shape[k] != act_shape[k0] for k in self.agent_keys):
+            raise NotImplementedError("heterogeneous agents are outside the hot-path scope (one parameter-sharing group)")
+        if act_shape[k0] != ():
+            raise NotImplementedError("MARL_OnPolicyBuffer: Box action spaces (Gaussian MAPPO) are not supported")
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise RuntimeError("xuance_b200 buffers are device-resident: device must be CUDA (no CPU fallback)")
+        _lib.load()
+        _lib.use_device(self.device)
+        self._obs_dim = int(np.prod(obs_shape[k0]))
+        self._state_dim = int(np.prod(space2shape(state_space))) if self.store_global_state else 0
+        self._n_act = int(self.avail_actions_shape[k0][0]) if self.use_actions_mask else 0
+        self._rows = self.n_envs * self.n_agents
+        self._scratch = _lib.scratch(self.device)
+        self.clear()
+
+    @property
+    def data_keys(self):
+        keys = ['obs'] + list(self.FIELDS)
+        if self.store_global_state:
+            keys.append('state')
+        if self.use_actions_mask:
+            keys.append('avail_actions')
+        return keys
+
+    @property
+    def full(self):
+        return self.size >= self.n_size
+
+    def clear(self):
+        R, T, dev = self._rows, self.n_size, self.device
+        self._scal = torch.zeros((len(self.FIELDS), R, T), dtype=torch.float32, device=dev)
+        self._obs = torch.zeros((R, T, self._obs_dim), dtype=torch.float32, device=dev)
+        self._avail = (torch.zeros((R, T, _pad4(self._n_act)), dtype=torch.uint8, device=dev)
+                       if self.use_actions_mask else None)
+        self._state = (torch.zeros((self.n_envs, T, self._state_dim), dtype=torch.float32, device=dev)
+                       if self.store_global_state else None)
+        self._seg_end = np.zeros((R, T), np.uint8)
+        self._boot = np.zeros((R, T), np.float32)
+        self._seg_end_d = torch.zeros((R, T), dtype=torch.uint8, device=dev)
+        self._boot_d = torch.zeros((R, T), dtype=torch.float32, device=dev)
+        self._start_d = torch.zeros(R, dtype=torch.int32, device=dev)
+        self._cov_d = torch.zeros(R, dtype=torch.int32, device=dev)
+        self.ptr, self.size = 0, 0
+        self.start_ids = np.zeros(self.n_envs, np.int64)
+
+    def field(self, name):
+        """[n_envs * n_agents, n_size] device view of a scalar field (row = env * n_agents + agent)."""
+        return self._scal[self.FIELDS.index(name)]
+
+    def _per_agent(self, d, dtype=np.float32):
+        """{agent: [n_envs, ...]} -> [n_envs * n_agents, ...] (env-major, agent-minor)."""
+        return np.stack([np.asarray(d[k], dtype=dtype) for k in self.agent_keys], axis=1).reshape(self._rows, -1)
+
+    # ---- reference :175-184
+    def store(self, **step_data):
+        t, R = self.ptr, self._rows
+        scal = np.concatenate([self._per_agent(step_data[k]).reshape(1, R) for k in self.FIELDS[:self.STORED]])
+        obs = self._per_agent(step_data['obs'])
+        scal_d = torch.from_numpy(np.ascontiguousarray(scal)).to(self.device)
+        obs_d = torch.from_numpy(np.ascontiguousarray(obs)).to(self.device)
+        _lib.call("xb_rollout_store", _lib.ptr(self._obs), _lib.ptr(obs_d), self._obs_dim * 4, _lib.ptr(self._scal),
+                  _lib.ptr(scal_d), self.STORED, R, self.n_size, t)
+        if self.use_actions_mask:
+            av = np.zeros((R, _pad4(self._n_act)), np.uint8)
+            av[:, :self._n_act] = self._per_agent(step_data['avail_actions'], np.float32) != 0
+            av_d = torch.from_numpy(av).to(self.device)
+            _lib.call("xb_rollout_store", _lib.ptr(self._avail), _lib.ptr(av_d), av.shape[1], None, None, 0, R,
+                      self.n_size, t)
+        if self.store_global_state:
+            st_d = torch.from_numpy(np.ascontiguousarray(step_data['state'], dtype=np.float32)).to(self.device)
+            _lib.call("xb_rollout_store", _lib.ptr(self._state), _lib.ptr(st_d), self._state_dim * 4, None, None, 0,
+                      self.n_envs, self.n_size, t)
+        self.ptr = (self.ptr + 1) % self.n_size
+        self.size = min(self.size + 1, self.n_size)
+
+    # ---- reference :186-240
+    def finish_path(self, i_env=None, agent_grouping=None, value_next=None, value_normalizer=None, **kwargs):
+        if self.size == 0:
+            return
+        beg = int(self.start_ids[i_env])
+        end = self.n_size if self.full else self.ptr
+        if end > beg:
+            n, T = self.n_agents, self.n_size
+            rows = slice(i_env * n, (i_env + 1) * n)
+            self._seg_end[rows, end - 1] = 1
+            self._boot[rows, end - 1] = [np.float32(value_next[k]) for k in self.agent_keys]
+            self._seg_end_d[rows].copy_(torch.from_numpy(self._seg_end[rows]))
+            self._boot_d[rows].copy_(torch.from_numpy(self._boot[rows]))
+            self._start_d[rows].fill_(beg)
+            self._cov_d[rows].fill_(end)
+            vn = None
+            if value_normalizer is not None:
+                groups = {agent_grouping.agent_to_group[k] for k in self.agent_keys} if agent_grouping is not None \
+                    else set(value_normalizer)
+                if len(groups) != 1:
+                    raise NotImplementedError("one parameter-sharing group")
+                vn = value_normalizer[groups.pop()]
+            vp = vn.state_pointers() if vn is not None else (None, None, None)
+            f = lambda name: _lib.ptr(self.field(name)[rows])
+            _lib.call("xb_gae_scan_vn", f('rewards'), f('values'), f('terminals'), _lib.ptr(self._seg_end_d[rows]),
+                      _lib.ptr(self._boot_d[rows]), _lib.ptr(self._start_d[rows]), _lib.ptr(self._cov_d[rows]),
+                      f('advantages'), f('returns'), n, T, float(self.gamma),
+                      float(self.gae_lambda if self.gae_lambda is not None else 0.0), 1 if self.use_gae else 0, *vp)
+        self.start_ids[i_env] = self.ptr
+
+    def _gather_rows(self, src, idx_t, row_bytes, shape, dtype):
+        out = torch.empty(shape, dtype=dtype, device=self.device)
+        _lib.call("xb_gather_rows", _lib.ptr(src), _lib.ptr(idx_t), idx_t.numel(), row_bytes, _lib.ptr(out))
+        return out
+
+    # ---- reference :242-270
+    def sample(self, indexes=None):
+        assert self.full, "Not enough transitions for on-policy buffer to random sample."
+        idx = np.asarray(indexes, dtype=np.int64).reshape(-1)
+        B, n, T = idx.size, self.n_agents, self.n_size
+        env, step = np.divmod(idx, T)
+        slots = ((env[None, :] * n + np.arange(n)[:, None]) * T + step[None, :]).reshape(-1)   # agent-major
+        slot_t = torch.from_numpy(slots).to(self.device)
+        F = len(self.FIELDS)
+        scal = torch.empty((F, n * B), dtype=torch.float32, device=self.device)
+        stats = torch.empty(2, dtype=torch.float32, device=self.device)
+        _lib.call("xb_gather_scalars", _lib.ptr(self._scal), self._rows * T, _lib.ptr(slot_t), n * B, F,
+                  _lib.ptr(scal), -1, _lib.ptr(stats), _lib.ptr(self._scratch))
+        if self.use_advantage_norm:
+            adv_plane, ia = self._scal[F - 1], F - 1
+            for k in range(n):
+                _lib.call("xb_gather_scalars", _lib.ptr(adv_plane), self._rows * T, _lib.ptr(slot_t[k * B:]), B, 1,
+                          _lib.ptr(scal[ia, k * B:]), 0, _lib.ptr(stats), _lib.ptr(self._scratch))
+        st = {name: scal[i] for i, name in enumerate(self.FIELDS)}
+        st['obs'] = self._gather_rows(self._obs, slot_t, self._obs_dim * 4, (n * B, self._obs_dim), torch.float32)
+        if self.use_actions_mask:
+            a4 = _pad4(self._n_act)
+            st['avail_actions'] = self._gather_rows(self._avail, slot_t, a4, (n * B, a4), torch.uint8)
+        if self.store_global_state:
+            s_idx = torch.from_numpy(np.tile(env * T + step, n)).to(self.device)
+            st['state'] = self._gather_rows(self._state, s_idx, self._state_dim * 4, (n * B, self._state_dim),
+                                            torch.float32)
+        out = {}
+        for key, v in st.items():
+            if key == 'state':
+                out[key] = v[:B]
+            elif key == 'avail_actions':
+                out[key] = {a: v[i * B:(i + 1) * B, :self._n_act].bool() for i, a in enumerate(self.agent_keys)}
+            elif key in ('terminals', 'agent_mask'):
+                out[key] = {a: v[i * B:(i + 1) * B].bool() for i, a in enumerate(self.agent_keys)}
+            else:
+                out[key] = {a: v[i * B:(i + 1) * B] for i, a in enumerate(self.agent_keys)}
+        out['batch_size'] = B
+        out['_stacked'] = st
+        return out
+
+    # ---- checkpoint (the reference does not save its rollout)
+    def state_dict(self):
+        return {"class": type(self).__name__, "buffer_size": self.buffer_size, "n_envs": self.n_envs,
+                "ptr": int(self.ptr), "size": int(self.size), "start_ids": self.start_ids.copy(),
+                "scal": self._scal.cpu(), "obs": self._obs.cpu(),
+                "avail": None if self._avail is None else self._avail.cpu(),
+                "state": None if self._state is None else self._state.cpu(),
+                "seg_end": self._seg_end.copy(), "boot": self._boot.copy()}
+
+    def load_state_dict(self, sd):
+        if (sd.get("class"), sd.get("buffer_size"), sd.get("n_envs")) != (type(self).__name__, self.buffer_size,
+                                                                           self.n_envs):
+            raise ValueError("on-policy MARL checkpoint does not match this buffer's size / envs")
+        self._scal.copy_(sd["scal"])
+        self._obs.copy_(sd["obs"])
+        if self._avail is not None:
+            self._avail.copy_(sd["avail"])
+        if self._state is not None:
+            self._state.copy_(sd["state"])
+        self._seg_end[:] = sd["seg_end"]
+        self._boot[:] = sd["boot"]
+        self.ptr, self.size, self.start_ids = int(sd["ptr"]), int(sd["size"]), np.array(sd["start_ids"])

@@ -379,3 +379,216 @@ extern "C" int xb_dqn_td_fwd_bwd(const float *q_eval, const float *q_next, const
                                                           1.0f / (float)B_total, gamma, dq, td, stats, scratch);
     return xb_launch_status();
 }
+
+// =====================================================================================================
+// K4M  xb_mappo_prepare / xb_value_norm_update / xb_mappo_loss_fwd_bwd
+// =====================================================================================================
+// MAPPO_Learner.update (mappo_learner.py:55-113) for one parameter-sharing group of a feed-forward actor and critic.
+// prepare: block[0..2] = (sum mask, sum ret, sum ret^2) over the local rows in float64 (deterministic grid reduction);
+// the learner SUM-all-reduces the block when the minibatch is sharded.
+__global__ void __launch_bounds__(256) mappo_prepare_kernel(const float *__restrict__ mask, const float *__restrict__ ret,
+                                                            int64_t R, double *__restrict__ block,
+                                                            double *__restrict__ scratch) {
+    __shared__ double red[3 * 32];
+    double acc[3] = {0, 0, 0};
+    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < R; b += (int64_t)gridDim.x * blockDim.x) {
+        const double r = (double)ret[b];
+        acc[0] += (double)mask[b];
+        acc[1] += r;
+        acc[2] += r * r;
+    }
+    grid_sum_finalize<3>(acc, scratch, red, [&](double(&t)[3]) {
+        block[0] = t[0];
+        block[1] = t[1];
+        block[2] = t[2];
+        block[3] = 0.0;
+    });
+}
+
+extern "C" int xb_mappo_prepare(const float *mask, const float *ret, int64_t R, double *block, double *scratch,
+                                void *stream) {
+    if (!mask || !ret || !block || !scratch || R <= 0) return XB_EINVAL;
+    const int64_t want = (R + 255) / 256;
+    const int grid = (int)(want < XB_MAX_PARTIALS ? want : XB_MAX_PARTIALS);
+    mappo_prepare_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(mask, ret, R, block, scratch);
+    return xb_launch_status();
+}
+
+// ValueNorm.running_mean_var (value_norm.py:29-33) in float32, in torch's operation order.
+__device__ __forceinline__ void value_norm_mean_std(float rm, float rmsq, float dt, float &mean, float &stdv) {
+    const float d = fmaxf(dt, 1e-5f);
+    mean = __fdiv_rn(rm, d);
+    const float msq = __fdiv_rn(rmsq, d);
+    const float var = fmaxf(__fsub_rn(msq, __fmul_rn(mean, mean)), 1e-2f);
+    stdv = __fsqrt_rn(var);
+}
+
+// ValueNorm.update (value_norm.py:35-52, per_element_update=False) on the batch moments of the prepared block, then
+// (mean, std) of the updated state into mean_std[2].
+__global__ void value_norm_update_kernel(float *rm, float *rmsq, float *dt, const double *block, int64_t R_total,
+                                         float w, float omw, float *mean_std) {
+    const float bm = (float)(block[1] / (double)R_total);
+    const float bsq = (float)(block[2] / (double)R_total);
+    const float m = __fadd_rn(__fmul_rn(rm[0], w), __fmul_rn(bm, omw));
+    const float msq = __fadd_rn(__fmul_rn(rmsq[0], w), __fmul_rn(bsq, omw));
+    const float d = __fadd_rn(__fmul_rn(dt[0], w), omw);
+    rm[0] = m, rmsq[0] = msq, dt[0] = d;
+    float mean, stdv;
+    value_norm_mean_std(m, msq, d, mean, stdv);
+    mean_std[0] = mean;
+    mean_std[1] = stdv;
+}
+
+extern "C" int xb_value_norm_update(float *running_mean, float *running_mean_sq, float *debiasing_term,
+                                    const double *block, int64_t R_total, double beta, float *mean_std, void *stream) {
+    if (!running_mean || !running_mean_sq || !debiasing_term || !block || !mean_std || R_total <= 0) return XB_EINVAL;
+    if (!(beta > 0.0 && beta < 1.0)) return XB_EINVAL;
+    value_norm_update_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(running_mean, running_mean_sq, debiasing_term, block,
+                                                                R_total, (float)beta, (float)(1.0 - beta), mean_std);
+    return xb_launch_status();
+}
+
+// nn.HuberLoss(reduction='none', delta) forward and d/d(input) at d = input - target (aten huber / huber_backward);
+// delta <= 0 selects (input - target)^2.
+__device__ __forceinline__ void value_loss(float d, float delta, float &l, float &g) {
+    if (delta > 0.f) {
+        const float z = fabsf(d);
+        l = z < delta ? __fmul_rn(__fmul_rn(0.5f, z), z) : __fmul_rn(delta, __fsub_rn(z, __fmul_rn(0.5f, delta)));
+        g = d <= -delta ? -delta : (d >= delta ? delta : d);
+    } else {
+        l = __fmul_rn(d, d);
+        g = 2.f * d;
+    }
+}
+
+template <int A_MAX>
+__global__ void __launch_bounds__(256, 1) mappo_loss_kernel(
+    const float *__restrict__ logits, const uint8_t *__restrict__ avail, int avail_ld,
+    const float *__restrict__ actions, const float *__restrict__ old_logp, const float *__restrict__ adv,
+    const float *__restrict__ value, const float *__restrict__ old_value, const float *__restrict__ ret,
+    const float *__restrict__ mask, const float *__restrict__ vn, const double *__restrict__ prep, int64_t R, int A,
+    int64_t R_total, float clip, float vclip, float hdelta, float vf_coef, float ent_coef,
+    float *__restrict__ dlogits, float *__restrict__ dvalue, float *__restrict__ stats, double *__restrict__ scratch) {
+    __shared__ double red[4 * 32];
+    double acc[4] = {0, 0, 0, 0};  // sum mask*(-min surrogate), mask*critic loss, mask*entropy, value
+    const double msum = prep[0];
+    // the reference divides by mask.sum(): with a global sum of 0 every weight is 0/0 = NaN, as there
+    const float inv_ms = (float)(1.0 / msum);
+    const float lo = 1.0f - clip, hi = 1.0f + clip;
+    float vmean = 0.f, vstd = 1.f;
+    if (vn) vmean = vn[0], vstd = vn[1];
+    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < R; b += (int64_t)gridDim.x * blockDim.x) {
+        const float *zr = logits + b * A;
+        const uint8_t *av = avail ? avail + b * avail_ld : nullptr;
+        float z[A_MAX];
+#pragma unroll
+        for (int i = 0; i < A_MAX; ++i)
+            if (i < A) z[i] = (av && !av[i]) ? -1e10f : zr[i];  // actor_head.py:40 (in place: no gradient there)
+        float m = -INFINITY;
+#pragma unroll
+        for (int i = 0; i < A_MAX; ++i)
+            if (i < A) m = fmaxf(m, z[i]);
+        float se = 0.f;
+#pragma unroll
+        for (int i = 0; i < A_MAX; ++i)
+            if (i < A) se += expf(z[i] - m);
+        const float lse = m + logf(se);
+        const int a = (int)actions[b];
+        float ent = 0.f, logp_a = 0.f;
+#pragma unroll
+        for (int i = 0; i < A_MAX; ++i) {
+            if (i < A) {
+                const float lp = z[i] - lse;
+                ent -= expf(lp) * lp;
+                if (i == a) logp_a = lp;
+            }
+        }
+        const float mk = mask[b], w = mk * inv_ms;
+        const float ad = adv[b];
+        // policy: -(min(ratio*adv, clip(ratio)*adv) * mask).sum() / mask.sum()
+        const float ratio = expf(logp_a - old_logp[b]);
+        const float rc = fminf(fmaxf(ratio, lo), hi);
+        const float s1 = ratio * ad, s2 = rc * ad;
+        const float smin = fminf(s1, s2);
+        const float g1 = s1 < s2 ? 1.f : (s1 == s2 ? 0.5f : 0.f);
+        const float g2 = s2 < s1 ? 1.f : (s1 == s2 ? 0.5f : 0.f);
+        const bool inside = ratio >= lo && ratio <= hi;  // clamp backward passes the gradient on the boundary
+        const float d_logp = -w * ad * (g1 + (inside ? g2 : 0.f)) * ratio;
+        const float dent = -ent_coef * w;
+        float *dz = dlogits + b * A;
+#pragma unroll
+        for (int i = 0; i < A_MAX; ++i) {
+            if (i < A) {
+                const float lp = z[i] - lse, p = expf(lp);
+                float g = d_logp * ((i == a ? 1.f : 0.f) - p) + dent * (-p * (lp + ent));
+                dz[i] = (av && !av[i]) ? 0.f : g;
+            }
+        }
+        // critic: value clipping, value normalisation of the target, Huber or squared error, torch.max of the two
+        const float vp = value[b];
+        const float tgt = vn ? __fdiv_rn(__fsub_rn(ret[b], vmean), vstd) : ret[b];
+        float l1, gv1, lc, dlc;
+        value_loss(__fsub_rn(vp, tgt), hdelta, l1, gv1);
+        if (vclip > 0.f) {
+            const float vo = old_value[b];
+            const float dd = __fsub_rn(vp, vo);
+            const float vc = __fadd_rn(vo, fminf(fmaxf(dd, -vclip), vclip));
+            const bool pass = dd >= -vclip && dd <= vclip;
+            float l2, gv2;
+            value_loss(__fsub_rn(vc, tgt), hdelta, l2, gv2);
+            lc = fmaxf(l1, l2);
+            const float h1 = l1 > l2 ? 1.f : (l1 == l2 ? 0.5f : 0.f);
+            const float h2 = l2 > l1 ? 1.f : (l1 == l2 ? 0.5f : 0.f);
+            dlc = h1 * gv1 + (pass ? h2 * gv2 : 0.f);
+        } else {
+            lc = l1;
+            dlc = gv1;
+        }
+        dvalue[b] = vf_coef * w * dlc;
+        acc[0] += (double)(-smin) * (double)mk;
+        acc[1] += (double)lc * (double)mk;
+        acc[2] += (double)ent * (double)mk;
+        acc[3] += (double)vp;
+    }
+    grid_sum_finalize<4>(acc, scratch, red, [&](double(&t)[4]) {
+        const double im = 1.0 / msum;
+        const float a_loss = (float)(t[0] * im), c_loss = (float)(t[1] * im), e = (float)(t[2] * im);
+        stats[0] = a_loss;
+        stats[1] = c_loss;
+        stats[2] = e;
+        stats[3] = (float)(t[3] / (double)R_total);
+        stats[4] = a_loss + vf_coef * c_loss - ent_coef * e;
+        stats[5] = 0.f;
+        stats[6] = 0.f;
+        stats[7] = 0.f;
+    });
+}
+
+extern "C" int xb_mappo_loss_fwd_bwd(const float *logits, const uint8_t *avail, int avail_ld, const float *actions,
+                                     const float *old_logp, const float *adv, const float *value,
+                                     const float *old_value, const float *ret, const float *mask, const float *vn,
+                                     const double *prep, int64_t R, int A, int64_t R_total, float clip_range,
+                                     float value_clip_range, float huber_delta, float vf_coef, float ent_coef,
+                                     float *dlogits, float *dvalue, float *stats, double *scratch, void *stream) {
+    if (!logits || !actions || !old_logp || !adv || !value || !ret || !mask || !prep || !dlogits || !dvalue ||
+        !stats || !scratch)
+        return XB_EINVAL;
+    if (value_clip_range > 0.f && !old_value) return XB_EINVAL;
+    if (R <= 0 || R_total < R || A <= 0) return XB_EINVAL;
+    if (avail && avail_ld < A) return XB_EINVAL;
+    if (A > 64) return XB_ERANGE;
+    const int64_t want = (R + 255) / 256;
+    const int grid = (int)(want < XB_MAX_PARTIALS ? want : XB_MAX_PARTIALS);
+    cudaStream_t s = (cudaStream_t)stream;
+#define XB_MAPPO(AM)                                                                                                 \
+    mappo_loss_kernel<AM><<<grid, 256, 0, s>>>(logits, avail, avail_ld, actions, old_logp, adv, value, old_value,   \
+                                               ret, mask, vn, prep, R, A, R_total, clip_range, value_clip_range,     \
+                                               huber_delta, vf_coef, ent_coef, dlogits, dvalue, stats, scratch)
+    if (A <= 4) XB_MAPPO(4);
+    else if (A <= 8) XB_MAPPO(8);
+    else if (A <= 18) XB_MAPPO(18);
+    else if (A <= 32) XB_MAPPO(32);
+    else XB_MAPPO(64);
+#undef XB_MAPPO
+    return xb_launch_status();
+}

@@ -218,6 +218,140 @@ extern "C" int xb_gae_scan(const float *rew, const float *val, const float *term
     return xb_launch_status();
 }
 
+// ---- K2 with value normalisation: MARL_OnPolicyBuffer.finish_path (memory_tools_marl.py:208-236)
+// Rows are (env, agent) pairs.  Values and the GAE bootstrap are denormalised with the ValueNorm state read here,
+// in float32 as ValueNorm.denormalize computes it; the recursion runs in float64 like the reference's Python floats;
+// returns are rounded to float32 and advantages = returns - denorm(values) in float32.  Only steps in
+// [start[row], covered[row]) are written, so a path keeps the state of the moment it was finished.
+__device__ __forceinline__ void vn_state(const float *rm, const float *rmsq, const float *dt, float &mean, float &stdv) {
+    mean = 0.f, stdv = 1.f;
+    if (!rm) return;
+    const float d = fmaxf(dt[0], 1e-5f);
+    mean = __fdiv_rn(rm[0], d);
+    const float var = fmaxf(__fsub_rn(__fdiv_rn(rmsq[0], d), __fmul_rn(mean, mean)), 1e-2f);
+    stdv = __fsqrt_rn(var);
+}
+__device__ __forceinline__ float vn_denorm(float x, bool on, float mean, float stdv) {
+    return on ? __fadd_rn(__fmul_rn(x, stdv), mean) : x;
+}
+
+// use_gae: the same warp scan of affine maps as K2 (one warp per row), in float64
+__global__ void __launch_bounds__(128) marl_gae_kernel(const float *__restrict__ rew, const float *__restrict__ val,
+                                                       const float *__restrict__ term,
+                                                       const uint8_t *__restrict__ seg_end,
+                                                       const float *__restrict__ boot, const int32_t *__restrict__ start,
+                                                       const int32_t *__restrict__ covered, float *__restrict__ adv,
+                                                       float *__restrict__ ret, int N, int T, double gamma, double lam,
+                                                       const float *rm, const float *rmsq, const float *dt) {
+    const int lane = threadIdx.x & 31;
+    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= N) return;
+    float mean, stdv;
+    vn_state(rm, rmsq, dt, mean, stdv);
+    const bool on = rm != nullptr;
+    const int64_t base = (int64_t)row * T;
+    const int beg = start ? start[row] : 0, cov = covered ? covered[row] : T;
+    constexpr int V = 4, TILE = 32 * V;
+    double carry = 0.0;
+    for (int hi = ((T + TILE - 1) / TILE) * TILE; hi > 0; hi -= TILE) {
+        const int t0 = hi - TILE + lane * V;
+        float v[V + 1];
+        Affine<double> loc[V];
+        Affine<double> acc = {1.0, 0.0};
+#pragma unroll
+        for (int j = 0; j < V; ++j) v[j] = (t0 + j < T) ? vn_denorm(val[base + t0 + j], on, mean, stdv) : 0.f;
+        {
+            float nxt = __shfl_down_sync(0xffffffffu, v[0], 1);
+            if (lane == 31) nxt = (t0 + V < T) ? vn_denorm(val[base + t0 + V], on, mean, stdv) : 0.f;
+            v[V] = nxt;
+        }
+#pragma unroll
+        for (int j = V - 1; j >= 0; --j) {
+            const int t = t0 + j;
+            const bool in = t < T;
+            const bool se = in ? seg_end[base + t] != 0 : true;
+            const double nd = in ? 1.0 - (double)term[base + t] : 1.0;
+            const double vnext = (double)((in && se) ? vn_denorm(boot[base + t], on, mean, stdv) : v[j + 1]);
+            const double r = in ? (double)rew[base + t] : 0.0;
+            Affine<double> f;
+            f.a = se ? 0.0 : nd * gamma * lam;
+            f.b = r + nd * gamma * vnext - (double)v[j];
+            acc = compose(f, acc);
+            loc[j] = acc;
+        }
+        Affine<double> inc = acc;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            Affine<double> other = {shfl_down_t<double>(inc.a, o), shfl_down_t<double>(inc.b, o)};
+            if (lane + o < 32) inc = compose(inc, other);
+        }
+        Affine<double> excl = {shfl_down_t<double>(inc.a, 1), shfl_down_t<double>(inc.b, 1)};
+        if (lane == 31) excl = {1.0, 0.0};
+        const double x_in = excl.a * carry + excl.b;
+#pragma unroll
+        for (int j = 0; j < V; ++j) {
+            const int t = t0 + j;
+            if (t < T && t >= beg && t < cov) {
+                const float r_out = (float)(loc[j].a * x_in + loc[j].b + (double)v[j]);
+                ret[base + t] = r_out;
+                adv[base + t] = __fsub_rn(r_out, v[j]);
+            }
+        }
+        const double first = loc[0].a * x_in + loc[0].b;
+        carry = __shfl_sync(0xffffffffu, first, 0);
+    }
+}
+
+// not use_gae: returns_[t] = r_t + (1 - d_t) * gamma * returns_[t+1], stored to float32 at every step as the reference's
+// float32 array does (a serial recursion, one thread per row); the bootstrap is the raw stored value, not denormalised
+__global__ void __launch_bounds__(128) marl_returns_kernel(const float *__restrict__ rew, const float *__restrict__ val,
+                                                           const float *__restrict__ term,
+                                                           const uint8_t *__restrict__ seg_end,
+                                                           const float *__restrict__ boot,
+                                                           const int32_t *__restrict__ start,
+                                                           const int32_t *__restrict__ covered, float *__restrict__ adv,
+                                                           float *__restrict__ ret, int N, int T, double gamma,
+                                                           const float *rm, const float *rmsq, const float *dt) {
+    const int row = blockIdx.x * blockDim.x + threadIdx.x;
+    if (row >= N) return;
+    float mean, stdv;
+    vn_state(rm, rmsq, dt, mean, stdv);
+    const bool on = rm != nullptr;
+    const int64_t base = (int64_t)row * T;
+    const int beg = start ? start[row] : 0, cov = covered ? covered[row] : T;
+    float next = 0.f;
+    for (int t = cov - 1; t >= beg; --t) {
+        if (seg_end[base + t]) next = boot[base + t];
+        const double nd = 1.0 - (double)term[base + t];
+        next = (float)((double)rew[base + t] + nd * gamma * (double)next);
+        ret[base + t] = next;
+        adv[base + t] = __fsub_rn(next, vn_denorm(val[base + t], on, mean, stdv));
+    }
+}
+
+extern "C" int xb_gae_scan_vn(const float *rew, const float *val, const float *term, const uint8_t *seg_end,
+                              const float *bootstrap, const int32_t *start, const int32_t *covered, float *adv,
+                              float *ret, int N, int T, double gamma, double lam, int use_gae,
+                              const float *running_mean, const float *running_mean_sq, const float *debiasing_term,
+                              void *stream) {
+    if (!rew || !val || !term || !seg_end || !bootstrap || !adv || !ret) return XB_EINVAL;
+    if (N <= 0 || T <= 0) return XB_EINVAL;
+    const bool some = running_mean || running_mean_sq || debiasing_term;
+    if (some && !(running_mean && running_mean_sq && debiasing_term)) return XB_EINVAL;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (use_gae) {
+        const int warps_per_block = 4;
+        marl_gae_kernel<<<(N + warps_per_block - 1) / warps_per_block, 32 * warps_per_block, 0, s>>>(
+            rew, val, term, seg_end, bootstrap, start, covered, adv, ret, N, T, gamma, lam, running_mean,
+            running_mean_sq, debiasing_term);
+    } else {
+        marl_returns_kernel<<<(N + 127) / 128, 128, 0, s>>>(rew, val, term, seg_end, bootstrap, start, covered, adv,
+                                                             ret, N, T, gamma, running_mean, running_mean_sq,
+                                                             debiasing_term);
+    }
+    return xb_launch_status();
+}
+
 // =====================================================================================================
 // K3  gathers
 // =====================================================================================================

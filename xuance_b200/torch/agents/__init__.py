@@ -13,3 +13,6 @@ except ImportError:
 from .marl import MARLAgents, OffPolicyMARLAgents, QMIX_Agents, VDN_Agents
 REGISTRY_Agents["QMIX"] = QMIX_Agents
 REGISTRY_Agents["VDN"] = VDN_Agents
+from .mappo_agents import OnPolicyMARLAgents, MAPPO_Agents, IPPO_Agents
+REGISTRY_Agents["MAPPO"] = MAPPO_Agents
+REGISTRY_Agents["IPPO"] = IPPO_Agents

@@ -1,0 +1,290 @@
+"""Multi-agent on-policy agents - mirrors of
+
+* ``OnPolicyMARLAgents``  xuance/torch/agents/core/on_policy_marl.py:16-693 (``store_experience``, ``get_actions``
+                          returning values and log-probabilities, ``values_next``, ``train``, ``run_episodes``,
+                          ``train_epochs``, ``test``), the feed-forward branch (``use_rnn=False``);
+* ``MAPPO_Agents``        xuance/torch/agents/multi_agent_rl/mappo_agents.py:18-112.
+
+Scope: one parameter-sharing group, Discrete actions (with or without action masks), Basic_MLP representations.
+Acting: one staged upload of the vector step's observations ([n_envs * n_agents, obs_dim]), the actor, the mask as
+-1e10 logits (actor_head.py:40), K10 sampling on the device, the critic, and ONE device-to-host read of actions,
+log-probabilities and values."""
+from copy import deepcopy
+from operator import itemgetter
+
+import numpy as np
+import torch
+import torch.nn as nn
+
+from ... import _lib
+from ...common import MARL_OnPolicyBuffer
+from ..rl_models import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic
+from .marl import MARLAgents
+
+
+class MARLActionOutput:
+    def __init__(self, env_actions=None, log_probs=None, values=None, rnn_states_actor=None, rnn_states_critic=None):
+        self.env_actions, self.log_probs, self.values = env_actions, log_probs, values
+        self.rnn_states_actor, self.rnn_states_critic = rnn_states_actor, rnn_states_critic
+
+
+class OnPolicyMARLAgents(MARLAgents):
+    """on_policy_marl.py:16-693."""
+
+    def __init__(self, config, envs=None, num_agents=None, agent_keys=None, state_space=None, observation_space=None,
+                 action_space=None, callback=None):
+        if getattr(config, "use_rnn", False):
+            raise NotImplementedError("recurrent MAPPO (use_rnn=True: MARL_OnPolicyBuffer_RNN, episode-major on-policy "
+                                      "storage) is not supported; use a feed-forward representation")
+        super().__init__(config, envs, num_agents, agent_keys, state_space, observation_space, action_space, callback)
+        self.on_policy = True
+        self.continuous_control = False
+        self.n_epochs, self.n_minibatch = config.n_epochs, config.n_minibatch
+        self.buffer_size = config.buffer_size
+        self.batch_size = self.buffer_size // self.n_minibatch
+
+    def _build_memory(self):
+        """on_policy_marl.py:77-98."""
+        avail_shape = {k: (self.action_space[k].n,) for k in self.agent_keys} if self.use_actions_mask else None
+        return MARL_OnPolicyBuffer(agent_keys=self.agent_keys,
+                                   state_space=self.state_space if self.use_global_state else None,
+                                   obs_space=self.observation_space, act_space=self.action_space, n_envs=self.n_envs,
+                                   buffer_size=self.config.buffer_size, use_gae=self.config.use_gae,
+                                   use_advnorm=self.config.use_advnorm, gamma=self.config.gamma,
+                                   gae_lam=self.config.gae_lambda, avail_actions_shape=avail_shape,
+                                   use_actions_mask=self.use_actions_mask, max_episode_steps=self.episode_length,
+                                   device=self.device)
+
+    def store_experience(self, obs_list, avail_actions, actions_list, log_pi_a, rewards_list, values_dict,
+                         terminals_list, info, **kwargs):
+        """on_policy_marl.py:103-158."""
+        K = self.agent_keys
+        data = {'obs': {k: np.array([d[k] for d in obs_list]) for k in K},
+                'actions': {k: np.array([d[k] for d in actions_list]) for k in K},
+                'log_pi_old': log_pi_a,
+                'rewards': {k: np.array([d[k] for d in rewards_list]) for k in K},
+                'values': values_dict,
+                'terminals': {k: np.array([d[k] for d in terminals_list]) for k in K},
+                'agent_mask': {k: np.array([d['agent_mask'][k] for d in info]) for k in K}}
+        if self.use_global_state:
+            data['state'] = np.array(kwargs['state'])
+        if self.use_actions_mask:
+            data['avail_actions'] = {k: np.array([d[k] for d in avail_actions]) for k in K}
+        self.memory.store(**data)
+
+    def _states(self, state, n_envs):
+        if not self.use_global_state or state is None:
+            return None
+        s = torch.as_tensor(np.asarray(state, np.float32), device=self.device)
+        return s.repeat_interleave(self.n_agents, dim=0)          # rows are env-major, agent-minor
+
+    @torch.no_grad()
+    def get_actions(self, obs_list, state=None, avail_actions_list=None, rnn_states_actor=None,
+                    rnn_states_critic=None, test_mode=False, deterministic=False, **kwargs):
+        """on_policy_marl.py:207-306."""
+        n_envs, K = len(obs_list), self.agent_keys
+        obs, avail = self._build_inputs(obs_list, avail_actions_list)
+        obs_d = torch.from_numpy(obs).to(self.device)
+        logits = self.model.logits(obs_d)
+        if avail is not None:
+            logits = logits.masked_fill(torch.from_numpy(avail).to(self.device) == 0, -1e10)
+        logits = logits.contiguous()
+        R, A = logits.shape
+        out = torch.empty((3, R), dtype=torch.float32, device=self.device)   # actions, log_pi, values
+        acts_i = torch.empty(R, dtype=torch.int32, device=self.device)
+        u = None if deterministic else torch.rand(R, device=self.device)
+        _lib.call("xb_categorical_act", _lib.ptr(logits), _lib.ptr(u), None, R, A, _lib.ptr(out[0]), _lib.ptr(acts_i),
+                  _lib.ptr(out[1]), None)
+        if not test_mode:
+            out[2] = self.model.values(obs_d, self._states(state, n_envs))
+        host = out.cpu().numpy().reshape(3, n_envs, len(K))
+        actions_list = [{k: int(host[0, e, i]) for i, k in enumerate(K)} for e in range(n_envs)]
+        log_pi, values = {}, {}
+        if not test_mode:
+            log_pi = {k: host[1, :, i].copy() for i, k in enumerate(K)}
+            values = {k: host[2, :, i].copy() for i, k in enumerate(K)}
+        return MARLActionOutput(env_actions=actions_list, log_probs=log_pi, values=values)
+
+    @torch.no_grad()
+    def values_next(self, i_env, obs_dict, state=None, rnn_states_critic=None):
+        """on_policy_marl.py:308-357."""
+        obs, _ = self._build_inputs([obs_dict])
+        st = None if state is None else np.asarray(state)[None]
+        v = self.model.values(torch.from_numpy(obs).to(self.device), self._states(st, 1)).cpu().numpy()
+        return None, {k: v[i] for i, k in enumerate(self.agent_keys)}
+
+    def _finish(self, i, terminated, next_obs, next_state):
+        if all(terminated.values()):
+            value_next = {k: 0.0 for k in self.agent_keys}
+        else:
+            _, value_next = self.values_next(i_env=i, obs_dict=next_obs, state=next_state)
+        self.memory.finish_path(i_env=i, agent_grouping=self.agent_grouping, value_next=value_next,
+                                value_normalizer=self.learner.value_normalizer)
+
+    def train(self, train_steps):
+        """on_policy_marl.py:405-482 (the feed-forward branch)."""
+        train_info = {}
+        envs = self.train_envs
+        obs_list = envs.buf_obs
+        avail_actions = envs.buf_avail_actions if self.use_actions_mask else None
+        state = envs.buf_state if self.use_global_state else None
+        for _ in range(train_steps):
+            policy_out = self.get_actions(obs_list=obs_list, state=state, avail_actions_list=avail_actions)
+            actions_list = policy_out.env_actions
+            next_obs_list, rewards_list, terminated_list, truncated, info = envs.step(actions_list)
+            next_state = envs.buf_state if self.use_global_state else None
+            next_avail_actions = envs.buf_avail_actions if self.use_actions_mask else None
+            self.callback.on_train_step(self.current_step, envs=envs, policy=self.model, obs=obs_list,
+                                        policy_out=policy_out, acts=actions_list, next_obs=next_obs_list,
+                                        rewards=rewards_list, state=state, next_state=next_state,
+                                        avail_actions=avail_actions, next_avail_actions=next_avail_actions,
+                                        terminals=terminated_list, truncations=truncated, infos=info,
+                                        train_steps=train_steps, values_dict=policy_out.values)
+            self.store_experience(obs_list, avail_actions, actions_list, policy_out.log_probs, rewards_list,
+                                  policy_out.values, terminated_list, info, state=state)
+            if self.memory.full:
+                for i in range(self.n_envs):
+                    self._finish(i, terminated_list[i], next_obs_list[i],
+                                 next_state[i] if self.use_global_state else None)
+            update_info = self.train_epochs(n_epochs=self.n_epochs)
+            self.log_infos(update_info, self.current_step)
+            train_info.update(update_info)
+            obs_list, avail_actions = deepcopy(next_obs_list), deepcopy(next_avail_actions)
+            state = deepcopy(next_state) if self.use_global_state else None
+            for i in range(self.n_envs):
+                if all(terminated_list[i].values()) or truncated[i]:
+                    self._finish(i, terminated_list[i], obs_list[i], state[i] if self.use_global_state else None)
+                    obs_list[i] = info[i]["reset_obs"]
+                    envs.buf_obs[i] = info[i]["reset_obs"]
+                    if self.use_actions_mask:
+                        avail_actions[i] = info[i]["reset_avail_actions"]
+                        envs.buf_avail_actions[i] = info[i]["reset_avail_actions"]
+                    if self.use_global_state:
+                        state[i] = info[i]["reset_state"]
+                        envs.buf_state[i] = info[i]["reset_state"]
+                    self.current_episode[i] += 1
+                    episode_info = {
+                        "Train-Results/Episode-Steps": {"env-%d" % i: info[i]["episode_step"]},
+                        "Train-Results/Episode-Rewards": {
+                            "env-%d" % i: float(np.mean(itemgetter(*self.agent_keys)(info[i]["episode_score"])))}}
+                    self.log_infos(episode_info, self.current_step)
+                    train_info.update(episode_info)
+                    self.callback.on_train_episode_info(envs=envs, policy=self.model, env_id=i, infos=info,
+                                                        rank=self.rank, use_wandb=self.use_wandb,
+                                                        current_step=self.current_step,
+                                                        current_episode=self.current_episode,
+                                                        train_steps=train_steps)
+            self.current_step += self.n_envs
+            self.callback.on_train_step_end(self.current_step, envs=envs, policy=self.model,
+                                            train_steps=train_steps, train_info=train_info)
+        return train_info
+
+    def run_episodes(self, n_episodes=1, deterministic_policy=False, run_envs=None, test_mode=False, close_envs=True):
+        """on_policy_marl.py:484-630 (feed-forward; no rendering)."""
+        envs = self.train_envs if run_envs is None else run_envs
+        num_envs = envs.num_envs
+        _current_episode, scores = 0, []
+        obs_list, info = envs.reset()
+        avail_actions = envs.buf_avail_actions if self.use_actions_mask else None
+        state = envs.buf_state if self.use_global_state else None
+        while _current_episode < n_episodes:
+            policy_out = self.get_actions(obs_list=obs_list, state=state, avail_actions_list=avail_actions,
+                                          test_mode=test_mode, deterministic=deterministic_policy)
+            actions_list = policy_out.env_actions
+            next_obs_list, rewards_list, terminated_list, truncated, info = envs.step(actions_list)
+            next_state = envs.buf_state if self.use_global_state else None
+            next_avail_actions = envs.buf_avail_actions if self.use_actions_mask else None
+            if not test_mode:
+                self.store_experience(obs_list, avail_actions, actions_list, policy_out.log_probs, rewards_list,
+                                      policy_out.values, terminated_list, info, state=state)
+            obs_list, avail_actions = deepcopy(next_obs_list), deepcopy(next_avail_actions)
+            state = deepcopy(next_state) if self.use_global_state else None
+            for i in range(num_envs):
+                if all(terminated_list[i].values()) or truncated[i]:
+                    _current_episode += 1
+                    scores.append(float(np.mean(itemgetter(*self.agent_keys)(info[i]["episode_score"]))))
+                    if not test_mode:
+                        self._finish(i, terminated_list[i], obs_list[i], None if state is None else state[i])
+                        self.current_step += info[i]["episode_step"]
+                        self.callback.on_train_episode_info(envs=envs, policy=self.model, env_id=i, infos=info,
+                                                            rank=self.rank, use_wandb=self.use_wandb,
+                                                            current_step=self.current_step,
+                                                            current_episode=self.current_episode,
+                                                            n_episodes=n_episodes)
+                    obs_list[i] = info[i]["reset_obs"]
+                    envs.buf_obs[i] = info[i]["reset_obs"]
+                    if self.use_actions_mask:
+                        avail_actions[i] = info[i]["reset_avail_actions"]
+                        envs.buf_avail_actions[i] = info[i]["reset_avail_actions"]
+                    if self.use_global_state:
+                        state[i] = info[i]["reset_state"]
+                        envs.buf_state[i] = info[i]["reset_state"]
+        if test_mode:
+            self.log_infos({"Test-Results/Episode-Rewards/Mean-Score": float(np.mean(scores)),
+                            "Test-Results/Episode-Rewards/Std-Score": float(np.std(scores))}, self.current_step)
+            if close_envs:
+                envs.close()
+        return scores
+
+    def train_epochs(self, n_epochs=1):
+        """on_policy_marl.py:632-661: shuffled n_minibatch slices per epoch; the info of the last update (only that
+        one reads the device statistics back)."""
+        info_train = {}
+        if self.memory.full:
+            indexes = np.arange(self.buffer_size)
+            for e in range(n_epochs):
+                np.random.shuffle(indexes)
+                for start in range(0, self.buffer_size, self.batch_size):
+                    last = e == n_epochs - 1 and start + self.batch_size >= self.buffer_size
+                    info_train = self.learner.update(self.memory.sample(indexes[start:start + self.batch_size]),
+                                                     sync=last)
+            self.callback.on_train_epochs_end(self.current_step, policy=self.model, memory=self.memory,
+                                              current_episode=self.current_episode, n_epochs=n_epochs,
+                                              buffer_size=self.buffer_size, update_info=info_train)
+            self.memory.clear()
+        return info_train
+
+    def test(self, test_episodes, deterministic_policy=True, test_envs=None, close_envs=True):
+        return self.run_episodes(n_episodes=test_episodes, run_envs=test_envs, test_mode=True,
+                                 deterministic_policy=deterministic_policy, close_envs=close_envs)
+
+
+class MAPPO_Agents(OnPolicyMARLAgents):
+    """mappo_agents.py:18-112."""
+
+    def __init__(self, config, envs=None, num_agents=None, agent_keys=None, state_space=None, observation_space=None,
+                 action_space=None, callback=None):
+        super().__init__(config, envs, num_agents, agent_keys, state_space, observation_space, action_space, callback)
+        if not all(hasattr(self.action_space[k], "n") for k in self.agent_keys):
+            raise NotImplementedError("Gaussian MAPPO (Box action spaces) is not supported: MAPPO here takes Discrete "
+                                      "action spaces")
+        self.model = self._build_model()
+        self.memory = self._build_memory()
+        self.learner = self._build_learner(self.config, self.agent_grouping, self.model, self.callback)
+
+    def _build_model(self):
+        actors, critics, critic_encoders = nn.ModuleDict(), nn.ModuleDict(), nn.ModuleDict()
+        for group_key, group_agents in self.groups.items():
+            ref = group_agents[0]
+            enc = self._build_agent_feature_encoder(self.config.representation, group_agents,
+                                                    self.observation_space[ref])
+            actors[group_key] = CategoricalActor(representation=enc, actor_hidden_size=self.config.actor_hidden_size,
+                                                 action_space=self.action_space[ref], normalizer=self.normalize_fn,
+                                                 initializer=self.initializer, activation=self.activation,
+                                                 device=self.device)
+            critic_encoders[group_key] = self._build_agent_feature_encoder(self.config.representation, group_agents,
+                                                                           self.observation_space[ref])
+        for group_key in self.groups:
+            critics[group_key] = CentralizedStateValueCritic(
+                grouping=self.agent_grouping, representations=critic_encoders,
+                state_space=self.state_space if self.use_global_state else None,
+                critic_hidden_size=self.config.critic_hidden_size, normalizer=self.normalize_fn,
+                initializer=self.initializer, activation=self.activation, device=self.device)
+        return MultiAgentActorCritic(grouping=self.agent_grouping, actors=actors, critics=critics,
+                                     use_rnn=self.use_rnn, device=self.device).to(self.device)
+
+
+class IPPO_Agents(OnPolicyMARLAgents):
+    def __init__(self, config, *args, **kwargs):
+        raise NotImplementedError("IPPO is not supported yet (MAPPO's loss kernel with a per-agent critic input; "
+                                  "DESIGN.md section 9)")

@@ -148,6 +148,17 @@ class MARLAgents:
             raise NotImplementedError("agent-identity embeddings are outside the hot-path scope (mode 'none')")
         return AgentFeatureEncoder(self._build_representation(representation_choice, input_space, self.config))
 
+    def _build_inputs(self, obs_list, avail_actions_list=None):
+        """[n_envs * n_agents, obs_dim] (env-major, agent-minor) float32 and the matching uint8 availability rows."""
+        K = self.agent_keys
+        obs = np.stack([np.stack([np.asarray(d[k], np.float32) for k in K]) for d in obs_list])
+        obs = obs.reshape(len(obs_list) * len(K), -1)
+        avail = None
+        if self.use_actions_mask and avail_actions_list is not None:
+            avail = np.stack([np.stack([np.asarray(d[k]) for k in K]) for d in avail_actions_list])
+            avail = (avail.reshape(len(obs_list) * len(K), -1) != 0).astype(np.uint8)
+        return obs, avail
+
     def _build_learner(self, *args):
         from ..learners import REGISTRY_Learners
         return REGISTRY_Learners[self.config.learner](*args)
@@ -234,17 +245,6 @@ class OffPolicyMARLAgents(MARLAgents):
                 out.append(d)
             return out
         return [{k: self.action_space[k].sample() for k in self.agent_keys} for _ in range(batch_size)]
-
-    def _build_inputs(self, obs_list, avail_actions_list=None):
-        """[n_envs * n_agents, obs_dim] (env-major, agent-minor) float32 and the matching uint8 availability rows."""
-        K = self.agent_keys
-        obs = np.stack([np.stack([np.asarray(d[k], np.float32) for k in K]) for d in obs_list])
-        obs = obs.reshape(len(obs_list) * len(K), -1)
-        avail = None
-        if self.use_actions_mask and avail_actions_list is not None:
-            avail = np.stack([np.stack([np.asarray(d[k]) for k in K]) for d in avail_actions_list])
-            avail = (avail.reshape(len(obs_list) * len(K), -1) != 0).astype(np.uint8)
-        return obs, avail
 
     @torch.no_grad()
     def get_actions(self, obs_list, avail_actions_list=None, rnn_states=None, test_mode=False, **kwargs):

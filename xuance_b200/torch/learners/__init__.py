@@ -16,3 +16,5 @@ try:
     REGISTRY_Learners["VDN_Learner"] = QMIX_Learner     # vdn_learner.py: the same update with the parameter-free sum mixer
 except ImportError:
     pass
+from .mappo_learner import MAPPO_Learner
+REGISTRY_Learners["MAPPO_Learner"] = MAPPO_Learner

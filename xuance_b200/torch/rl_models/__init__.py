@@ -7,3 +7,4 @@ from .architectures import (ActorCritic, SharedActorCritic, DeepQNetwork, Duelin
                             TwinActionValueCritic, SoftActorCritic)
 from .qmix import Basic_RNN, AgentFeatureEncoder, DiscreteActionValueCritic, QMIX_Mixer, VDN_mixer, MixingQNetwork
 REGISTRY_Representation["Basic_RNN"] = Basic_RNN
+from .mappo import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic
