@@ -258,6 +258,31 @@ int xb_sac_critic_loss(const float *q1, const float *q2, const float *target_q, 
                        int64_t B_total, float *dq1, float *dq2, float *backup, float *stats, double *scratch,
                        void *stream);
 
+/* ---------------------------------------------------------------- K8D: SAC-Discrete loss stages -------
+ * Replaces the elementwise/reduction parts of SACDIS_Learner.update (xuance/torch/learners/policy_gradient/
+ * sacdis_learner.py:52-75) for a Categorical policy over A actions, 1 <= A <= 64 (else XB_ERANGE).  All matrices are
+ * row-major [B, A] float32; `alpha` is a DEVICE scalar.  Per row, as Categorical(logits).probs and the reference's
+ * log rule compute them in float32 (actor_critic.py:184-205):
+ *   p = softmax(z - logsumexp(z));  log_pi = log(p + 1e-8*[p == 0])  (floored at log(1e-8) only where p is exactly 0;
+ *   subnormal p are kept: the library is built with flush-to-zero off)
+ * actor : p_loss = mean_b sum_a p*(alpha*log_pi - min(q1,q2)).  Writes dlogits = p*(g - sum_a p*g) / B_total with
+ *         g = alpha*log_pi - min(q1,q2) + alpha*p/(p + z) (the softmax backward; entries with p = 0 get exactly 0) and
+ *         stats[4] = {Ploss, Qvalue = sum min(q1,q2) / (B_total*A), sum log_pi / (B_total*A), 0}.  No gradient to q1 /
+ *         q2 is written: the reference's critic.zero_grad() discards the one its p_loss.backward() leaves there.
+ * critic: target = sum_a p'*(min(tq1,tq2) - alpha*log_pi') of the next-state logits and the target critic's values;
+ *         backup = r + (1-d)*gamma*target; q_loss = mse(q1[a], backup) + mse(q2[a], backup), a = trunc(actions[b])
+ *         (float32 as stored).  Writes backup[B], dq1 / dq2 dense [B, A]: 2*(q_i[a] - backup)/B_total in column a and
+ *         0 elsewhere, and stats[2] = {Qloss, 0}.  A row whose action is not in [0, A) (or NaN) selects no column:
+ *         its dq rows are all 0 and it adds NaN to Qloss, so a corrupt batch shows in the log without an out-of-bounds
+ *         read.
+ * Both: B_total >= B rows scale the means (a SUM all-reduce of shards gives the global values); scratch as for K4. */
+int xb_sacdis_actor_loss(const float *logits, const float *q1, const float *q2, const float *alpha, int64_t B, int A,
+                         int64_t B_total, float *dlogits, float *stats, double *scratch, void *stream);
+int xb_sacdis_critic_loss(const float *q1, const float *q2, const float *actions, const float *logits_next,
+                          const float *tq1, const float *tq2, const float *rew, const float *term, const float *alpha,
+                          float gamma, int64_t B, int A, int64_t B_total, float *dq1, float *dq2, float *backup,
+                          float *stats, double *scratch, void *stream);
+
 /* ---------------------------------------------------------------- K7: flat-bucket optimiser step -----
  * Replaces clip_grad_norm_ + torch.optim.Adam.step on the learner's parameters (ppo_learner.py:61-65;
  * Adam eps=1e-5, no weight decay, no amsgrad) over ONE flat float32 bucket (params/grads/exp_avg/exp_avg_sq

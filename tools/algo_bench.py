@@ -3,7 +3,9 @@
 DQN+PER (2^20-transition HBM replay, B=512), SAC (1M replay, B=1024) and QMIX (5 agents x 72-d, T=60, 32 episodes)
 on one GPU, next to the oracle port of the reference's torch-CPU path on the host; and ``ppo_gauss``, continuous-control
 PPO in the shape of the reference's ppo/mujoco.yaml (train_epochs env-steps/s); ``mappo``, MAPPO in the shape of
-configs/mappo/sc2/5m_vs_6m.yaml (train_epochs env-steps/s).  Prints one JSON object.
+configs/mappo/sc2/5m_vs_6m.yaml (train_epochs env-steps/s); ``sacdis``, SAC-Discrete in the shape of
+configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (train_epochs, eager and graphed).  Prints one
+JSON object.
 
     python tools/algo_bench.py [--iters 200] [--cpu-iters 5] [--no-cpu] [--graph]
     torchrun --nnodes=1 --nproc-per-node G --master-addr 127.0.0.1 tools/algo_bench.py --no-cpu --graph    (G GPUs)
@@ -286,6 +288,53 @@ def bench_mappo(args):
     return out
 
 
+def bench_sacdis(args):
+    """SAC-Discrete: ``train_epochs(1)`` (one replay sample of 256 rows + one SACDIS_Learner.update) of a SAC_Agent built
+    from configs/sac/CartPole-v1.yaml (4-d obs, A = 2, Basic_MLP 128, heads [128], alpha fixed), and the same at A = 18 with
+    use_automatic_entropy_tuning on.  Eager and CUDA-graphed, next to the torch-CPU oracle's update on the host."""
+    from xuance_b200 import _lib
+    from xuance_b200.common import Box, Discrete
+    from xuance_b200.common.common_tools import get_arguments
+    from xuance_b200.torch.agents import SAC_Agent
+    out = {}
+    for name, A, auto in (("cartpole_A2", 2, False), ("A18_auto_alpha", 18, True)):
+        od, N, S = 4, 10, 20000
+        res = {"config": "SAC-Discrete, %d-d obs, A = %d, B = 256, Basic_MLP 128 + heads [128], auto alpha %s"
+                         % (od, A, auto)}
+        for graph in (False, True):
+            cfg = get_arguments("sac", "classic_control", "CartPole-v1")
+            for k, v in dict(device=DEV, use_cuda_graph=graph, use_automatic_entropy_tuning=auto, model_dir="/tmp/x",
+                             logger=None, distributed_training=False).items():
+                setattr(cfg, k, v)
+            agent = SAC_Agent(cfg, None, Box(-10, 10, (od,), np.float32), Discrete(A))
+            buf = agent.memory
+            buf._obs.normal_(), buf._next_obs.normal_(), buf._fields.uniform_(0, 1)
+            buf._fields[buf._fid["actions"]].mul_(A).floor_()
+            buf._fields[buf._fid["terminals"]].copy_((buf._fields[buf._fid["terminals"]] < 0.05).float())
+            buf.size = S
+            if not graph:
+                agent.train_epochs(1)
+                before = _lib.launch_count
+                agent.train_epochs(1)
+                res["xb_launches_per_update"] = _lib.launch_count - before
+            dt = timed(lambda: agent.train_epochs(1), args.iters)
+            res["gpu_%s_ms_per_update" % ("graphed" if graph else "eager")] = dt * 1e3
+            res["gpu_%s_updates_per_s" % ("graphed" if graph else "eager")] = 1 / dt
+        if not args.no_cpu:
+            from oracle_sacdis import SACDISModelOracle, SACDISLearnerOracle
+            ol = SACDISLearnerOracle(SACDISModelOracle(od, A, (128,), (128,), (128,)), auto_alpha=auto)
+            rng = np.random.default_rng(0)
+            s = {"obs": rng.normal(size=(256, od)).astype(np.float32), "obs_next": rng.normal(size=(256, od)).astype(np.float32),
+                 "actions": rng.integers(0, A, 256).astype(np.float32), "rewards": rng.random(256).astype(np.float32),
+                 "terminals": (rng.random(256) < 0.05).astype(np.float32)}
+            cdt = cpu_timed(lambda: ol.update(**s), max(args.cpu_iters, 20))
+            res.update(cpu_ms_per_update=cdt * 1e3, cpu_threads=torch.get_num_threads(),
+                       speedup_eager=cdt / (res["gpu_eager_ms_per_update"] / 1e3),
+                       speedup_graphed=cdt / (res["gpu_graphed_ms_per_update"] / 1e3))
+        out[name] = res
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=200)
@@ -317,6 +366,8 @@ def main():
         res["ppo_gauss"] = bench_ppo_gauss(args)
     if (not only and WORLD == 1) or "mappo" in only:
         res["mappo"] = bench_mappo(args)
+    if (not only and WORLD == 1) or "sacdis" in only:
+        res["sacdis"] = bench_sacdis(args)
     res["cuda_graph"] = bool(args.graph)
     res["n_gpus"] = WORLD
     if RANK == 0:

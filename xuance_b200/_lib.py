@@ -71,6 +71,9 @@ _SIGNATURES = {
     "xb_rms_update_normalize": (c_int, [_P, c_int, c_int64, _P, _P, c_double, c_int, _P, c_float, c_float, _P]),
     "xb_sac_actor_loss": (c_int, [_P, _P, _P, _P, c_int64, c_int64, _P, _P, _P, _P, _P, _P]),
     "xb_sac_critic_loss": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_float, c_int64, c_int64, _P, _P, _P, _P, _P, _P]),
+    "xb_sacdis_actor_loss": (c_int, [_P, _P, _P, _P, c_int64, c_int, c_int64, _P, _P, _P, _P]),
+    "xb_sacdis_critic_loss": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_float, c_int64, c_int, c_int64, _P, _P, _P,
+                                      _P, _P, _P]),
     "xb_qmix_select_fwd": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     "xb_qmix_select_bwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
     "xb_qmix_mix_fwd": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int, c_int, _P, _P]),

@@ -8,6 +8,8 @@ REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner,
 try:
     from .sac_learner import SAC_Learner
     REGISTRY_Learners["SAC_Learner"] = SAC_Learner
+    from .sacdis_learner import SACDIS_Learner
+    REGISTRY_Learners["SACDIS_Learner"] = SACDIS_Learner
 except ImportError:
     pass
 try:

@@ -4,7 +4,7 @@ from .distributions import CategoricalDistribution, DiagGaussianDistribution, Ac
 from .representations import Basic_Identical, Basic_MLP, Basic_CNN, AC_CNN_Atari, REGISTRY_Representation
 from .heads import CategoricalActorHead, GaussianActorHead, SAC_GaussianActorHead, ValueHead, QValueHead, DuelingQValueHead
 from .architectures import (ActorCritic, SharedActorCritic, DeepQNetwork, DuelingDeepQNetwork, GaussianActor, SAC_GaussianActor,
-                            TwinActionValueCritic, SoftActorCritic)
+                            TwinActionValueCritic, SoftActorCritic, TwinDiscreteActionValueCritic, SoftActorCriticDiscrete)
 from .qmix import Basic_RNN, AgentFeatureEncoder, DiscreteActionValueCritic, QMIX_Mixer, VDN_mixer, MixingQNetwork
 REGISTRY_Representation["Basic_RNN"] = Basic_RNN
 from .mappo import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic

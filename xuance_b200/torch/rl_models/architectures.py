@@ -201,3 +201,62 @@ class SoftActorCritic(ActorCritic):
         for ep, tp in zip(self.critic.parameters(), self.target_critic.parameters()):
             tp.data.mul_(1 - tau)
             tp.data.add_(tau * ep.data)
+
+
+class TwinDiscreteActionValueCritic(nn.Module):
+    """critics/twin_critics.py:65-117: two (representation, QValueHead) towers, each giving Q(s, .) over the A actions."""
+
+    def __init__(self, representation, action_space, critic_hidden_size, normalizer=None, initializer=None,
+                 activation=None, device=None, **kwargs):
+        super().__init__()
+        if not is_discrete(action_space):
+            raise ValueError('action_space must be Discrete')
+        self.action_space = action_space
+        self.n_actions = action_space.n
+        self.representation_1 = representation
+        self.representation_2 = deepcopy(representation)
+        self.representation_info_shape = representation.output_shapes
+        self.feature_dim = self.representation_info_shape['state'][0]
+        kw = dict(feature_dim=self.feature_dim, hidden_size=critic_hidden_size, n_actions=self.n_actions,
+                  normalizer=normalizer, initializer=initializer, activation=activation, device=device)
+        self.critic_head_1 = QValueHead(**kw)
+        self.critic_head_2 = QValueHead(**kw)
+
+    def forward(self, observation, **kwargs):
+        r1, r2 = self.representation_1(observation), self.representation_2(observation)
+        return TwinCriticOutput(representations_1=r1, representations_2=r2,
+                                values_1=self.critic_head_1(r1.embeddings), values_2=self.critic_head_2(r2.embeddings))
+
+
+class SoftActorCriticDiscrete(SoftActorCritic):
+    """actor_critic.py:162-214 over a CategoricalActor.  Qpolicy / Qtarget / Qaction return the raw logits and [B, A] Q
+    matrices: the probability and log rules (p = softmax, log(p + 1e-8*[p == 0])) and the losses run in the K8D kernels,
+    and the agent samples with K10."""
+
+    def forward(self, observation, **kwargs):
+        """The reference returns the actor's distribution and the critic's output; here the raw logits stand in for the
+        distribution (``actor_rep_out``)."""
+        return ModelOutput(values=self.critic(observation), actor_rep_out=self.actor.logits(observation))
+
+    def act(self, observation, deterministic=False, **kwargs):
+        """K10 ``xb_categorical_act`` on the actor's logits: inverse-CDF sampling of uniforms, or the first argmax when
+        ``deterministic``.  Returns int32 actions [N]."""
+        from ... import _lib
+        logits = self.actor.logits(observation).contiguous()
+        N, A = logits.shape
+        u = None if deterministic else torch.rand(N, device=logits.device)
+        actions = torch.empty(N, dtype=torch.int32, device=logits.device)
+        _lib.call("xb_categorical_act", _lib.ptr(logits), _lib.ptr(u), None, N, A, None, _lib.ptr(actions), None, None)
+        return actions
+
+    def Qpolicy(self, observation):
+        q1, q2 = self.Qaction(observation)
+        return self.actor.logits(observation), q1, q2
+
+    def Qtarget(self, observation):
+        out = self.target_critic(observation)
+        return self.actor.logits(observation), out.values_1, out.values_2
+
+    def Qaction(self, observation, *args, **kwargs):
+        out = self.critic(observation)
+        return out.values_1, out.values_2
