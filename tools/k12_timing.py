@@ -26,9 +26,11 @@ def report(label, fn):
     assert rc == 0, rc
     t = np.frombuffer(buf, dtype=np.uint64).reshape(132, 12).astype(np.float64)
     m = t.mean(0)
-    # consumer warpgroups (wgmma issue + epilogue): slots 0-1, 3; producer warpgroup: slots 4-6 (conv_tc.cu, xb_k12_timing)
-    print("%-34s consumer %8.0f clk: wait operands %4.1f%%  wait halo tile %4.1f%% | producer: wait ring %4.1f%%  wait tile buf %4.1f%%"
-          % (label, m[0], 100 * m[1] / max(m[0], 1), 100 * m[3] / max(m[0], 1), 100 * m[5] / max(m[4], 1), 100 * m[6] / max(m[4], 1)))
+    # consumer warpgroups (wgmma issue + epilogue): slots 0-3, 7; producer warpgroup: slots 4-6 (conv_tc.cu, xb_k12_timing)
+    c = lambda s: 100 * m[s] / max(m[0], 1)
+    print("%-34s consumer %8.0f clk: wait operands %4.1f%%  wait halo tile %4.1f%%  wgmma wait %4.1f%%  epilogue %4.1f%% | "
+          "producer: wait ring %4.1f%%  wait tile buf %4.1f%%"
+          % (label, m[0], c(1), c(3), c(2), c(7), 100 * m[5] / max(m[4], 1), 100 * m[6] / max(m[4], 1)))
 
 
 def roles():

@@ -49,8 +49,9 @@ constexpr int XB_HALO_MAX_CHUNKS = 16;
 constexpr int XB_K12_MAX_DYN_SMEM = 208 * 1024;      // + ~18 KB static (barriers, bias, column sums, tap table) <= 227 KB
 
 // Optional role timing (XB_K12_TIMING=1): clock64 cycles each role of CTA b spent inside its barrier waits, written at kernel
-// exit to xb_k12_timing[b][..]: 0 consumer total, 1 consumer wait full (operands), 3 consumer wait a_full (halo tile),
-// 4 producer total, 5 producer wait empty (ring), 6 producer wait a_empty (tools/k12_timing.py); the other slots are unused
+// exit to xb_k12_timing[b][..]: 0 consumer total, 1 consumer wait full (operands), 2 consumer wgmma_wait (MMAs in flight),
+// 3 consumer wait a_full (halo tile), 4 producer total, 5 producer wait empty (ring), 6 producer wait a_empty, 7 consumer
+// epilogue (last stage released .. column sums stored) (tools/k12_timing.py); the other slots are unused
 __device__ unsigned long long xb_k12_timing[160][12];
 
 struct ConvParams {
@@ -166,6 +167,25 @@ __device__ __forceinline__ void mma_plane(float (&acc)[PB * NC][16], const uint3
     }
 }
 
+// role timing: the low 32 bits of the SM clock (differences and sums of waits stay far below 2^32 cycles in one launch;
+// 32-bit sums keep the consumers' register budget)
+__device__ __forceinline__ uint32_t clock32() {
+    uint32_t c;
+    asm volatile("mov.u32 %0, %%clock;" : "=r"(c));
+    return c;
+}
+// wgmma_wait<N>, its cycles added to `cycles` when the role timing is on
+template <int N>
+__device__ __forceinline__ void timed_wgmma_wait(bool timing, uint32_t &cycles) {
+    if (timing) {
+        const uint32_t t0 = clock32();
+        wgmma_wait<N>();
+        cycles += clock32() - t0;
+    } else {
+        wgmma_wait<N>();
+    }
+}
+
 // register split between the roles (setmaxnreg): 384 threads at the 168 registers one CTA per SM allows = 64512 per CTA;
 // the producer warpgroup gives back to PROD_REGS and the consumer warpgroups, which hold the accumulators and the double
 // buffered A fragments, take CONS_REGS: 2 * 128 * CONS_REGS + 128 * PROD_REGS must not exceed 128 * 3 * 168, or the
@@ -247,13 +267,15 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
     }
     __syncthreads();
     const uint32_t smem_base = smem_u32(smem);
-    unsigned long long t_wait[3] = {0, 0, 0};
-    const unsigned long long t_begin = p.timing ? clock64() : 0ull;
+    uint32_t t_wait[5] = {0, 0, 0, 0, 0};                   // role timing: slots 0-2 barrier waits, 3 wgmma_wait, 4 epilogue
+    // role timing: the two reporting threads park their start clock in their total slot until kernel exit (not in a
+    // register that would stay live across the whole main loop)
+    if (p.timing && blockIdx.x < 160 && (tid == 0 || tid == CONS_WARPS * 32)) xb_k12_timing[blockIdx.x][tid == 0 ? 0 : 4] = clock64();
     auto timed_wait = [&](uint64_t *bar, uint32_t parity, int slot) {
         if (p.timing) {
-            const unsigned long long t0 = clock64();
+            const uint32_t t0 = clock32();
             mbar_wait(bar, parity);
-            t_wait[slot] += clock64() - t0;
+            t_wait[slot] += clock32() - t0;
         } else {
             mbar_wait(bar, parity);
         }
@@ -463,12 +485,13 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
                     scale_d = 1;
                 }
                 wgmma_commit();
-                wgmma_wait<0>();
+                timed_wgmma_wait<0>(p.timing, t_wait[3]);
                 // every wgmma that read the stage has retired: it is free
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty_bar[stage]);
                 ++it;
             }
+            const uint32_t t_epi = p.timing ? clock32() : 0u;
             if (!WGRAD) asm volatile("bar.sync 1, %0;" ::"n"(CONS_WARPS * 32) : "memory");     // s_bias written
             // ---- epilogue on the fragments: rows rbase (h = 0) and rbase + 8 (h = 1)
             bool live[2];
@@ -517,6 +540,27 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
             }
 #pragma unroll
             for (int cc = 0; cc < NC; ++cc) {
+                // the ReLU mask of these 32 columns, all its words loaded before any store (the mask and the outputs may alias
+                // as far as the compiler knows: a load issued after a store would wait out its whole latency, once per
+                // 8-column block and row) and kept as one bit per element, bit 4 (2 i + h) + e; bf16 > 0 <=> sign bit clear
+                // and not (+)zero
+                uint32_t keep = 0u;
+                if (!WGRAD && p.mask) {
+                    uint32_t mw[4][2];
+#pragma unroll
+                    for (int i = 0; i < 4; ++i)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            mw[i][h] = live[h] ? *reinterpret_cast<const uint32_t *>(p.mask + mrow[h] + 32 * cc + 8 * i + cq) : 0u;
+#pragma unroll
+                    for (int i = 0; i < 4; ++i)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const uint32_t lo16 = mw[i][h] & 0xffffu, hi16 = mw[i][h] >> 16;
+                            keep |= (uint32_t)(lo16 != 0u && lo16 < 0x8000u) << (4 * (2 * i + h));
+                            keep |= (uint32_t)(hi16 != 0u && hi16 < 0x8000u) << (4 * (2 * i + h) + 1);
+                        }
+                }
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const int c = 32 * cc + 8 * i + cq;                        // columns c, c + 1
@@ -532,14 +576,8 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
                             if (!WGRAD) {
                                 v[e] += s_bias[c + e];
                                 if (p.relu) v[e] = fmaxf(v[e], 0.f);
+                                if (p.mask && !((keep >> (4 * (2 * i + h) + e)) & 1u)) v[e] = 0.f;
                             }
-                        }
-                        if (!WGRAD && p.mask && live[h]) {
-                            // bf16 > 0  <=>  sign bit clear and not (+)zero
-                            const uint32_t mw = *reinterpret_cast<const uint32_t *>(p.mask + mrow[h] + c);
-                            const uint32_t lo16 = mw & 0xffffu, hi16 = mw >> 16;
-                            if (!(lo16 != 0u && lo16 < 0x8000u)) v[0] = 0.f;
-                            if (!(hi16 != 0u && hi16 < 0x8000u)) v[1] = 0.f;
                         }
                         if (live[h]) {
                             if (p.out_f32) *reinterpret_cast<float2 *>(p.out_f32 + orow[h] + c) = make_float2(v[0], v[1]);
@@ -574,6 +612,7 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
                     p.colsum[(mt * p.n_tiles + nt) * (int64_t)N + i] = s;
                 }
             }
+            if (p.timing) t_wait[4] += clock32() - t_epi;
           }
           if (halo) {
               __syncwarp();                                   // every MMA of this tile has retired (wait above)
@@ -583,10 +622,10 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
         }
     }
     if (p.timing && blockIdx.x < 160) {
-        const unsigned long long tot = clock64() - t_begin;
+        const unsigned long long now = clock64();
         unsigned long long *o = xb_k12_timing[blockIdx.x];
-        if (tid == 0) o[0] = tot, o[1] = t_wait[0], o[3] = t_wait[2];
-        if (warp == CONS_WARPS && lane == 0) o[4] = tot, o[5] = t_wait[0], o[6] = t_wait[1];
+        if (tid == 0) o[0] = now - o[0], o[1] = t_wait[0], o[2] = t_wait[3], o[3] = t_wait[2], o[7] = t_wait[4];
+        if (tid == CONS_WARPS * 32) o[4] = now - o[4], o[5] = t_wait[0], o[6] = t_wait[1];
     }
 }
 
