@@ -283,6 +283,30 @@ int xb_sacdis_critic_loss(const float *q1, const float *q2, const float *actions
                           float gamma, int64_t B, int A, int64_t B_total, float *dq1, float *dq2, float *backup,
                           float *stats, double *scratch, void *stream);
 
+/* ---------------------------------------------------------------- K8T: DDPG / TD3 stages --------------
+ * Replaces the elementwise/reduction parts of DDPG_Learner.update / TD3_Learner.update (xuance/torch/learners/
+ * policy_gradient/{ddpg,td3}_learner.py) and the action noise of core/off_policy.py:142-144 and
+ * TwinDelayedActorCritic.Qtarget (actor_critic.py:289-296).  float32 throughout; the elementwise outputs are
+ * bit-identical to torch's expressions (no FMA contraction); NaN propagates as in torch.clamp / minimum / maximum.
+ * perturb: a, noise, out [B, D] row-major, low / high [D].  n = noise*scale; if noise_clip >= 0, n is clamped to
+ *          [-noise_clip, noise_clip]; out = clamp(a + n, low[j], high[j]).  `out` may alias `a`.  The noise is a
+ *          standard normal tensor the caller draws (torch.randn_like), so the random stream stays torch's.
+ * critic: q2, tq2, dq2 all NULL (DDPG, one critic) or all non-NULL (TD3, twin critics); a mix is XB_EINVAL.
+ *         t = tq1 or min(tq1, tq2); backup = rew + (gamma*(1 - term))*t; q_loss = sum_i mse(q_i, backup).
+ *         Writes backup[B], dq_i = 2*(q_i - backup)/B_total, stats[4] = {Qloss (the per-critic means added in
+ *         float32), mean(q1), mean(q2) (0 for DDPG), 0}.
+ * actor : DDPG: p_loss = -mean(q1), dq1 = -1/B_total.  TD3 (q2, dq2 non-NULL): p_loss = -mean((q1 + q2)/2) (the row's
+ *         half-sum rounded in float32), dq1 = dq2 = (-1/B_total)*0.5.  stats[4] = {Ploss, 0, 0, 0}.
+ * Both losses: B_total >= B rows scale the means (a SUM all-reduce of shards gives the global values); scratch as for
+ * K4.  XB_EINVAL on NULL pointers, B <= 0, B_total < B or D <= 0. */
+int xb_perturb_actions(const float *a, const float *noise, int64_t B, int D, float scale, float noise_clip,
+                       const float *low, const float *high, float *out, void *stream);
+int xb_ddpg_critic_loss(const float *q1, const float *q2, const float *tq1, const float *tq2, const float *rew,
+                        const float *term, float gamma, int64_t B, int64_t B_total, float *dq1, float *dq2,
+                        float *backup, float *stats, double *scratch, void *stream);
+int xb_ddpg_actor_loss(const float *q1, const float *q2, int64_t B, int64_t B_total, float *dq1, float *dq2,
+                       float *stats, double *scratch, void *stream);
+
 /* ---------------------------------------------------------------- K7: flat-bucket optimiser step -----
  * Replaces clip_grad_norm_ + torch.optim.Adam.step on the learner's parameters (ppo_learner.py:61-65;
  * Adam eps=1e-5, no weight decay, no amsgrad) over ONE flat float32 bucket (params/grads/exp_avg/exp_avg_sq

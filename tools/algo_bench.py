@@ -4,8 +4,9 @@ DQN+PER (2^20-transition HBM replay, B=512), SAC (1M replay, B=1024) and QMIX (5
 on one GPU, next to the oracle port of the reference's torch-CPU path on the host; and ``ppo_gauss``, continuous-control
 PPO in the shape of the reference's ppo/mujoco.yaml (train_epochs env-steps/s); ``mappo``, MAPPO in the shape of
 configs/mappo/sc2/5m_vs_6m.yaml (train_epochs env-steps/s); ``sacdis``, SAC-Discrete in the shape of
-configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (train_epochs, eager and graphed).  Prints one
-JSON object.
+configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (train_epochs, eager and graphed); ``ddpg`` and
+``td3``, DDPG / TD3 in the shape of the reference's ddpg/mujoco.yaml and td3/mujoco.yaml (sample + update, eager and
+graphed).  Prints one JSON object.
 
     python tools/algo_bench.py [--iters 200] [--cpu-iters 5] [--no-cpu] [--graph]
     torchrun --nnodes=1 --nproc-per-node G --master-addr 127.0.0.1 tools/algo_bench.py --no-cpu --graph    (G GPUs)
@@ -335,6 +336,65 @@ def bench_sacdis(args):
     return out
 
 
+def bench_ddpg_td3(args, algo):
+    """DDPG / TD3 in the shape of the reference's ddpg/mujoco.yaml and td3/mujoco.yaml: 17-d observations, 6 action
+    components, Basic_Identical representation, actor and critic MLPs [400, 300] with leaky_relu, B = 100 (DDPG) or 256
+    (TD3, actor_update_delay 2: the time is the mean over critic-only and actor iterations).  One replay sample + one
+    update, eager and CUDA-graphed, next to the torch-CPU oracle's update on the host."""
+    from copy import deepcopy
+    from xuance_b200 import _lib
+    from xuance_b200.common import DummyOffPolicyBuffer, Box, BaseCallback
+    from xuance_b200.torch.rl_models import (Basic_Identical, DeterministicActor, ActionValueCritic, TwinActionValueCritic,
+                                             DeterministicActorCritic, TwinDelayedActorCritic)
+    from xuance_b200.torch.learners import REGISTRY_Learners
+    twin = algo == "td3"
+    N, S, B, od, ad = 4, 250000, 256 if twin else 100, 17, 6
+    aspace = Box(-1, 1, (ad,), np.float32)
+    res = {"config": "%s, 17-d obs / 6-d act, 1M replay, B=%d, Basic_Identical + MLP 400-300 leaky_relu%s"
+                     % (algo.upper(), B, ", actor_update_delay 2" if twin else "")}
+    for graph in (False, True):
+        buf = DummyOffPolicyBuffer(Box(-10, 10, (od,), np.float32), aspace, None, N, N * S, B, device=DEV)
+        buf._obs.normal_(), buf._next_obs.normal_(), buf._act_rows.uniform_(-1, 1), buf._fields.normal_()
+        buf.size = S
+        rep = Basic_Identical((od,), device=DEV)
+        actor = DeterministicActor(rep, [400, 300], aspace, None, None, nn.LeakyReLU, nn.Tanh, DEV)
+        if twin:
+            model = TwinDelayedActorCritic(actor, TwinActionValueCritic(deepcopy(rep), aspace, [400, 300], None, None,
+                                                                        nn.LeakyReLU, DEV))
+        else:
+            model = DeterministicActorCritic(actor, ActionValueCritic(deepcopy(rep), aspace, [400, 300], None, None,
+                                                                      nn.LeakyReLU, DEV))
+        cfg = Namespace(distributed_training=False, episode_length=1000, use_grad_clip=False, grad_clip_norm=0.5,
+                        device=DEV, model_dir="/tmp/x", running_steps=10**6, parallels=N, start_training=0,
+                        training_frequency=1, learning_rate_actor=1e-3, learning_rate_critic=1e-3, tau=0.005,
+                        gamma=0.99, actor_update_delay=2, use_cuda_graph=graph)
+        lrn = REGISTRY_Learners["TD3_Learner" if twin else "DDPG_Learner"](cfg, model.to(DEV), BaseCallback())
+        if not graph:
+            lrn.update(sync=False, **buf.sample())
+            before = _lib.launch_count
+            lrn.update(sync=False, **buf.sample())
+            lrn.update(sync=False, **buf.sample())
+            res["xb_launches_per_2_updates"] = _lib.launch_count - before
+        dt = timed(lambda: lrn.update(sync=False, **buf.sample()), args.iters)
+        res["gpu_%s_ms_per_update" % ("graphed" if graph else "eager")] = dt * 1e3
+        res["gpu_%s_updates_per_s" % ("graphed" if graph else "eager")] = 1 / dt
+    if not args.no_cpu:
+        from oracle_ddpg import DDPGModelOracle, DDPGLearnerOracle
+        ol = DDPGLearnerOracle(DDPGModelOracle(od, ad, -np.ones(ad, np.float32), np.ones(ad, np.float32), twin, (),
+                                               (400, 300), (400, 300), act=nn.LeakyReLU),
+                               actor_update_delay=2 if twin else 1)
+        rng = np.random.default_rng(0)
+        s = {"obs": rng.normal(size=(B, od)).astype(np.float32), "obs_next": rng.normal(size=(B, od)).astype(np.float32),
+             "actions": rng.uniform(-1, 1, (B, ad)).astype(np.float32), "rewards": rng.random(B).astype(np.float32),
+             "terminals": (rng.random(B) < 0.05).astype(np.float32)}
+        noise = rng.normal(size=(B, ad)).astype(np.float32) if twin else None
+        cdt = cpu_timed(lambda: ol.update(noise_next=noise, **s), max(args.cpu_iters, 20))
+        res.update(cpu_ms_per_update=cdt * 1e3, cpu_threads=torch.get_num_threads(),
+                   speedup_eager=cdt / (res["gpu_eager_ms_per_update"] / 1e3),
+                   speedup_graphed=cdt / (res["gpu_graphed_ms_per_update"] / 1e3))
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=200)
@@ -368,6 +428,9 @@ def main():
         res["mappo"] = bench_mappo(args)
     if (not only and WORLD == 1) or "sacdis" in only:
         res["sacdis"] = bench_sacdis(args)
+    for algo in ("ddpg", "td3"):
+        if (not only and WORLD == 1) or algo in only:
+            res[algo] = bench_ddpg_td3(args, algo)
     res["cuda_graph"] = bool(args.graph)
     res["n_gpus"] = WORLD
     if RANK == 0:

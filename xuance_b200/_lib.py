@@ -74,6 +74,9 @@ _SIGNATURES = {
     "xb_sacdis_actor_loss": (c_int, [_P, _P, _P, _P, c_int64, c_int, c_int64, _P, _P, _P, _P]),
     "xb_sacdis_critic_loss": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_float, c_int64, c_int, c_int64, _P, _P, _P,
                                       _P, _P, _P]),
+    "xb_perturb_actions": (c_int, [_P, _P, c_int64, c_int, c_float, c_float, _P, _P, _P, _P]),
+    "xb_ddpg_critic_loss": (c_int, [_P, _P, _P, _P, _P, _P, c_float, c_int64, c_int64, _P, _P, _P, _P, _P, _P]),
+    "xb_ddpg_actor_loss": (c_int, [_P, _P, c_int64, c_int64, _P, _P, _P, _P, _P]),
     "xb_qmix_select_fwd": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     "xb_qmix_select_bwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
     "xb_qmix_mix_fwd": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int, c_int, _P, _P]),

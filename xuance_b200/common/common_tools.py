@@ -26,7 +26,9 @@ def get_arguments(algo, env, env_id=None, config_path=None, parser_args=None):
     """``algo`` e.g. 'ppo', ``env`` e.g. 'atari' / 'classic_control', ``env_id`` e.g. 'CartPole-v1'."""
     cfg = load_yaml(os.path.join(_CONFIG_ROOT, "basic.yaml"))
     if config_path is None:
-        cands = [os.path.join(_CONFIG_ROOT, algo, f"{env_id}.yaml"), os.path.join(_CONFIG_ROOT, algo, f"{env}.yaml")]
+        # the third candidate is the reference's own layout, configs/<algo>/<env>/<env_id>.yaml
+        cands = [os.path.join(_CONFIG_ROOT, algo, f"{env_id}.yaml"), os.path.join(_CONFIG_ROOT, algo, f"{env}.yaml"),
+                 os.path.join(_CONFIG_ROOT, algo, env, f"{env_id}.yaml")]
         found = [c for c in cands if os.path.exists(c)]
         if not found:
             raise AttributeError(f"no config for algo={algo} env={env} env_id={env_id} under {_CONFIG_ROOT}")

@@ -8,6 +8,9 @@ REGISTRY_Agents = {"PPO": PPO_Agent, "PPO_Clip": PPO_Agent, "DQN": DQN_Agent, "P
 try:
     from .sac_agent import SAC_Agent
     REGISTRY_Agents["SAC"] = SAC_Agent
+    from .ddpg_agent import DDPG_Agent, TD3_Agent
+    REGISTRY_Agents["DDPG"] = DDPG_Agent
+    REGISTRY_Agents["TD3"] = TD3_Agent
 except ImportError:
     pass
 from .marl import MARLAgents, OffPolicyMARLAgents, QMIX_Agents, VDN_Agents

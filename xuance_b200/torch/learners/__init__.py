@@ -10,6 +10,9 @@ try:
     REGISTRY_Learners["SAC_Learner"] = SAC_Learner
     from .sacdis_learner import SACDIS_Learner
     REGISTRY_Learners["SACDIS_Learner"] = SACDIS_Learner
+    from .ddpg_learner import DDPG_Learner, TD3_Learner
+    REGISTRY_Learners["DDPG_Learner"] = DDPG_Learner
+    REGISTRY_Learners["TD3_Learner"] = TD3_Learner
 except ImportError:
     pass
 try:

@@ -1,10 +1,13 @@
 from .layers import mlp_block, cnn_block, ActivationFunctions
-from .outputs import ModelOutput, RepresentationOutput, ActionOutput, StochasticActorOutput, TwinCriticOutput
+from .outputs import (ModelOutput, RepresentationOutput, ActionOutput, StochasticActorOutput, TwinCriticOutput,
+                      DeterministicActorOutput, CriticOutput)
 from .distributions import CategoricalDistribution, DiagGaussianDistribution, ActivatedDiagGaussianDistribution
 from .representations import Basic_Identical, Basic_MLP, Basic_CNN, AC_CNN_Atari, REGISTRY_Representation
-from .heads import CategoricalActorHead, GaussianActorHead, SAC_GaussianActorHead, ValueHead, QValueHead, DuelingQValueHead
+from .heads import (CategoricalActorHead, GaussianActorHead, SAC_GaussianActorHead, ValueHead, QValueHead, DuelingQValueHead,
+                    DeterministicActorHead)
 from .architectures import (ActorCritic, SharedActorCritic, DeepQNetwork, DuelingDeepQNetwork, GaussianActor, SAC_GaussianActor,
-                            TwinActionValueCritic, SoftActorCritic, TwinDiscreteActionValueCritic, SoftActorCriticDiscrete)
+                            TwinActionValueCritic, SoftActorCritic, TwinDiscreteActionValueCritic, SoftActorCriticDiscrete,
+                            DeterministicActor, ActionValueCritic, DeterministicActorCritic, TwinDelayedActorCritic)
 from .qmix import Basic_RNN, AgentFeatureEncoder, DiscreteActionValueCritic, QMIX_Mixer, VDN_mixer, MixingQNetwork
 REGISTRY_Representation["Basic_RNN"] = Basic_RNN
 from .mappo import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic

@@ -8,8 +8,9 @@ import torch
 import torch.nn as nn
 
 from ...common.spaces import is_discrete
-from .heads import DuelingQValueHead, QValueHead, SAC_GaussianActorHead, GaussianActorHead, ValueHead
-from .outputs import ModelOutput, StochasticActorOutput, TwinCriticOutput
+from .heads import (DuelingQValueHead, QValueHead, SAC_GaussianActorHead, GaussianActorHead, ValueHead,
+                    DeterministicActorHead)
+from .outputs import ModelOutput, StochasticActorOutput, TwinCriticOutput, DeterministicActorOutput, CriticOutput
 
 
 class ActorCritic(nn.Module):
@@ -260,3 +261,138 @@ class SoftActorCriticDiscrete(SoftActorCritic):
     def Qaction(self, observation, *args, **kwargs):
         out = self.critic(observation)
         return out.values_1, out.values_2
+
+
+class DeterministicActor(nn.Module):
+    """actors/deterministic_actors.py:10-52.  ``action_low`` / ``action_high`` are float32 device tensors (plain
+    attributes, as in the reference, so they are not part of the state_dict)."""
+
+    actor_head_cls = DeterministicActorHead
+
+    def __init__(self, representation, actor_hidden_size, action_space=None, normalizer=None, initializer=None,
+                 activation=None, activation_action=None, device=None, **kwargs):
+        super().__init__()
+        if is_discrete(action_space) or not hasattr(action_space, "low"):
+            raise ValueError('action_space must be Box')
+        self.action_space = action_space
+        self.action_dim = action_space.shape[0]
+        self.action_low = torch.as_tensor(action_space.low, dtype=torch.float32, device=device)
+        self.action_high = torch.as_tensor(action_space.high, dtype=torch.float32, device=device)
+        self.representation = representation
+        self.representation_info_shape = representation.output_shapes
+        self.actor_head = self.actor_head_cls(feature_dim=self.representation_info_shape['state'][0],
+                                              hidden_size=actor_hidden_size, action_dim=self.action_dim,
+                                              normalizer=normalizer, initializer=initializer, activation=activation,
+                                              activation_action=activation_action, device=device)
+
+    def forward(self, observation, **kwargs):
+        rep_out = self.representation(observation, **kwargs)
+        return DeterministicActorOutput(representations=rep_out, actions=self.actor_head(rep_out.embeddings, **kwargs))
+
+
+class ActionValueCritic(nn.Module):
+    """critics/base_critics.py:47-88: Q(s, a) = ValueHead(concat(features, action))."""
+
+    def __init__(self, representation, action_space, critic_hidden_size, normalizer=None, initializer=None,
+                 activation=None, device=None, **kwargs):
+        super().__init__()
+        if is_discrete(action_space) or not hasattr(action_space, "low"):
+            raise ValueError('action_space must be Box.')
+        self.action_space = action_space
+        self.action_dim = action_space.shape[-1]
+        self.representation = representation
+        self.representation_info_shape = representation.output_shapes
+        self.critic_head = ValueHead(feature_dim=self.representation_info_shape['state'][0] + self.action_dim,
+                                     hidden_size=critic_hidden_size, normalizer=normalizer, initializer=initializer,
+                                     activation=activation, device=device)
+
+    def forward(self, observations, actions, **kwargs):
+        rep_out = self.representation(observations, **kwargs)
+        return CriticOutput(representations=rep_out,
+                            values=self.critic_head(torch.concat([rep_out.embeddings, actions], dim=-1)))
+
+
+class DeterministicActorCritic(nn.Module):
+    """actor_critic.py:217-261: actor, critic and their deep-copied targets.  ``Qtarget_pair`` / ``Qpolicy_pair`` give
+    the learner the raw critic outputs ((q, None) for one critic); the losses run in the K8T kernels."""
+
+    def __init__(self, actor, critic, **kwargs):
+        super().__init__()
+        self.actor, self.critic = actor, critic
+        self.target_actor = deepcopy(actor)
+        self.target_critic = deepcopy(critic)
+
+    def forward(self, observations, **kwargs):
+        a = self.actor(observations, **kwargs)
+        c = self.critic(observations, a.actions, **kwargs)
+        return ModelOutput(actions=a.actions, values=c.values, actor_rep_out=a.representations,
+                           critic_rep_out=c.representations)
+
+    def act(self, observation, **kwargs):
+        return self.actor(observation, **kwargs).actions
+
+    def Qtarget_pair(self, observation, noise=None):
+        return self.target_critic(observation, self.target_actor(observation).actions).values, None
+
+    def Qpolicy_pair(self, observation):
+        return self.critic(observation, self.actor(observation).actions).values, None
+
+    def Qtarget(self, observation):
+        return self.Qtarget_pair(observation)[0]
+
+    def Qaction(self, observations, actions):
+        return self.critic(observations, actions).values
+
+    def Qpolicy(self, observation):
+        return self.Qpolicy_pair(observation)[0]
+
+    def soft_update(self, tau=0.005):
+        for src, dst in ((self.actor, self.target_actor), (self.critic, self.target_critic)):
+            for ep, tp in zip(src.parameters(), dst.parameters()):
+                tp.data.mul_(1 - tau)
+                tp.data.add_(tau * ep.data)
+
+
+class TwinDelayedActorCritic(DeterministicActorCritic):
+    """actor_critic.py:264-319 over a TwinActionValueCritic.  Target-policy smoothing runs in K8T
+    ``xb_perturb_actions``: clamp(a' + clip(noise*target_policy_noise, +-target_noise_clip), action_low, action_high)
+    with ``noise`` a standard normal [B, action_dim] tensor (drawn with torch.randn_like when not given)."""
+
+    def __init__(self, actor, critic, target_policy_noise=0.2, target_noise_clip=0.5, **kwargs):
+        super().__init__(actor, critic, **kwargs)
+        self.target_policy_noise = target_policy_noise
+        self.target_noise_clip = target_noise_clip
+
+    def forward(self, observation, **kwargs):
+        a = self.actor(observation)
+        return ModelOutput(actions=a.actions, actor_rep_out=a.representations)
+
+    def smoothed_target_actions(self, observation, noise=None):
+        from ... import _lib
+        ta = self.target_actor(observation).actions.contiguous()
+        noise = torch.randn_like(ta) if noise is None else noise.to(torch.float32).contiguous()
+        out = torch.empty_like(ta)
+        B, D = ta.shape
+        _lib.call("xb_perturb_actions", _lib.ptr(ta), _lib.ptr(noise), B, D, float(self.target_policy_noise),
+                  float(self.target_noise_clip), _lib.ptr(self.actor.action_low), _lib.ptr(self.actor.action_high),
+                  _lib.ptr(out))
+        return out
+
+    def Qtarget_pair(self, observation, noise=None):
+        out = self.target_critic(observation, self.smoothed_target_actions(observation, noise))
+        return out.values_1, out.values_2
+
+    def Qpolicy_pair(self, observation):
+        out = self.critic(observation, self.actor(observation).actions)
+        return out.values_1, out.values_2
+
+    def Qtarget(self, observation, noise=None):
+        return torch.minimum(*self.Qtarget_pair(observation, noise))
+
+    def Qaction(self, observations, actions):
+        out = self.critic(observations, actions)
+        return out.values_1, out.values_2
+
+    def Qpolicy(self, observation):
+        q1, q2 = self.Qpolicy_pair(observation)
+        return (q1 + q2) / 2.0

@@ -71,6 +71,23 @@ class SAC_GaussianActorHead(nn.Module):
         return self.policy_distribution
 
 
+class DeterministicActorHead(nn.Module):
+    """actor_head.py:108-135: hidden layers, then Linear(action_dim) + activation_action (tanh in every shipped config)."""
+
+    def __init__(self, feature_dim, hidden_size, action_dim, normalizer=None, initializer=None, activation=None,
+                 activation_action=None, device=None, **kwargs):
+        super().__init__()
+        layers, shape = _stack(feature_dim, hidden_size, normalizer, activation, initializer, device)
+        layers.extend(mlp_block(shape[0], action_dim, None, activation_action, initializer, device)[0])
+        self.model = nn.Sequential(*layers)
+
+    def forward(self, features, avail_actions=None, **kwargs):
+        actions = self.model(features)
+        if avail_actions is not None:
+            actions[avail_actions == 0] = 0
+        return actions
+
+
 class ValueHead(nn.Module):
     """critic_head.py:9-30."""
 

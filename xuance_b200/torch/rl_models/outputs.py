@@ -17,6 +17,18 @@ class StochasticActorOutput:
 
 
 @dataclass
+class DeterministicActorOutput:
+    representations: Any
+    actions: Any = None
+
+
+@dataclass
+class CriticOutput:
+    representations: Any
+    values: Any = None
+
+
+@dataclass
 class TwinCriticOutput:
     representations_1: Any
     representations_2: Any
