@@ -201,6 +201,36 @@ int xb_dqn_td_fwd_bwd(const float *q_eval, const float *q_next, const float *q_s
                       const float *term, int64_t B, int A, int64_t B_total, float gamma,
                       float *dq, float *td, float *stats, double *scratch, void *stream);
 
+/* ---------------------------------------------------------------- K6Z: C51 / QR-DQN head tail + loss ---
+ * z [B, A, N] float32 row-major is a head's raw output viewed as rows x actions x atoms (C51 logits) or quantiles
+ * (QR).  Supported: 2 <= N <= 64 atoms / quantiles, 1 <= A <= 256 actions; anything else (and N < 2, where the
+ * reference divides by zero) is XB_EINVAL, as are NULL required pointers and B <= 0.  One warp per row.
+ * greedy: replaces deep_q_network.py:202-203 / 230-231 (C51: supports != NULL, Q = sum_i supports_i*softmax(z)_i) and
+ *         :289-290 / 317-318 (QR: supports == NULL, Q = mean_i z_i) under no_grad.  Writes actions[B] int64, the first
+ *         maximal index as torch.argmax; optional q[B, A] and (C51 only, else XB_EINVAL) probs[B, A, N].
+ * c51   : replaces c51_learner.py:38-51 and its autograd to the eval logits.  Target action = the greedy action of
+ *         z_next (the same device routine as greedy); Tz = clamp(rew + (gamma*z)*(1 - ter), v_min, v_max);
+ *         target_i = sum_j p'_j * clamp(1 - |Tz_j - z_i| / delta_z, 0, 1); p = softmax(z_eval[b, a_b]);
+ *         loss = mean_b -sum_i target_i*log(p_i + 1e-8).  Writes dlogits[B, A, N] (the taken row
+ *         p*(g - sum p*g), g_i = ((-1/B_total)*target_i)/(p_i + 1e-8); the other rows 0), target_actions[B]
+ *         int64, the optional target_dist[B, N] (the projected target, as the reference hands it to on_update_end;
+ *         NULL skips it) and stats[4] = {Qloss, 0, 0, 0}.  supports[N] is the model's tensor.
+ * qrdqn : replaces qrdqn_learner.py:40-48 and its autograd.  Target action = argmax_a mean(z_next[b, a]);
+ *         y = rew + (gamma*theta')*(1 - ter); loss = mse(y, z_eval[b, a_b]) over B_total*N.  Writes dq[B, A, N]
+ *         (2*(theta - y)/(B_total*N) on the taken row, 0 elsewhere), target_actions[B], stats[4] = {Qloss,0,0,0}.
+ * Both losses: actions are float32 as stored; a row whose action is not in [0, A) gets zero gradient and makes Qloss
+ * NaN.  Tz, the projection weights and the QR backup are bit-identical to torch's float32 expressions.  B_total >= B
+ * rows scale the means (a SUM all-reduce of shards gives the global values); scratch as for K4. */
+int xb_dist_greedy(const float *z, const float *supports, int64_t B, int A, int N, int64_t *actions, float *q,
+                   float *probs, void *stream);
+int xb_c51_loss_fwd_bwd(const float *z_eval, const float *z_next, const float *supports, const float *actions,
+                        const float *rew, const float *ter, int64_t B, int A, int N, int64_t B_total, float gamma,
+                        float v_min, float v_max, float delta_z, float *dlogits, int64_t *target_actions,
+                        float *target_dist, float *stats, double *scratch, void *stream);
+int xb_qrdqn_loss_fwd_bwd(const float *z_eval, const float *z_next, const float *actions, const float *rew,
+                          const float *ter, int64_t B, int A, int N, int64_t B_total, float gamma, float *dq,
+                          int64_t *target_actions, float *stats, double *scratch, void *stream);
+
 /* ---------------------------------------------------------------- K9: QMIX selection / mixing / TD ----
  * Replaces, for one parameter-sharing group with use_rnn=True (episodes padded to T, `filled` mask):
  * select  : qmix_learner.py:42-66 + iql_learner.py:57-59 - gather Q(o_t, a_t) from the eval net outputs

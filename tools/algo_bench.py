@@ -6,7 +6,8 @@ PPO in the shape of the reference's ppo/mujoco.yaml (train_epochs env-steps/s); 
 configs/mappo/sc2/5m_vs_6m.yaml (train_epochs env-steps/s); ``sacdis``, SAC-Discrete in the shape of
 configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (train_epochs, eager and graphed); ``ddpg`` and
 ``td3``, DDPG / TD3 in the shape of the reference's ddpg/mujoco.yaml and td3/mujoco.yaml (sample + update, eager and
-graphed).  Prints one JSON object.
+graphed); ``c51`` and ``qrdqn`` on CartPole (Basic_MLP 128, B=256) and SyntheticAtari (Basic_CNN, B=32) shapes (update,
+eager and graphed).  Prints one JSON object.
 
     python tools/algo_bench.py [--iters 200] [--cpu-iters 5] [--no-cpu] [--graph]
     torchrun --nnodes=1 --nproc-per-node G --master-addr 127.0.0.1 tools/algo_bench.py --no-cpu --graph    (G GPUs)
@@ -395,6 +396,67 @@ def bench_ddpg_td3(args, algo):
     return res
 
 
+def bench_dist_dqn(args, algo):
+    """C51 / QR-DQN updates at the shapes of the shipped configs: CartPole-v1 (4-d observations, 2 actions, Basic_MLP [128]
+    + head [128], B = 256) and SyntheticAtari (84x84x4 uint8, 4 actions, Basic_CNN 32-64-64 + head [512], B = 32; fp32
+    cuDNN encoder).  One update on a fixed batch, eager and CUDA-graphed, with the xb200 launches per update, next to the
+    torch-CPU oracle's update on the host at the same shape."""
+    from xuance_b200 import _lib
+    from xuance_b200.common import Discrete, BaseCallback
+    from xuance_b200.torch.rl_models import Basic_MLP, Basic_CNN, C51DeepQNetwork, QRDeepQNetwork
+    from xuance_b200.torch.learners import REGISTRY_Learners
+    N = 51 if algo == "c51" else 20
+    res = {}
+    rng = np.random.default_rng(0)
+    for shape, B, A in (("cartpole", 256, 2), ("atari", 32, 4)):
+        r = {"config": "%s %s: B=%d, A=%d, N=%d" % (algo.upper(), shape, B, A, N)}
+        if shape == "cartpole":
+            obs = lambda: rng.normal(size=(B, 4)).astype(np.float32)
+        else:
+            obs = lambda: rng.integers(0, 256, (B, 84, 84, 4), dtype=np.uint8)
+        s = {"obs": obs(), "obs_next": obs(), "actions": rng.integers(0, A, B).astype(np.float32),
+             "rewards": rng.normal(size=B).astype(np.float32), "terminals": (rng.random(B) < 0.05).astype(np.float32)}
+        s_dev = {k: torch.as_tensor(v, device=DEV) for k, v in s.items()}
+        for graph in (False, True):
+            if shape == "cartpole":
+                rep = Basic_MLP((4,), [128], None, nn.init.orthogonal_, nn.ReLU, DEV)
+                hidden = [128]
+            else:
+                rep = Basic_CNN((84, 84, 4), kernels=[8, 4, 3], strides=[4, 2, 1], filters=[32, 64, 64], normalize=None,
+                                initialize=nn.init.orthogonal_, activation=nn.ReLU, device=DEV)
+                hidden = [512]
+            if algo == "c51":
+                model = C51DeepQNetwork(rep, hidden, Discrete(A), N, 0, 200, None, nn.init.orthogonal_, nn.ReLU, DEV)
+            else:
+                model = QRDeepQNetwork(rep, hidden, Discrete(A), N, None, nn.init.orthogonal_, nn.ReLU, DEV)
+            cfg = Namespace(distributed_training=False, episode_length=1000, use_grad_clip=False, grad_clip_norm=0.5,
+                            device=DEV, model_dir="/tmp/x", running_steps=10**6, parallels=10, start_training=0,
+                            training_frequency=1, learning_rate=1e-3, gamma=0.99, sync_frequency=100,
+                            use_cuda_graph=graph)
+            lrn = REGISTRY_Learners["C51_Learner" if algo == "c51" else "QRDQN_Learner"](cfg, model.to(DEV),
+                                                                                         BaseCallback())
+            if not graph:
+                lrn.update(sync=False, **s_dev)
+                before = _lib.launch_count
+                lrn.update(sync=False, **s_dev)
+                r["xb_launches_per_update"] = _lib.launch_count - before
+            dt = timed(lambda: lrn.update(sync=False, **s_dev), args.iters)
+            r["gpu_%s_ms_per_update" % ("graphed" if graph else "eager")] = dt * 1e3
+        if not args.no_cpu:
+            from oracle_dist import DistModelOracle, DistLearnerOracle
+            if shape == "cartpole":
+                om = DistModelOracle(algo, 4, A, N, (128,), (128,), 0, 200)
+            else:
+                om = DistModelOracle(algo, None, A, N, q_hidden=(512,), v_min=0, v_max=200, pixels=True)
+            ol = DistLearnerOracle(om, sync_frequency=100)
+            cdt = cpu_timed(lambda: ol.update(**s), max(args.cpu_iters, 20))
+            r.update(cpu_ms_per_update=cdt * 1e3, cpu_threads=torch.get_num_threads(),
+                     speedup_eager=cdt / (r["gpu_eager_ms_per_update"] / 1e3),
+                     speedup_graphed=cdt / (r["gpu_graphed_ms_per_update"] / 1e3))
+        res[shape] = r
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=200)
@@ -431,6 +493,9 @@ def main():
     for algo in ("ddpg", "td3"):
         if (not only and WORLD == 1) or algo in only:
             res[algo] = bench_ddpg_td3(args, algo)
+    for algo in ("c51", "qrdqn"):
+        if (not only and WORLD == 1) or algo in only:
+            res[algo] = bench_dist_dqn(args, algo)
     res["cuda_graph"] = bool(args.graph)
     res["n_gpus"] = WORLD
     if RANK == 0:

@@ -138,6 +138,32 @@ def main():
                                           _lib.ptr(stats), _lib.ptr(scratch)), R)
             add(entry("K4 xb_ppo_loss_fwd_bwd", f"B={B}, A=4", us, B * 56, hbm))
 
+    if want("k6z"):
+        # C51 / QR-DQN at the config shapes: CartPole (B=256, A=2), SyntheticAtari (B=32, A=4), full ALE set (A=18).
+        # Algorithmic bytes per row: greedy 4*A*N in + 8 out; losses 8*A*N in (eval + target rows) + 12 scalars in,
+        # 4*A*N gradient + 8 target action out.
+        for B, A in ((256, 2), (32, 4), (32, 18)):
+            for algo, N in (("c51", 51), ("qrdqn", 20)):
+                z, zn = torch.randn((B, A, N), device=DEV), torch.randn((B, A, N), device=DEV)
+                sup = torch.linspace(-10, 10, N).to(DEV) if algo == "c51" else None
+                act = torch.randint(0, A, (B,), device=DEV).float()
+                rew, ter = torch.randn(B, device=DEV), (torch.rand(B, device=DEV) < 0.1).float()
+                grad, ga = torch.empty_like(z), torch.empty(B, dtype=torch.int64, device=DEV)
+                stats, scratch = torch.zeros(4, device=DEV), _lib.scratch(DEV)
+                us = timeit(lambda: _lib.call("xb_dist_greedy", _lib.ptr(z), _lib.ptr(sup), B, A, N, _lib.ptr(ga), None,
+                                              None), R)
+                add(entry("K6Z xb_dist_greedy (%s)" % algo, f"B={B}, A={A}, N={N}", us, B * (4 * A * N + 8), hbm))
+                if algo == "c51":
+                    fn = lambda: _lib.call("xb_c51_loss_fwd_bwd", _lib.ptr(z), _lib.ptr(zn), _lib.ptr(sup), _lib.ptr(act),
+                                           _lib.ptr(rew), _lib.ptr(ter), B, A, N, B, 0.99, -10.0, 10.0, 0.4,
+                                           _lib.ptr(grad), _lib.ptr(ga), None, _lib.ptr(stats), _lib.ptr(scratch))
+                else:
+                    fn = lambda: _lib.call("xb_qrdqn_loss_fwd_bwd", _lib.ptr(z), _lib.ptr(zn), _lib.ptr(act),
+                                           _lib.ptr(rew), _lib.ptr(ter), B, A, N, B, 0.99, _lib.ptr(grad), _lib.ptr(ga),
+                                           _lib.ptr(stats), _lib.ptr(scratch))
+                us = timeit(fn, R)
+                add(entry("K6Z xb_%s_loss_fwd_bwd" % algo, f"B={B}, A={A}, N={N}", us, B * (12 * A * N + 20), hbm))
+
     if want("k5"):
         N, cap, B = 16, 65536, 512
         k = B // N

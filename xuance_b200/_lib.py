@@ -43,6 +43,10 @@ _SIGNATURES = {
     "xb_per_sample": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int64, c_float, _P, _P, _P, _P]),
     "xb_per_update": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, _P]),
     "xb_dqn_td_fwd_bwd": (c_int, [_P, _P, _P, _P, _P, _P, c_int64, c_int, c_int64, c_float, _P, _P, _P, _P, _P]),
+    "xb_dist_greedy": (c_int, [_P, _P, c_int64, c_int, c_int, _P, _P, _P, _P]),
+    "xb_c51_loss_fwd_bwd": (c_int, [_P, _P, _P, _P, _P, _P, c_int64, c_int, c_int, c_int64, c_float, c_float, c_float,
+                                    c_float, _P, _P, _P, _P, _P, _P]),
+    "xb_qrdqn_loss_fwd_bwd": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int, c_int, c_int64, c_float, _P, _P, _P, _P, _P]),
     "xb_grad_sumsq": (c_int, [_P, c_int64, c_float, _P, _P, _P]),
     "xb_adam_step": (c_int, [_P, _P, _P, _P, c_int64, _P, c_float, c_float, c_float, c_float, _P, c_float,
                              c_int, _P]),
@@ -60,7 +64,8 @@ _SIGNATURES = {
                                 c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, c_int64, c_int, _P, c_int, c_int,
                                 c_int, c_int, _P, _P, c_int64, c_int, c_int, _P, _P]),
     "xb_debug_k12_timing": (c_int, [_P, c_int]),
-    "xb_debug_tma_box": (c_int, [_P, c_int64] + [c_int] * 12 + [ctypes.c_uint32, _P, ctypes.c_uint32, _P]),
+    "xb_debug_tma_box": (c_int, [_P, c_int64, c_int, c_int, c_int, c_int64] + [c_int] * 8
+                         + [ctypes.c_uint32, _P, ctypes.c_uint32, _P]),
     "xb_wgrad_box_tc": (c_int, [c_int, c_int, _P, c_int64, c_int, c_int, c_int64, c_int, c_int, c_int, c_int, c_int, _P, _P, _P,
                                 _P, c_int64, c_int64, c_int, c_int, _P, _P]),
     "xb_wgrad_gather_tc": (c_int, [c_int, c_int, _P, c_int64, _P, c_int64, c_int64] + [c_int] * 9 + [_P, _P, c_int, c_int, c_int,

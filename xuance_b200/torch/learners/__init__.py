@@ -1,10 +1,12 @@
 from .learner import Learner
 from .ppo_learner import PPO_Learner, A2C_Learner, PG_Learner
 from .dqn_learner import DQN_Learner, PerDQN_Learner, DDQN_Learner, DuelDQN_Learner
+from .dist_dqn_learner import C51_Learner, QRDQN_Learner
 
 REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner, "DQN_Learner": DQN_Learner,
                      "PerDQN_Learner": PerDQN_Learner, "DDQN_Learner": DDQN_Learner, "A2C_Learner": A2C_Learner,
-                     "PG_Learner": PG_Learner, "DuelDQN_Learner": DuelDQN_Learner}
+                     "PG_Learner": PG_Learner, "DuelDQN_Learner": DuelDQN_Learner,
+                     "C51_Learner": C51_Learner, "QRDQN_Learner": QRDQN_Learner}
 try:
     from .sac_learner import SAC_Learner
     REGISTRY_Learners["SAC_Learner"] = SAC_Learner

@@ -82,8 +82,7 @@ class DQN_Learner(Learner):
         if self.iterations % self.sync_frequency == 0:
             self.model.copy_target()
         if sync:
-            s = self._stats.tolist()
-            vals = {"Qloss": s[0], "learning_rate": self.optimizer.param_groups[0]['lr'], "predictQ": s[1]}
+            vals = self._info_values()
             if self.distributed_training:
                 vals = {f"{k}/rank_{self.rank}": v for k, v in vals.items()}
             info.update(vals)
@@ -91,6 +90,11 @@ class DQN_Learner(Learner):
         if self.returns_td:
             return abs_td, info   # |td| stays on the device; PerOffPolicyBuffer.update_priorities takes it as is
         return info
+
+    def _info_values(self):
+        """The logged values of one update (read back from the bucket tail: the one host synchronisation)."""
+        s = self._stats.tolist()
+        return {"Qloss": s[0], "learning_rate": self.optimizer.param_groups[0]['lr'], "predictQ": s[1]}
 
 
 class PerDQN_Learner(DQN_Learner):

@@ -4,10 +4,11 @@ from .outputs import (ModelOutput, RepresentationOutput, ActionOutput, Stochasti
 from .distributions import CategoricalDistribution, DiagGaussianDistribution, ActivatedDiagGaussianDistribution
 from .representations import Basic_Identical, Basic_MLP, Basic_CNN, AC_CNN_Atari, REGISTRY_Representation
 from .heads import (CategoricalActorHead, GaussianActorHead, SAC_GaussianActorHead, ValueHead, QValueHead, DuelingQValueHead,
-                    DeterministicActorHead)
+                    DeterministicActorHead, C51QValueHead, QuantileRegressionQValueHead)
 from .architectures import (ActorCritic, SharedActorCritic, DeepQNetwork, DuelingDeepQNetwork, GaussianActor, SAC_GaussianActor,
                             TwinActionValueCritic, SoftActorCritic, TwinDiscreteActionValueCritic, SoftActorCriticDiscrete,
-                            DeterministicActor, ActionValueCritic, DeterministicActorCritic, TwinDelayedActorCritic)
+                            DeterministicActor, ActionValueCritic, DeterministicActorCritic, TwinDelayedActorCritic,
+                            C51DeepQNetwork, QRDeepQNetwork)
 from .qmix import Basic_RNN, AgentFeatureEncoder, DiscreteActionValueCritic, QMIX_Mixer, VDN_mixer, MixingQNetwork
 REGISTRY_Representation["Basic_RNN"] = Basic_RNN
 from .mappo import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic

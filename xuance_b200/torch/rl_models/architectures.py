@@ -9,7 +9,7 @@ import torch.nn as nn
 
 from ...common.spaces import is_discrete
 from .heads import (DuelingQValueHead, QValueHead, SAC_GaussianActorHead, GaussianActorHead, ValueHead,
-                    DeterministicActorHead)
+                    DeterministicActorHead, C51QValueHead, QuantileRegressionQValueHead)
 from .outputs import ModelOutput, StochasticActorOutput, TwinCriticOutput, DeterministicActorOutput, CriticOutput
 
 
@@ -112,6 +112,132 @@ class DeepQNetwork(nn.Module):
 class DuelingDeepQNetwork(DeepQNetwork):
     """deep_q_network.py:102-103."""
     q_head_cls = DuelingQValueHead
+
+
+DIST_MAX_ATOMS, DIST_MAX_ACTIONS = 64, 256     # include/xb200.h K6Z: 2 <= N <= 64 atoms / quantiles, 1 <= A <= 256
+
+
+class _DistributionalQNetwork(nn.Module):
+    """The shared body of C51DeepQNetwork / QRDeepQNetwork: eval representation + distributional head and their
+    deep-copied targets.  Greedy actions (and C51's probabilities under no_grad) come from one K6Z ``xb_dist_greedy``
+    launch over the head's raw [B, A, N] output; only a forward under autograd builds the reference's softmax in torch,
+    for the gradient."""
+
+    head_cls = None
+    uses_supports = False
+
+    def __init__(self, representation, hidden_size, action_space, n_atoms, normalizer=None, initializer=None,
+                 activation=None, device=None, use_distributed_training=False):
+        super().__init__()
+        if not is_discrete(action_space):
+            raise ValueError('action_space must be Discrete')
+        self.n_actions = action_space.n
+        if not 2 <= n_atoms <= DIST_MAX_ATOMS:
+            raise NotImplementedError("%s supports 2 to %d atoms / quantiles, got %d"
+                                      % (type(self).__name__, DIST_MAX_ATOMS, n_atoms))
+        if self.n_actions > DIST_MAX_ACTIONS:
+            raise NotImplementedError("%s supports at most %d actions, got %d"
+                                      % (type(self).__name__, DIST_MAX_ACTIONS, self.n_actions))
+        self.device = device
+        self.representation = representation
+        self.target_representation = deepcopy(representation)
+        self.representation_info_shape = representation.output_shapes
+        self.eval_Z_head = self.head_cls(feature_dim=self.representation_info_shape['state'][0],
+                                         hidden_size=hidden_size, n_actions=self.n_actions, atom_num=n_atoms,
+                                         normalizer=normalizer, initializer=initializer, activation=activation,
+                                         device=device)
+        self.target_Z_head = deepcopy(self.eval_Z_head)
+        self.distributed_training = use_distributed_training
+
+    def eval_parameters(self):
+        return list(self.representation.parameters()) + list(self.eval_Z_head.parameters())
+
+    def target_parameters(self):
+        return list(self.target_representation.parameters()) + list(self.target_Z_head.parameters())
+
+    def forward_raw(self, observation):
+        """The eval head's raw [B, A, N] output (C51 logits / QR quantiles), under autograd: the learner's input."""
+        return self.eval_Z_head.logits(self.representation(observation).embeddings)
+
+    @torch.no_grad()
+    def target_raw(self, observation):
+        return self.target_Z_head.logits(self.target_representation(observation).embeddings)
+
+    def greedy(self, z, with_probs=False):
+        """One ``xb_dist_greedy`` launch over raw [B, A, N] -> (actions int64 [B], C51 probabilities or None)."""
+        from ... import _lib
+        z = z.detach().to(torch.float32).contiguous()
+        B, A, N = z.shape
+        actions = torch.empty(B, dtype=torch.int64, device=z.device)
+        probs = torch.empty_like(z) if with_probs else None
+        sup = self.supports if self.uses_supports else None
+        _lib.call("xb_dist_greedy", _lib.ptr(z), _lib.ptr(sup), B, A, N, _lib.ptr(actions), None, _lib.ptr(probs))
+        return actions, probs
+
+    def _output(self, z, rep=None):
+        if torch.is_grad_enabled() and z.requires_grad:
+            actions, _ = self.greedy(z)
+            values = torch.softmax(z, dim=-1) if self.uses_supports else z
+        else:
+            actions, probs = self.greedy(z, with_probs=self.uses_supports)
+            values = probs if self.uses_supports else z
+        return ModelOutput(actions=actions, values=values, rep_out=rep)
+
+    def forward(self, observation, **kwargs):
+        rep = self.representation(observation)
+        return self._output(self.eval_Z_head.logits(rep.embeddings), rep)
+
+    @torch.no_grad()
+    def greedy_actions(self, observation):
+        """The eval network's greedy actions alone: one xb_dist_greedy launch that writes no probabilities (acting)."""
+        return self.greedy(self.eval_Z_head.logits(self.representation(observation).embeddings))[0]
+
+    def act(self, observation, deterministic=True, epsilon_greedy=0.0, **kwargs):
+        greedy = self.greedy_actions(observation)
+        if deterministic or epsilon_greedy <= 0.0:
+            return greedy
+        rand = torch.randint(low=0, high=self.n_actions, size=greedy.shape, device=greedy.device)
+        mask = torch.rand(greedy.shape, device=greedy.device) < epsilon_greedy
+        return torch.where(mask, rand, greedy)
+
+    def target(self, observation, **kwargs):
+        rep = self.target_representation(observation)
+        out = self._output(self.target_Z_head.logits(rep.embeddings))
+        return ModelOutput(actions=out.actions, values=out.values)
+
+    def copy_target(self):
+        for ep, tp in zip(self.representation.parameters(), self.target_representation.parameters()):
+            tp.data.copy_(ep)
+        for ep, tp in zip(self.eval_Z_head.parameters(), self.target_Z_head.parameters()):
+            tp.data.copy_(ep)
+
+
+class C51DeepQNetwork(_DistributionalQNetwork):
+    """deep_q_network.py:146-238.  ``supports`` is a registered, frozen Parameter filled by torch.linspace on the CPU (the
+    values a CPU-built reference model holds and saves in its state_dict; DESIGN section 4)."""
+
+    head_cls = C51QValueHead
+    uses_supports = True
+
+    def __init__(self, representation, hidden_size, action_space, atom_num, v_min, v_max, normalizer=None,
+                 initializer=None, activation=None, device=None, use_distributed_training=False, **kwargs):
+        super().__init__(representation, hidden_size, action_space, atom_num, normalizer, initializer, activation,
+                         device, use_distributed_training)
+        self.atom_num, self.v_min, self.v_max = atom_num, v_min, v_max
+        self.supports = nn.Parameter(torch.linspace(v_min, v_max, atom_num).to(device), requires_grad=False)
+        self.delta_z = (v_max - v_min) / (atom_num - 1)
+
+
+class QRDeepQNetwork(_DistributionalQNetwork):
+    """deep_q_network.py:241-325."""
+
+    head_cls = QuantileRegressionQValueHead
+
+    def __init__(self, representation, hidden_size, action_space, quantile_num, normalizer=None, initializer=None,
+                 activation=None, device=None, use_distributed_training=False, **kwargs):
+        super().__init__(representation, hidden_size, action_space, quantile_num, normalizer, initializer, activation,
+                         device, use_distributed_training)
+        self.quantile_num = quantile_num
 
 
 class GaussianActor(nn.Module):

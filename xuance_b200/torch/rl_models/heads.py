@@ -142,3 +142,33 @@ class DuelingQValueHead(nn.Module):
         if avail_actions is not None:
             q_values[avail_actions == 0] = -1e10
         return q_values
+
+
+class C51QValueHead(nn.Module):
+    """q_head.py:83-114: hidden layers, then Linear(n_actions * atom_num).  ``logits`` is the raw [B, A, N] view the
+    K6Z kernels consume; ``forward`` is the reference's softmax over atoms (autograd path)."""
+
+    def __init__(self, feature_dim, hidden_size, n_actions, atom_num, normalizer=None, initializer=None,
+                 activation=None, device=None, **kwargs):
+        super().__init__()
+        self.feature_dim, self.n_actions, self.atom_num = feature_dim, n_actions, atom_num
+        layers, shape = _stack(feature_dim, hidden_size, normalizer, activation, initializer, device)
+        layers.extend(mlp_block(shape[0], n_actions * atom_num, None, None, initializer, device)[0])
+        self.model = nn.Sequential(*layers)
+
+    def logits(self, features):
+        return self.model(features).view(-1, self.n_actions, self.atom_num)
+
+    def forward(self, features, avail_actions=None, **kwargs):
+        if avail_actions is not None:
+            raise NotImplementedError("action masks are not supported by the distributional Q heads")
+        return torch.softmax(self.logits(features), dim=-1)
+
+
+class QuantileRegressionQValueHead(C51QValueHead):
+    """q_head.py:117-123: the same layers; the output is the [B, A, N] quantiles themselves."""
+
+    def forward(self, features, avail_actions=None, **kwargs):
+        if avail_actions is not None:
+            raise NotImplementedError("action masks are not supported by the distributional Q heads")
+        return self.logits(features)
