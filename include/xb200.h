@@ -50,6 +50,12 @@ int xb_device_info(int *sm_count, int *cc_major, int *cc_minor);
 int xb_rollout_store(void *rows_dst, const void *rows_src, int64_t row_bytes,
                      float *scal_dst, const float *scal_src, int F,
                      int N, int T, int t, void *stream);
+/* xb_rollout_store with a per-row step: row n goes to step step[n] (device int32[N]); rows whose step is outside
+ * [0, T) are not written.  The per-env episode staging of MARL_OnPolicyBuffer_RNN, where each env sits at its own
+ * episode step (memory_tools_marl.py:461-470). */
+int xb_rollout_store_at(void *rows_dst, const void *rows_src, int64_t row_bytes,
+                        float *scal_dst, const float *scal_src, int F,
+                        int N, int T, const int32_t *step, void *stream);
 
 /* ---------------------------------------------------------------- K2: GAE / returns scan -------------
  * Replaces DummyOnPolicyBuffer.finish_path (memory_tools.py:242-265) for ALL envs and ALL path segments of a
@@ -336,6 +342,24 @@ int xb_ddpg_critic_loss(const float *q1, const float *q2, const float *tq1, cons
                         float *backup, float *stats, double *scratch, void *stream);
 int xb_ddpg_actor_loss(const float *q1, const float *q2, int64_t B, int64_t B_total, float *dq1, float *dq2,
                        float *stats, double *scratch, void *stream);
+
+/* ---------------------------------------------------------------- K13: GRU sequence kernels ----------
+ * The recurrence of a one-layer torch.nn.GRU (gate order r, z, n) over S independent sequences of T steps, as the
+ * recurrent representations of MAPPO run it (Basic_RNN, rl_models/representations/rnn.py:9-99).  xg[S, T, 3H] is the
+ * projected input x W_ih^T + b_ih (a cuBLAS GEMM the caller runs for all T at once); w_hh[3H, H], b_hh[3H] are torch's
+ * weight_hh_l0 / bias_hh_l0; h0[S, H] is nullable (zeros).  Per step, gh = W_hh h + b_hh and
+ *     r = sigmoid(xg_r + gh_r), z = sigmoid(xg_z + gh_z), n = tanh(xg_n + r * gh_n), h' = (1 - z) * n + z * h.
+ * fwd: writes y[S, T, H] (every h'), hT[S, H] and, when gates != NULL (training), gates[S, T, 4H] = {r, z, n, gh_n}.
+ * bwd: from dy[S, T, H] and a nullable dhT[S, H], with the forward's gates, y and h0, writes dxg[S, T, 3H] (the gradient
+ *      of xg: dW_ih, db_ih and dx follow by GEMMs / sums), dgh[S, T, 3H] (the gradient of W_hh h + b_hh: dW_hh =
+ *      sum dgh^T h_{t-1}, db_hh = sum dgh) and, when dh0 != NULL, dh0[S, H].
+ * float32 on the CUDA cores with accurate expf / tanhf; one CTA walks all T steps of 4 sequences with W_hh resident in
+ * shared memory.  No atomics: every sequence's result is bit-identical from launch to launch and whichever CTA owns it.
+ * 1 <= H <= 64, T >= 1, S >= 1, and NULL required pointers, are XB_EINVAL. */
+int xb_gru_seq_fwd(const float *xg, const float *w_hh, const float *b_hh, const float *h0, int64_t S, int T, int H,
+                   float *y, float *hT, float *gates, void *stream);
+int xb_gru_seq_bwd(const float *dy, const float *dhT, const float *w_hh, const float *gates, const float *y,
+                   const float *h0, int64_t S, int T, int H, float *dxg, float *dgh, float *dh0, void *stream);
 
 /* ---------------------------------------------------------------- K7: flat-bucket optimiser step -----
  * Replaces clip_grad_norm_ + torch.optim.Adam.step on the learner's parameters (ppo_learner.py:61-65;

@@ -3,7 +3,8 @@
 DQN+PER (2^20-transition HBM replay, B=512), SAC (1M replay, B=1024) and QMIX (5 agents x 72-d, T=60, 32 episodes)
 on one GPU, next to the oracle port of the reference's torch-CPU path on the host; and ``ppo_gauss``, continuous-control
 PPO in the shape of the reference's ppo/mujoco.yaml (train_epochs env-steps/s); ``mappo``, MAPPO in the shape of
-configs/mappo/sc2/5m_vs_6m.yaml (train_epochs env-steps/s); ``sacdis``, SAC-Discrete in the shape of
+configs/mappo/sc2/5m_vs_6m.yaml (train_epochs env-steps/s); ``mappo_rnn``, recurrent MAPPO in the shape of
+configs/mappo/sc2/3m.yaml (update, eager and graphed); ``sacdis``, SAC-Discrete in the shape of
 configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (train_epochs, eager and graphed); ``ddpg`` and
 ``td3``, DDPG / TD3 in the shape of the reference's ddpg/mujoco.yaml and td3/mujoco.yaml (sample + update, eager and
 graphed); ``c51`` and ``qrdqn`` on CartPole (Basic_MLP 128, B=256) and SyntheticAtari (Basic_CNN, B=32) shapes (update,
@@ -290,6 +291,59 @@ def bench_mappo(args):
     return out
 
 
+def bench_mappo_rnn(args):
+    """Recurrent MAPPO in the shape of configs/mappo/sc2/3m.yaml: one MAPPO_Learner.update over its minibatch of 128
+    episodes x 3 agents x T = 60 (384 GRU sequences, 23040 rows; fc [64, 64, 64], GRU 64, LayerNorm, 9 masked actions),
+    eager and as a CUDA graph, next to the torch-CPU oracle's update (nn.GRU on the host) on the same model."""
+    import copy
+    from xuance_b200.common import Box, Discrete
+    from xuance_b200.common.common_tools import get_arguments
+    from xuance_b200.torch.agents import MAPPO_Agents
+    from oracle_mappo import MAPPOLearnerOracle
+    from oracle_mappo_rnn import RecurrentModelOracle
+    B, n, T, od, A = 128, 3, 60, 30, 9
+    keys = ["agent_%d" % i for i in range(n)]
+    rng = np.random.default_rng(0)
+    S = B * n
+    avail = np.zeros((S, T, 12), np.uint8)
+    avail[..., :A] = rng.random((S, T, A)) > 0.3
+    avail[..., 0] = 1
+    lengths = np.tile(rng.integers(20, T + 1, B), n)
+    st = dict(obs=rng.uniform(-1, 1, (S, T, od)).astype(np.float32), actions=np.zeros((S, T), np.float32),
+              log_pi_old=np.full((S, T), -2.2, np.float32), advantages=rng.normal(size=(S, T)).astype(np.float32),
+              values=rng.normal(size=(S, T)).astype(np.float32), returns=rng.normal(size=(S, T)).astype(np.float32),
+              agent_mask=(rng.random((S, T)) > 0.05).astype(np.float32),
+              filled=(np.arange(T)[None] < lengths[:, None]).astype(np.float32), avail_actions=avail)
+    sample = {'_stacked': {k: torch.from_numpy(v).to(DEV) for k, v in st.items()}, 'batch_size': B,
+              'sequence_length': T}
+    out = {"config": "recurrent MAPPO 3m shape: 128 episodes x 3 agents x T = 60 per update, Basic_RNN (fc 64-64-64, "
+                     "GRU 64, LayerNorm) actor and critic, 9 masked actions, value clip + ValueNorm + Huber"}
+    model = None
+    for graph in (False, True):
+        cfg = get_arguments("mappo", "sc2", "3m")
+        for k, v in dict(device=DEV, parallels=8, logger=None, model_dir="/tmp/x", use_cuda_graph=graph,
+                         distributed_training=False, episode_length=T).items():
+            setattr(cfg, k, v)
+        torch.manual_seed(0)
+        agent = MAPPO_Agents(cfg, None, n, keys, None, {k: Box(-1, 1, (od,), np.float32) for k in keys},
+                             {k: Discrete(A) for k in keys})
+        if model is None:
+            model = copy.deepcopy(agent.model)
+        dt = timed(lambda: agent.learner.update(sample, sync=False), max(5, args.iters // 10), warm=3)
+        out["gpu_ms_per_update_" + ("graph" if graph else "eager")] = dt * 1e3
+    if not args.no_cpu:
+        ol = MAPPOLearnerOracle(RecurrentModelOracle(model), cfg)
+        t = {k: torch.from_numpy(v) for k, v in st.items()}
+        fl = lambda k: t[k].reshape(-1)
+        b = (t['obs'], fl('actions'), fl('log_pi_old'), fl('advantages'), fl('values'), fl('returns'),
+             fl('agent_mask') * fl('filled'), t['avail_actions'][..., :A].reshape(-1, A) != 0)
+        cdt = cpu_timed(lambda: ol.update(*b), max(args.cpu_iters, 3))
+        out.update(cpu_ms_per_update=cdt * 1e3, cpu_threads=torch.get_num_threads(),
+                   speedup_eager=cdt * 1e3 / out["gpu_ms_per_update_eager"],
+                   speedup_graph=cdt * 1e3 / out["gpu_ms_per_update_graph"])
+    return out
+
+
 def bench_sacdis(args):
     """SAC-Discrete: ``train_epochs(1)`` (one replay sample of 256 rows + one SACDIS_Learner.update) of a SAC_Agent built
     from configs/sac/CartPole-v1.yaml (4-d obs, A = 2, Basic_MLP 128, heads [128], alpha fixed), and the same at A = 18 with
@@ -488,6 +542,8 @@ def main():
         res["ppo_gauss"] = bench_ppo_gauss(args)
     if (not only and WORLD == 1) or "mappo" in only:
         res["mappo"] = bench_mappo(args)
+    if (not only and WORLD == 1) or "mappo_rnn" in only:
+        res["mappo_rnn"] = bench_mappo_rnn(args)
     if (not only and WORLD == 1) or "sacdis" in only:
         res["sacdis"] = bench_sacdis(args)
     for algo in ("ddpg", "td3"):

@@ -4,7 +4,7 @@ shapes (SURVEY.md section 7 "hard parts": at the named PPO shape K2/K4/K5 move <
 bandwidth fraction is also reported at a scaled shape).  CUDA events on the launching stream, >= 3 warm-ups, L2
 flushed between timed launches (256 MB memset).  Prints one JSON object.
 
-    python tools/kernel_bench.py [--only k2,k4] [--reps 20]      (k12 / k12box / k3p: the tensor-core encoder layers, gathered and TMA-box / halo variants)
+    python tools/kernel_bench.py [--only k2,k4] [--reps 20]      (k12 / k12box / k3p: the tensor-core encoder layers, gathered and TMA-box / halo variants; k13: the GRU sequence kernels against cuDNN)
 """
 import argparse
 import json
@@ -370,7 +370,71 @@ def main():
             us = timeit(lambda: tc.wgrad_box(xp_, g3, P[bgk], 6, sp), R)
             add(entry("K12-box weight gradient %s (P=3, %d splits)" % (nm, sp), f"M={B * 100} N=64 K={K}", us,
                       xp_.numel() * 2 + g3.numel() * 2, hbm, 2.0 * B * 100 * 64 * K, tpk))
+    if want("k13"):
+        out["k13"] = k13_bench(R, hbm)
     print(json.dumps(out))
+
+
+def k13_bench(R, hbm):
+    """K13 at recurrent MAPPO's SMAC shape (S = 640 sequences of T = 60 steps, H = 64, GRU input 64): each kernel alone,
+    then a whole GRU forward + backward (input projection and weight-gradient GEMMs included) through gru_sequence
+    against nn.GRU on cuDNN, both in IEEE fp32, with the number of kernels each launches (torch.profiler, separate run)."""
+    saved = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        return _k13_bench(R)
+    finally:        # IEEE fp32 for this comparison only
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = saved
+
+
+def _k13_bench(R):
+    import subprocess
+    import torch.nn as nn
+    from xuance_b200.torch.rl_models import gru_sequence
+    S, T, H, I = 640, 60, 64, 64
+    res = {"shape": f"S={S} T={T} H={H} I={I}"}
+    try:
+        res["gpu"] = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm",
+                                     "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    except OSError:
+        res["gpu"] = "nvidia-smi unavailable"
+    torch.manual_seed(0)
+    gru = nn.GRU(I, H, batch_first=True, device=DEV)
+    x = torch.randn(S, T, I, device=DEV, requires_grad=True)
+    dy = torch.randn(S, T, H, device=DEV)
+    xg = torch.randn(S, T, 3 * H, device=DEV)
+    w, b = gru.weight_hh_l0.detach().contiguous(), gru.bias_hh_l0.detach().contiguous()
+    y, hT = torch.empty(S, T, H, device=DEV), torch.empty(S, H, device=DEV)
+    gates = torch.empty(S, T, 4 * H, device=DEV)
+    dxg, dgh = torch.empty(S, T, 3 * H, device=DEV), torch.empty(S, T, 3 * H, device=DEV)
+    fwd = lambda: _lib.call("xb_gru_seq_fwd", _lib.ptr(xg), _lib.ptr(w), _lib.ptr(b), None, S, T, H, _lib.ptr(y),
+                            _lib.ptr(hT), _lib.ptr(gates))
+    bwd = lambda: _lib.call("xb_gru_seq_bwd", _lib.ptr(dy), None, _lib.ptr(w), _lib.ptr(gates), _lib.ptr(y), None, S, T,
+                            H, _lib.ptr(dxg), _lib.ptr(dgh), None)
+    fl = 2.0 * S * T * 3 * H * H
+    res["k13_fwd_us"] = round(timeit(fwd, R), 2)
+    res["k13_bwd_us"] = round(timeit(bwd, R), 2)
+    res["k13_fwd_TFLOPs_fp32"] = round(fl / res["k13_fwd_us"] / 1e6, 3)
+
+    def step(use_k13):
+        x.grad = None
+        gru.zero_grad(set_to_none=True)
+        yy = gru_sequence(gru, x)[0] if use_k13 else gru(x)[0]
+        yy.backward(dy)
+
+    for name, k in (("gru_sequence_k13", True), ("nn_gru_cudnn", False)):
+        res[name + "_fwd_bwd_us"] = round(timeit(lambda: step(k), R), 2)
+        from torch.profiler import profile, ProfilerActivity
+        torch.cuda.synchronize()
+        try:
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                step(k)
+                torch.cuda.synchronize()
+            res[name + "_kernels"] = sum(e.count for e in prof.key_averages() if str(e.device_type).endswith("CUDA")
+                                         and not e.key.startswith(("Memcpy", "Memset")))
+        except Exception as exc:     # the timing above stands without the count
+            res[name + "_kernels"] = "profiler failed: %s" % exc
+    return res
 
 
 if __name__ == "__main__":

@@ -22,6 +22,7 @@ _SIGNATURES = {
     "xb_error_string": (c_char_p, [c_int]),
     "xb_device_info": (c_int, [POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     "xb_rollout_store": (c_int, [_P, _P, c_int64, _P, _P, c_int, c_int, c_int, c_int, _P]),
+    "xb_rollout_store_at": (c_int, [_P, _P, c_int64, _P, _P, c_int, c_int, c_int, _P, _P]),
     "xb_gae_scan": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_float, c_float, c_int, _P]),
     "xb_gae_scan_vn": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_double, c_double, c_int, _P, _P,
                                 _P, _P]),
@@ -82,6 +83,8 @@ _SIGNATURES = {
     "xb_perturb_actions": (c_int, [_P, _P, c_int64, c_int, c_float, c_float, _P, _P, _P, _P]),
     "xb_ddpg_critic_loss": (c_int, [_P, _P, _P, _P, _P, _P, c_float, c_int64, c_int64, _P, _P, _P, _P, _P, _P]),
     "xb_ddpg_actor_loss": (c_int, [_P, _P, c_int64, c_int64, _P, _P, _P, _P, _P]),
+    "xb_gru_seq_fwd": (c_int, [_P, _P, _P, _P, c_int64, c_int, c_int, _P, _P, _P, _P]),
+    "xb_gru_seq_bwd": (c_int, [_P, _P, _P, _P, _P, _P, c_int64, c_int, c_int, _P, _P, _P, _P]),
     "xb_qmix_select_fwd": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     "xb_qmix_select_bwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
     "xb_qmix_mix_fwd": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int, c_int, _P, _P]),

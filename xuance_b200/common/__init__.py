@@ -3,4 +3,4 @@ from .memory_tools import (Buffer, DummyOnPolicyBuffer, DummyOnPolicyBuffer_Atar
                            DummyOffPolicyBuffer_Atari, PerOffPolicyBuffer, PreparedObs)
 from .callback import BaseCallback
 from .agent_grouping import AgentGrouping
-from .memory_tools_marl import MARL_OffPolicyBuffer_RNN, MARL_OnPolicyBuffer
+from .memory_tools_marl import MARL_OffPolicyBuffer_RNN, MARL_OnPolicyBuffer, MARL_OnPolicyBuffer_RNN

@@ -379,3 +379,220 @@ class MARL_OnPolicyBuffer:
         self._seg_end[:] = sd["seg_end"]
         self._boot[:] = sd["boot"]
         self.ptr, self.size, self.start_ids = int(sd["ptr"]), int(sd["size"]), np.array(sd["start_ids"])
+
+
+class MARL_OnPolicyBuffer_RNN:
+    """Episode-major on-policy rollout for recurrent MAPPO - mirror of MARL_OnPolicyBuffer_RNN
+    (xuance/common/memory_tools_marl.py:273-515): same constructor arguments, keys, ``ptr / size / full``, ``clear /
+    clear_episodes / store / store_episodes / finish_path / sample``.  ``buffer_size`` counts episodes.
+
+    Everything lives in HBM.  The per-env staging rows are (env, agent) pairs over ``T_max = max_episode_steps``; each
+    vector step is one ``xb_rollout_store_at`` launch per array, at each env's own episode step.  ``finish_path`` runs
+    ``xb_gae_scan_vn`` over env i's rows on ``[0, min(i_step, T_max))`` with the ValueNorm state of that moment, then
+    copies the rows into ring slot ``ptr`` and clears only that env's ``filled``: as in the reference, the staging is
+    never zeroed between episodes, so the padded tail of an env's second episode still holds its first episode's data.
+    ``sample`` gathers whole episodes with K3 into sequence-major ``[B*n, T, .]`` (sequence k*B + b is agent k of
+    episode b) and does not normalise advantages (the reference's recurrent ``sample`` does not either)."""
+    FIELDS = MARL_OnPolicyBuffer.FIELDS
+    STORED = MARL_OnPolicyBuffer.STORED
+
+    def __init__(self, agent_keys, state_space=None, obs_space=None, act_space=None, n_envs=1, buffer_size=1,
+                 max_episode_steps=1, use_gae=False, use_advnorm=False, gamma=None, gae_lam=None, device="cuda:0",
+                 **kwargs):
+        self.agent_keys = list(agent_keys)
+        self.n_agents = len(self.agent_keys)
+        self.n_envs, self.buffer_size, self.max_eps_len = n_envs, buffer_size, max_episode_steps
+        self.state_space = state_space
+        self.store_global_state = state_space is not None
+        self.use_actions_mask = kwargs.get("use_actions_mask", False)
+        self.avail_actions_shape = kwargs.get("avail_actions_shape", None)
+        self.use_gae, self.use_advantage_norm = use_gae, use_advnorm
+        self.gamma, self.gae_lambda = gamma, gae_lam
+        k0 = self.agent_keys[0]
+        obs_shape = {k: tuple(space2shape(obs_space[k])) for k in self.agent_keys}
+        act_shape = {k: tuple(space2shape(act_space[k])) for k in self.agent_keys}
+        if any(obs_shape[k] != obs_shape[k0] or act_shape[k] != act_shape[k0] for k in self.agent_keys):
+            raise NotImplementedError("heterogeneous agents are outside the hot-path scope (one parameter-sharing group)")
+        if act_shape[k0] != ():
+            raise NotImplementedError("MARL_OnPolicyBuffer_RNN: Box action spaces (Gaussian MAPPO) are not supported")
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise RuntimeError("xuance_b200 buffers are device-resident: device must be CUDA (no CPU fallback)")
+        _lib.load()
+        _lib.use_device(self.device)
+        self._obs_dim = int(np.prod(obs_shape[k0]))
+        self._state_dim = int(np.prod(space2shape(state_space))) if self.store_global_state else 0
+        self._n_act = int(self.avail_actions_shape[k0][0]) if self.use_actions_mask else 0
+        self._a4 = _pad4(self._n_act)
+        self._rows = self.n_envs * self.n_agents
+        self._seg_end = np.zeros((self._rows, self.max_eps_len), np.uint8)
+        self._boot = np.zeros((self._rows, self.max_eps_len), np.float32)
+        self.clear()
+        self.clear_episodes()
+
+    @property
+    def data_keys(self):
+        keys = ['obs'] + list(self.FIELDS) + ['filled']
+        if self.store_global_state:
+            keys.append('state')
+        if self.use_actions_mask:
+            keys.append('avail_actions')
+        return keys
+
+    @property
+    def full(self):
+        return self.size >= self.buffer_size
+
+    def clear(self):
+        """The episode ring: scalars [buffer_size * n, F, T] (row = slot * n + agent), obs [buffer_size * n, T, obs],
+        filled [buffer_size, T]."""
+        S, T, dev = self.buffer_size * self.n_agents, self.max_eps_len, self.device
+        self._scal = torch.zeros((S, len(self.FIELDS), T), dtype=torch.float32, device=dev)
+        self._obs = torch.zeros((S, T, self._obs_dim), dtype=torch.float32, device=dev)
+        self._avail = torch.zeros((S, T, self._a4), dtype=torch.uint8, device=dev) if self.use_actions_mask else None
+        self._state = (torch.zeros((self.buffer_size, T, self._state_dim), dtype=torch.float32, device=dev)
+                       if self.store_global_state else None)
+        self._filled = torch.zeros((self.buffer_size, T), dtype=torch.float32, device=dev)
+        self.ptr, self.size = 0, 0
+
+    def clear_episodes(self):
+        """The per-env staging: scalars [F, n_envs * n, T] (K1's layout), obs [n_envs * n, T, obs], filled [n_envs, T]."""
+        R, T, dev = self._rows, self.max_eps_len, self.device
+        self._ep_scal = torch.zeros((len(self.FIELDS), R, T), dtype=torch.float32, device=dev)
+        self._ep_obs = torch.zeros((R, T, self._obs_dim), dtype=torch.float32, device=dev)
+        self._ep_avail = torch.zeros((R, T, self._a4), dtype=torch.uint8, device=dev) if self.use_actions_mask else None
+        self._ep_state = (torch.zeros((self.n_envs, T, self._state_dim), dtype=torch.float32, device=dev)
+                          if self.store_global_state else None)
+        self._ep_filled = torch.zeros((1, self.n_envs, T), dtype=torch.float32, device=dev)
+        self._ones = torch.ones((1, self.n_envs), dtype=torch.float32, device=dev)
+
+    def field(self, name):
+        """[n_envs * n_agents, T] device view of a staging scalar field (row = env * n_agents + agent)."""
+        return self._ep_scal[self.FIELDS.index(name)]
+
+    def _per_agent(self, d, dtype=np.float32):
+        return np.stack([np.asarray(d[k], dtype=dtype) for k in self.agent_keys], axis=1).reshape(self._rows, -1)
+
+    # ---- reference :397-414
+    def store(self, **step_data):
+        T, R = self.max_eps_len, self._rows
+        steps = np.asarray(step_data['episode_steps'], np.int32).reshape(self.n_envs)
+        steps_env = torch.from_numpy(steps).to(self.device)
+        steps_row = torch.from_numpy(np.repeat(steps, self.n_agents)).to(self.device)
+        scal = np.concatenate([self._per_agent(step_data[k]).reshape(1, R) for k in self.FIELDS[:self.STORED]])
+        scal_d = torch.from_numpy(np.ascontiguousarray(scal)).to(self.device)
+        obs_d = torch.from_numpy(np.ascontiguousarray(self._per_agent(step_data['obs']))).to(self.device)
+        _lib.call("xb_rollout_store_at", _lib.ptr(self._ep_obs), _lib.ptr(obs_d), self._obs_dim * 4,
+                  _lib.ptr(self._ep_scal), _lib.ptr(scal_d), self.STORED, R, T, _lib.ptr(steps_row))
+        if self.use_actions_mask:
+            av = np.zeros((R, self._a4), np.uint8)
+            av[:, :self._n_act] = self._per_agent(step_data['avail_actions'], np.float32) != 0
+            av_d = torch.from_numpy(av).to(self.device)
+            _lib.call("xb_rollout_store_at", _lib.ptr(self._ep_avail), _lib.ptr(av_d), self._a4, None, None, 0, R, T,
+                      _lib.ptr(steps_row))
+        st_d = None
+        if self.store_global_state:
+            st_d = torch.from_numpy(np.ascontiguousarray(step_data['state'], dtype=np.float32)).to(self.device)
+        # filled[env, step] = 1, in the same launch as the global state rows
+        _lib.call("xb_rollout_store_at", _lib.ptr(self._ep_state), _lib.ptr(st_d), self._state_dim * 4,
+                  _lib.ptr(self._ep_filled), _lib.ptr(self._ones), 1, self.n_envs, T, _lib.ptr(steps_env))
+
+    # ---- reference :416-435: env i's staging rows -> ring slot ptr (device copies), then clear only its `filled`
+    def store_episodes(self, i_env):
+        n, p = self.n_agents, self.ptr
+        rows = slice(i_env * n, (i_env + 1) * n)
+        self._scal[p * n:(p + 1) * n].copy_(self._ep_scal[:, rows].transpose(0, 1))
+        self._obs[p * n:(p + 1) * n].copy_(self._ep_obs[rows])
+        if self.use_actions_mask:
+            self._avail[p * n:(p + 1) * n].copy_(self._ep_avail[rows])
+        if self.store_global_state:
+            self._state[p].copy_(self._ep_state[i_env])
+        self._filled[p].copy_(self._ep_filled[0, i_env])
+        self.ptr = (self.ptr + 1) % self.buffer_size
+        self.size = min(self.size + 1, self.buffer_size)
+        self._ep_filled[0, i_env].zero_()
+
+    # ---- reference :437-490
+    def finish_path(self, i_env=None, i_step=None, agent_grouping=None, value_next=None, value_normalizer=None,
+                    **kwargs):
+        n, T = self.n_agents, self.max_eps_len
+        env_step = min(int(i_step), T)
+        if env_step > 0:
+            rows = slice(i_env * n, (i_env + 1) * n)
+            self._seg_end[rows] = 0
+            self._seg_end[rows, env_step - 1] = 1
+            self._boot[rows] = 0
+            self._boot[rows, env_step - 1] = [np.float32(value_next[k]) for k in self.agent_keys]
+            seg_d = torch.from_numpy(self._seg_end[rows]).to(self.device)
+            boot_d = torch.from_numpy(self._boot[rows]).to(self.device)
+            cov_d = torch.full((n,), env_step, dtype=torch.int32, device=self.device)
+            vn = None
+            if value_normalizer is not None:
+                groups = {agent_grouping.agent_to_group[k] for k in self.agent_keys} if agent_grouping is not None \
+                    else set(value_normalizer)
+                if len(groups) != 1:
+                    raise NotImplementedError("one parameter-sharing group")
+                vn = value_normalizer[groups.pop()]
+            vp = vn.state_pointers() if vn is not None else (None, None, None)
+            f = lambda name: _lib.ptr(self.field(name)[rows])
+            _lib.call("xb_gae_scan_vn", f('rewards'), f('values'), f('terminals'), _lib.ptr(seg_d), _lib.ptr(boot_d),
+                      None, _lib.ptr(cov_d), f('advantages'), f('returns'), n, T, float(self.gamma),
+                      float(self.gae_lambda if self.gae_lambda is not None else 0.0), 1 if self.use_gae else 0, *vp)
+        self.store_episodes(i_env)
+
+    def _gather_rows(self, src, idx_t, row_bytes, shape, dtype):
+        out = torch.empty(shape, dtype=dtype, device=self.device)
+        _lib.call("xb_gather_rows", _lib.ptr(src), _lib.ptr(idx_t), idx_t.numel(), row_bytes, _lib.ptr(out))
+        return out
+
+    # ---- reference :492-515
+    def sample(self, indexes=None):
+        assert self.full, "Not enough transitions for on-policy buffer to random sample"
+        idx = np.asarray(indexes, dtype=np.int64).reshape(-1)
+        B, n, T, F = idx.size, self.n_agents, self.max_eps_len, len(self.FIELDS)
+        seq = (idx[None, :] * n + np.arange(n)[:, None]).reshape(-1)                # agent-major: k * B + b
+        seq_t = torch.from_numpy(seq).to(self.device)
+        ep_t = torch.from_numpy(np.tile(idx, n)).to(self.device)
+        scal = self._gather_rows(self._scal, seq_t, F * T * 4, (n * B, F, T), torch.float32)
+        st = {name: scal[:, i].contiguous() for i, name in enumerate(self.FIELDS)}    # [n*B, T]
+        st['obs'] = self._gather_rows(self._obs, seq_t, T * self._obs_dim * 4, (n * B, T, self._obs_dim), torch.float32)
+        st['filled'] = self._gather_rows(self._filled, ep_t, T * 4, (n * B, T), torch.float32)
+        if self.use_actions_mask:
+            st['avail_actions'] = self._gather_rows(self._avail, seq_t, T * self._a4, (n * B, T, self._a4), torch.uint8)
+        if self.store_global_state:
+            st['state'] = self._gather_rows(self._state, ep_t, T * self._state_dim * 4, (n * B, T, self._state_dim),
+                                            torch.float32)
+        out = {}
+        for key, v in st.items():
+            if key in ('filled', 'state'):
+                out[key] = v[:B].bool() if key == 'filled' else v[:B]
+            elif key == 'avail_actions':
+                out[key] = {a: v[i * B:(i + 1) * B, :, :self._n_act].bool() for i, a in enumerate(self.agent_keys)}
+            elif key in ('terminals', 'agent_mask'):
+                out[key] = {a: v[i * B:(i + 1) * B].bool() for i, a in enumerate(self.agent_keys)}
+            else:
+                out[key] = {a: v[i * B:(i + 1) * B] for i, a in enumerate(self.agent_keys)}
+        out['batch_size'] = B
+        out['sequence_length'] = T
+        out['_stacked'] = st
+        return out
+
+    # ---- checkpoint (the reference does not save its rollout)
+    def state_dict(self):
+        t = lambda x: None if x is None else x.cpu()
+        return {"class": type(self).__name__, "buffer_size": self.buffer_size, "n_envs": self.n_envs,
+                "max_eps_len": self.max_eps_len, "ptr": int(self.ptr), "size": int(self.size),
+                "data": {k: t(getattr(self, k)) for k in ("_scal", "_obs", "_avail", "_state", "_filled")},
+                "episode_data": {k: t(getattr(self, k)) for k in ("_ep_scal", "_ep_obs", "_ep_avail", "_ep_state",
+                                                                  "_ep_filled")}}
+
+    def load_state_dict(self, sd):
+        if (sd.get("class"), sd.get("buffer_size"), sd.get("n_envs"), sd.get("max_eps_len")) != \
+                (type(self).__name__, self.buffer_size, self.n_envs, self.max_eps_len):
+            raise ValueError("recurrent on-policy MARL checkpoint does not match this buffer's size / envs / length")
+        for group in ("data", "episode_data"):
+            for k, v in sd[group].items():
+                dst = getattr(self, k)
+                if dst is not None:
+                    dst.copy_(v)
+        self.ptr, self.size = int(sd["ptr"]), int(sd["size"])

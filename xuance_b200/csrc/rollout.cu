@@ -57,6 +57,63 @@ extern "C" int xb_rollout_store(void *rows_dst, const void *rows_src, int64_t ro
     return xb_launch_status();
 }
 
+// xb_rollout_store_at: the same store with a per-row step index step[n] read on the device (rows whose step is outside
+// [0, T) are left alone).  A separate kernel so that xb_rollout_store's instructions stay as they are.
+__global__ void __launch_bounds__(256) store_rows_at_kernel(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src,
+                                                            int64_t row_bytes, int N, int T,
+                                                            const int32_t *__restrict__ step, bool vec16,
+                                                            float *__restrict__ sdst, const float *__restrict__ ssrc,
+                                                            int F, int row_blocks) {
+    if ((int)blockIdx.x >= row_blocks) {
+        int i = (blockIdx.x - row_blocks) * blockDim.x + threadIdx.x;
+        if (i < F * N) {
+            int f = i / N, n = i - f * N;
+            const int t = step[n];
+            if (t >= 0 && t < T) sdst[((int64_t)f * N + n) * T + t] = ssrc[i];
+        }
+        return;
+    }
+    const int64_t per_row = vec16 ? row_bytes / 16 : row_bytes / 4;
+    const int64_t total = per_row * N;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)row_blocks * blockDim.x) {
+        int64_t n = i / per_row, c = i - n * per_row;
+        const int t = step[n];
+        if (t < 0 || t >= T) continue;
+        if (vec16) {
+            uint4 v = ldg_stream16(src + n * row_bytes + c * 16);
+            stg_stream16(dst + (n * T + t) * row_bytes + c * 16, v);
+        } else {
+            uint32_t v = *reinterpret_cast<const uint32_t *>(src + n * row_bytes + c * 4);
+            *reinterpret_cast<uint32_t *>(dst + (n * T + t) * row_bytes + c * 4) = v;
+        }
+    }
+}
+
+extern "C" int xb_rollout_store_at(void *rows_dst, const void *rows_src, int64_t row_bytes, float *scal_dst,
+                                   const float *scal_src, int F, int N, int T, const int32_t *step, void *stream) {
+    if (N <= 0 || T <= 0 || F < 0 || !step) return XB_EINVAL;
+    if ((rows_dst == nullptr) != (rows_src == nullptr)) return XB_EINVAL;
+    if (F > 0 && (!scal_dst || !scal_src)) return XB_EINVAL;
+    int row_blocks = 0;
+    bool vec16 = false;
+    if (rows_dst) {
+        if (row_bytes <= 0 || (row_bytes & 3)) return XB_EALIGN;
+        vec16 = (row_bytes % 16 == 0) && xb_aligned(rows_dst, 16) && xb_aligned(rows_src, 16);
+        if (!vec16 && (!xb_aligned(rows_dst, 4) || !xb_aligned(rows_src, 4))) return XB_EALIGN;
+        int64_t items = (vec16 ? row_bytes / 16 : row_bytes / 4) * N;
+        int64_t want = (items + 255) / 256;
+        int64_t cap = (int64_t)xb_sm_count() * 8;
+        row_blocks = (int)(want < cap ? want : cap);
+        if (row_blocks < 1) row_blocks = 1;
+    }
+    int scal_blocks = F > 0 ? (F * N + 255) / 256 : 0;
+    if (row_blocks + scal_blocks == 0) return XB_OK;
+    store_rows_at_kernel<<<row_blocks + scal_blocks, 256, 0, (cudaStream_t)stream>>>(
+        (uint8_t *)rows_dst, (const uint8_t *)rows_src, row_bytes, N, T, step, vec16, scal_dst, scal_src, F,
+        row_blocks);
+    return xb_launch_status();
+}
+
 // =====================================================================================================
 // K2  xb_gae_scan : one warp per env, reverse inclusive scan of affine maps x -> a*x + b over the T steps.
 // =====================================================================================================

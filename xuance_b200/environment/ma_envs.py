@@ -15,7 +15,8 @@ import numpy as np
 
 from ..common.spaces import Box, Discrete
 
-SMAC_SHAPES = {"5m_vs_6m": dict(n_agents=5, obs_dim=72, state_dim=98, n_actions=12, episode_limit=60)}
+SMAC_SHAPES = {"5m_vs_6m": dict(n_agents=5, obs_dim=72, state_dim=98, n_actions=12, episode_limit=60),
+               "3m": dict(n_agents=3, obs_dim=30, state_dim=48, n_actions=9, episode_limit=60)}
 
 
 class SyntheticSMACEnv:

@@ -5,7 +5,11 @@
                           ``train_epochs``, ``test``), the feed-forward branch (``use_rnn=False``);
 * ``MAPPO_Agents``        xuance/torch/agents/multi_agent_rl/mappo_agents.py:18-112.
 
-Scope: one parameter-sharing group, Discrete actions (with or without action masks), Basic_MLP representations.
+Scope: one parameter-sharing group, Discrete actions (with or without action masks), Basic_MLP representations or,
+with ``use_rnn=True``, the LayerNorm Basic_RNN whose GRU runs on K13 (``Basic_RNN_K13``).  The recurrent branch is the
+reference's: ``train`` repeats ``run_episodes(n_envs)`` -> ``train_epochs``; the actor and critic hidden states live on
+the device as [1, n_envs * n_agents, H] and a finished env's rows are zeroed there; acting runs K13 with T = 1 from the
+carried states.
 Acting: one staged upload of the vector step's observations ([n_envs * n_agents, obs_dim]), the actor, the mask as
 -1e10 logits (actor_head.py:40), K10 sampling on the device, the critic, and ONE device-to-host read of actions,
 log-probabilities and values."""
@@ -17,8 +21,10 @@ import torch
 import torch.nn as nn
 
 from ... import _lib
-from ...common import MARL_OnPolicyBuffer
-from ..rl_models import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic
+from ...common import MARL_OnPolicyBuffer, MARL_OnPolicyBuffer_RNN
+from ...common.spaces import space2shape
+from ..rl_models import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic, Basic_RNN_K13
+from ..rl_models.qmix import AgentFeatureEncoder
 from .marl import MARLAgents
 
 
@@ -33,9 +39,6 @@ class OnPolicyMARLAgents(MARLAgents):
 
     def __init__(self, config, envs=None, num_agents=None, agent_keys=None, state_space=None, observation_space=None,
                  action_space=None, callback=None):
-        if getattr(config, "use_rnn", False):
-            raise NotImplementedError("recurrent MAPPO (use_rnn=True: MARL_OnPolicyBuffer_RNN, episode-major on-policy "
-                                      "storage) is not supported; use a feed-forward representation")
         super().__init__(config, envs, num_agents, agent_keys, state_space, observation_space, action_space, callback)
         self.on_policy = True
         self.continuous_control = False
@@ -46,6 +49,15 @@ class OnPolicyMARLAgents(MARLAgents):
     def _build_memory(self):
         """on_policy_marl.py:77-98."""
         avail_shape = {k: (self.action_space[k].n,) for k in self.agent_keys} if self.use_actions_mask else None
+        if self.use_rnn:
+            return MARL_OnPolicyBuffer_RNN(agent_keys=self.agent_keys,
+                                           state_space=self.state_space if self.use_global_state else None,
+                                           obs_space=self.observation_space, act_space=self.action_space,
+                                           n_envs=self.n_envs, buffer_size=self.config.buffer_size,
+                                           max_episode_steps=self.episode_length, use_gae=self.config.use_gae,
+                                           use_advnorm=self.config.use_advnorm, gamma=self.config.gamma,
+                                           gae_lam=self.config.gae_lambda, avail_actions_shape=avail_shape,
+                                           use_actions_mask=self.use_actions_mask, device=self.device)
         return MARL_OnPolicyBuffer(agent_keys=self.agent_keys,
                                    state_space=self.state_space if self.use_global_state else None,
                                    obs_space=self.observation_space, act_space=self.action_space, n_envs=self.n_envs,
@@ -70,6 +82,8 @@ class OnPolicyMARLAgents(MARLAgents):
             data['state'] = np.array(kwargs['state'])
         if self.use_actions_mask:
             data['avail_actions'] = {k: np.array([d[k] for d in avail_actions]) for k in K}
+        if self.use_rnn:
+            data['episode_steps'] = np.array([d['episode_step'] - 1 for d in info])
         self.memory.store(**data)
 
     def _states(self, state, n_envs):
@@ -85,7 +99,10 @@ class OnPolicyMARLAgents(MARLAgents):
         n_envs, K = len(obs_list), self.agent_keys
         obs, avail = self._build_inputs(obs_list, avail_actions_list)
         obs_d = torch.from_numpy(obs).to(self.device)
-        logits = self.model.logits(obs_d)
+        if self.use_rnn:
+            logits, rnn_states_actor = self.model.logits(obs_d, rnn_states=rnn_states_actor, return_states=True)
+        else:
+            logits = self.model.logits(obs_d)
         if avail is not None:
             logits = logits.masked_fill(torch.from_numpy(avail).to(self.device) == 0, -1e10)
         logits = logits.contiguous()
@@ -96,22 +113,44 @@ class OnPolicyMARLAgents(MARLAgents):
         _lib.call("xb_categorical_act", _lib.ptr(logits), _lib.ptr(u), None, R, A, _lib.ptr(out[0]), _lib.ptr(acts_i),
                   _lib.ptr(out[1]), None)
         if not test_mode:
-            out[2] = self.model.values(obs_d, self._states(state, n_envs))
+            if self.use_rnn:
+                out[2], rnn_states_critic = self.model.values(obs_d, self._states(state, n_envs),
+                                                              rnn_states=rnn_states_critic, return_states=True)
+            else:
+                out[2] = self.model.values(obs_d, self._states(state, n_envs))
         host = out.cpu().numpy().reshape(3, n_envs, len(K))
         actions_list = [{k: int(host[0, e, i]) for i, k in enumerate(K)} for e in range(n_envs)]
         log_pi, values = {}, {}
         if not test_mode:
             log_pi = {k: host[1, :, i].copy() for i, k in enumerate(K)}
             values = {k: host[2, :, i].copy() for i, k in enumerate(K)}
-        return MARLActionOutput(env_actions=actions_list, log_probs=log_pi, values=values)
+        return MARLActionOutput(env_actions=actions_list, log_probs=log_pi, values=values,
+                                rnn_states_actor=rnn_states_actor, rnn_states_critic=rnn_states_critic)
 
     @torch.no_grad()
     def values_next(self, i_env, obs_dict, state=None, rnn_states_critic=None):
         """on_policy_marl.py:308-357."""
         obs, _ = self._build_inputs([obs_dict])
         st = None if state is None else np.asarray(state)[None]
-        v = self.model.values(torch.from_numpy(obs).to(self.device), self._states(st, 1)).cpu().numpy()
+        h = None
+        if self.use_rnn:      # the critic rows of env i (on_policy_marl.py:337-344)
+            n = len(self.agent_keys)
+            h = rnn_states_critic[:, i_env * n:(i_env + 1) * n]
+        v = self.model.values(torch.from_numpy(obs).to(self.device), self._states(st, 1), rnn_states=h).cpu().numpy()
         return None, {k: v[i] for i, k in enumerate(self.agent_keys)}
+
+    def init_rnn_states(self, n_envs):
+        """on_policy_marl.py:160-178: zero actor / critic states for n_envs envs (None without recurrence)."""
+        if not self.use_rnn:
+            return None, None
+        return self.model.init_rnn_states(n_envs * len(self.agent_keys))
+
+    def init_rnn_states_item(self, i_env, rnn_states_actor=None, rnn_states_critic=None):
+        """on_policy_marl.py:180-205: zero env i_env's rows."""
+        if not self.use_rnn:
+            return rnn_states_actor, rnn_states_critic
+        n = len(self.agent_keys)
+        return self.model.init_rnn_states_item(slice(i_env * n, (i_env + 1) * n), rnn_states_actor, rnn_states_critic)
 
     def _finish(self, i, terminated, next_obs, next_state):
         if all(terminated.values()):
@@ -122,8 +161,18 @@ class OnPolicyMARLAgents(MARLAgents):
                                 value_normalizer=self.learner.value_normalizer)
 
     def train(self, train_steps):
-        """on_policy_marl.py:405-482 (the feed-forward branch)."""
+        """on_policy_marl.py:384-482."""
         train_info = {}
+        if self.use_rnn:        # :384-403: whole episodes, then the epochs
+            step_start = self.current_step
+            while self.current_step - step_start < train_steps * self.n_envs:
+                self.run_episodes(n_episodes=self.n_envs, test_mode=False, close_envs=False)
+                update_info = self.train_epochs(n_epochs=self.n_epochs)
+                self.log_infos(update_info, self.current_step)
+                train_info.update(update_info)
+            self.callback.on_train_step_end(self.current_step, envs=self.train_envs, policy=self.model,
+                                            train_steps=train_steps, train_info=train_info)
+            return train_info
         envs = self.train_envs
         obs_list = envs.buf_obs
         avail_actions = envs.buf_avail_actions if self.use_actions_mask else None
@@ -180,16 +229,21 @@ class OnPolicyMARLAgents(MARLAgents):
         return train_info
 
     def run_episodes(self, n_episodes=1, deterministic_policy=False, run_envs=None, test_mode=False, close_envs=True):
-        """on_policy_marl.py:484-630 (feed-forward; no rendering)."""
+        """on_policy_marl.py:484-630 (no rendering)."""
         envs = self.train_envs if run_envs is None else run_envs
         num_envs = envs.num_envs
         _current_episode, scores = 0, []
         obs_list, info = envs.reset()
         avail_actions = envs.buf_avail_actions if self.use_actions_mask else None
         state = envs.buf_state if self.use_global_state else None
+        if self.use_rnn and not test_mode:
+            self.memory.clear_episodes()        # :523-525: a fresh staging per call (not per episode)
+        rnn_states_actor, rnn_states_critic = self.init_rnn_states(num_envs)
         while _current_episode < n_episodes:
             policy_out = self.get_actions(obs_list=obs_list, state=state, avail_actions_list=avail_actions,
+                                          rnn_states_actor=rnn_states_actor, rnn_states_critic=rnn_states_critic,
                                           test_mode=test_mode, deterministic=deterministic_policy)
+            rnn_states_actor, rnn_states_critic = policy_out.rnn_states_actor, policy_out.rnn_states_critic
             actions_list = policy_out.env_actions
             next_obs_list, rewards_list, terminated_list, truncated, info = envs.step(actions_list)
             next_state = envs.buf_state if self.use_global_state else None
@@ -203,8 +257,22 @@ class OnPolicyMARLAgents(MARLAgents):
                 if all(terminated_list[i].values()) or truncated[i]:
                     _current_episode += 1
                     scores.append(float(np.mean(itemgetter(*self.agent_keys)(info[i]["episode_score"]))))
+                    if not test_mode and self.use_rnn:
+                        if all(terminated_list[i].values()):
+                            value_next = {k: 0.0 for k in self.agent_keys}
+                        else:
+                            _, value_next = self.values_next(i_env=i, obs_dict=obs_list[i],
+                                                             state=None if state is None else state[i],
+                                                             rnn_states_critic=rnn_states_critic)
+                        self.memory.finish_path(i_env=i, i_step=info[i]['episode_step'],
+                                                agent_grouping=self.agent_grouping, value_next=value_next,
+                                                value_normalizer=self.learner.value_normalizer)
+                    if self.use_rnn:
+                        rnn_states_actor, rnn_states_critic = self.init_rnn_states_item(
+                            i, rnn_states_actor, None if test_mode else rnn_states_critic)
                     if not test_mode:
-                        self._finish(i, terminated_list[i], obs_list[i], None if state is None else state[i])
+                        if not self.use_rnn:
+                            self._finish(i, terminated_list[i], obs_list[i], None if state is None else state[i])
                         self.current_step += info[i]["episode_step"]
                         self.callback.on_train_episode_info(envs=envs, policy=self.model, env_id=i, infos=info,
                                                             rank=self.rank, use_wandb=self.use_wandb,
@@ -230,7 +298,7 @@ class OnPolicyMARLAgents(MARLAgents):
         """on_policy_marl.py:632-661: shuffled n_minibatch slices per epoch; the info of the last update (only that
         one reads the device statistics back)."""
         info_train = {}
-        if self.memory.full:
+        if self.memory.full:       # buffer_size counts steps per env-row, or episodes with use_rnn
             indexes = np.arange(self.buffer_size)
             for e in range(n_epochs):
                 np.random.shuffle(indexes)
@@ -261,6 +329,19 @@ class MAPPO_Agents(OnPolicyMARLAgents):
         self.model = self._build_model()
         self.memory = self._build_memory()
         self.learner = self._build_learner(self.config, self.agent_grouping, self.model, self.callback)
+
+    def _build_agent_feature_encoder(self, representation_choice, group_agents, input_space):
+        if not self.use_rnn:
+            return super()._build_agent_feature_encoder(representation_choice, group_agents, input_space)
+        if representation_choice != "Basic_RNN":
+            raise NotImplementedError("use_rnn=True (recurrent MAPPO) takes representation: Basic_RNN, got %s"
+                                      % representation_choice)
+        c = self.config
+        return AgentFeatureEncoder(Basic_RNN_K13(
+            input_shape=space2shape(input_space), normalize=self.normalize_fn, initialize=nn.init.orthogonal_,
+            activation=self.activation, device=self.device, fc_hidden_sizes=c.fc_hidden_sizes,
+            recurrent_hidden_size=c.recurrent_hidden_size, N_recurrent_layers=getattr(c, "N_recurrent_layers", 1),
+            rnn=getattr(c, "rnn", "GRU"), dropout=getattr(c, "dropout", 0)))
 
     def _build_model(self):
         actors, critics, critic_encoders = nn.ModuleDict(), nn.ModuleDict(), nn.ModuleDict()

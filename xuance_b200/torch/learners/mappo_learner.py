@@ -5,7 +5,12 @@ update(sample): actor and critic forward over the packed rows -> ``xb_mappo_prep
 of the returns) -> [all-reduce of that 4-double block] -> ``xb_value_norm_update`` (use_value_norm) -> K4M fused loss
 forward + backward (dlogits, dvalue, statistics into the bucket tail) -> torch backward into the flat bucket ->
 [one all-reduce of gradient + statistics] -> K7 clip + Adam.  No host synchronisation until the info dict is built, so
-the device half is capturable as a CUDA graph (``use_cuda_graph``)."""
+the device half is capturable as a CUDA graph (``use_cuda_graph``).
+
+With ``use_rnn`` the batch is B whole episodes: the actor and the critic run over the [B*n, T] sequences from zero states
+(the GRU recurrence on K13, captured with the rest), and K4M runs over the R = B*n*T rows with mask = agent_mask * filled
+(modules/outputs.py:133-143 ``valid_mask``).  The ValueNorm update and predict_value see every row, masked or not, as in
+the reference."""
 import torch
 
 from ... import _lib
@@ -28,6 +33,7 @@ class MAPPO_Learner(Learner):
         self.use_value_clip, self.value_clip_range = config.use_value_clip, config.value_clip_range
         self.use_huber_loss, self.huber_delta = config.use_huber_loss, config.huber_delta
         self.use_value_norm = config.use_value_norm
+        self.use_rnn = getattr(config, "use_rnn", False)
         self.vf_coef, self.ent_coef = config.vf_coef, config.ent_coef
         # LearnerMAS.build_optimizer (marl_learner.py:64-76): Adam(eps=1e-5) + LinearLR, stepped only with decay on
         self.optimizer = FusedAdam(self.model.parameters(), lr=self.learning_rate, eps=1e-5,
@@ -45,7 +51,10 @@ class MAPPO_Learner(Learner):
 
     def estimate_total_iterations(self):
         """marl_learner.py:203-214."""
-        update_times = self.config.running_steps // self.config.buffer_size
+        if getattr(self.config, "use_rnn", False):
+            update_times = (self.config.running_steps // self.config.episode_length) // self.config.buffer_size
+        else:
+            update_times = self.config.running_steps // self.config.buffer_size
         return update_times * getattr(self.config, "n_epochs", 1) * getattr(self.config, "n_minibatch", 1)
 
     def _snapshot(self):
@@ -66,9 +75,10 @@ class MAPPO_Learner(Learner):
         """mappo_learner.py:41-137 on the device (static shapes, no host synchronisation)."""
         R = actions.shape[0]
         R_total = R * self.world_size
-        logits = self.model.logits(obs).contiguous()
-        v_pred = self.model.values(obs, state if self.use_global_state else None).contiguous()
+        logits = self.model.logits(obs)
         A = logits.shape[-1]
+        logits = logits.reshape(-1, A).contiguous()             # [B*n, T, A] -> rows (recurrent batches)
+        v_pred = self.model.values(obs, state if self.use_global_state else None).reshape(-1).contiguous()
         _lib.call("xb_mappo_prepare", _lib.ptr(mask), _lib.ptr(returns), R, _lib.ptr(self._prep),
                   _lib.ptr(self._scratch))
         if self.world_size > 1:
@@ -94,12 +104,17 @@ class MAPPO_Learner(Learner):
 
     def _args(self, sample):
         st = sample['_stacked']
-        args = [st['obs'], st['actions'], st['log_pi_old'], st['advantages'], st['values'], st['returns'],
-                st['agent_mask']]
+        if self.use_rnn:            # [B*n, T] fields -> B*n*T rows; the loss mask is agent_mask * filled
+            f = lambda k: st[k].reshape(-1)
+            args = [st['obs'], f('actions'), f('log_pi_old'), f('advantages'), f('values'), f('returns'),
+                    (st['agent_mask'] * st['filled']).reshape(-1)]
+        else:
+            args = [st['obs'], st['actions'], st['log_pi_old'], st['advantages'], st['values'], st['returns'],
+                    st['agent_mask']]
         avail = st.get('avail_actions') if self.use_actions_mask else None
         state = st.get('state') if self.use_global_state else None
         if avail is not None:
-            avail = avail.contiguous()
+            avail = avail.reshape(-1, avail.shape[-1]).contiguous()
         return [a.contiguous() for a in args] + [avail, state]
 
     def update(self, sample, sync=True):

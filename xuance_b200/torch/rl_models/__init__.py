@@ -12,3 +12,4 @@ from .architectures import (ActorCritic, SharedActorCritic, DeepQNetwork, Duelin
 from .qmix import Basic_RNN, AgentFeatureEncoder, DiscreteActionValueCritic, QMIX_Mixer, VDN_mixer, MixingQNetwork
 REGISTRY_Representation["Basic_RNN"] = Basic_RNN
 from .mappo import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic
+from .gru import GRUSequence, gru_sequence, Basic_RNN_K13

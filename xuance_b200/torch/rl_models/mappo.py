@@ -27,8 +27,11 @@ class CategoricalActor(nn.Module):
                                                normalizer=normalizer, initializer=initializer, activation=activation,
                                                device=device)
 
-    def logits(self, observations):
-        return self.actor_head.logits(self.representation(observations).embeddings)
+    def logits(self, observations, rnn_states=None, return_states=False):
+        """Recurrent representations take [S, T, obs] (or [S, obs] for one step) and the state [1, S, H]."""
+        rep = self.representation(observations, rnn_hidden=rnn_states)
+        out = self.actor_head.logits(rep.embeddings)
+        return (out, rep.rnn_states) if return_states else out
 
 
 class CentralizedStateValueCritic(nn.Module):
@@ -46,23 +49,40 @@ class CentralizedStateValueCritic(nn.Module):
                                      normalizer=normalizer, initializer=initializer, activation=activation,
                                      device=device)
 
-    def values(self, observations, states=None):
-        x = self.representations[self.group_keys[0]](observations).embeddings
+    def values(self, observations, states=None, rnn_states=None, return_states=False):
+        rep = self.representations[self.group_keys[0]](observations, rnn_hidden=rnn_states)
+        x = rep.embeddings
         if states is not None:
             x = torch.cat([states, x], dim=-1)
-        return self.critic_head(x)
+        out = self.critic_head(x)
+        return (out, rep.rnn_states) if return_states else out
 
 
 class MultiAgentActorCritic(nn.Module):
     def __init__(self, grouping, actors, critics, use_rnn=False, device=None, **kwargs):
         super().__init__()
-        if use_rnn:
-            raise NotImplementedError("recurrent MAPPO (use_rnn=True, MARL_OnPolicyBuffer_RNN) is not supported")
         self.grouping, self.group_keys = grouping, grouping.group_keys
         self.actors, self.critics = actors, critics
+        self.use_rnn = use_rnn
 
-    def logits(self, observations, group=None):
-        return self.actors[group or self.group_keys[0]].logits(observations)
+    def logits(self, observations, group=None, rnn_states=None, return_states=False):
+        return self.actors[group or self.group_keys[0]].logits(observations, rnn_states, return_states)
 
-    def values(self, observations, states=None, group=None):
-        return self.critics[group or self.group_keys[0]].values(observations, states)
+    def values(self, observations, states=None, group=None, rnn_states=None, return_states=False):
+        return self.critics[group or self.group_keys[0]].values(observations, states, rnn_states, return_states)
+
+    # ---- recurrent states (actor_critic.py init_rnn_states / init_rnn_states_item): rows are (env, agent) pairs
+    def _rnn(self, part):
+        g = self.group_keys[0]
+        return (self.actors[g].representation if part == "actor" else self.critics[g].representations[g]).obs_representation
+
+    def init_rnn_states(self, n_rows):
+        """Zero actor and critic hidden states [1, n_rows, H] on the device."""
+        return self._rnn("actor").init_rnn_states(n_rows), self._rnn("critic").init_rnn_states(n_rows)
+
+    def init_rnn_states_item(self, rows, rnn_states_actor, rnn_states_critic=None):
+        """Zero the rows of a finished env in place, on the device."""
+        rnn_states_actor[:, rows] = 0.0
+        if rnn_states_critic is not None:
+            rnn_states_critic[:, rows] = 0.0
+        return rnn_states_actor, rnn_states_critic
