@@ -14,74 +14,29 @@ One collective per optimiser step, critic then actor (they cannot merge: the act
 import torch
 
 from ... import _lib
-from ..utils import FusedAdam, FlatBucket, allreduce_sum_, CapturedStep
-from .learner import Learner
+from .sac_learner import _ActorCritic_Learner
 
 
-def _target_bucket(target, live_bucket):
-    """The target network's parameters in their own flat array, in the live bucket's parameter order and layout."""
-    params = list(target.parameters())
-    bucket = FlatBucket([p.requires_grad_(True) for p in params])
-    for p in params:
-        p.requires_grad_(False)
-        p.grad = None
-    assert bucket.numel == live_bucket.numel and bucket.offsets == live_bucket.offsets
-    return bucket
-
-
-class DDPG_Learner(Learner):
+class DDPG_Learner(_ActorCritic_Learner):
     twin = False
+    target_names = ('actor', 'critic')
 
     def __init__(self, config, model, callback):
         super().__init__(config, model, callback)
-        self.optimizer = {
-            'actor': FusedAdam(self.model.actor.parameters(), self.config.learning_rate_actor),
-            'critic': FusedAdam(self.model.critic.parameters(), self.config.learning_rate_critic)}
-        mk = lambda o: torch.optim.lr_scheduler.LinearLR(o, start_factor=1.0, end_factor=self.end_factor_lr_decay,
-                                                         total_iters=self.total_iters)
-        self.scheduler = {'actor': mk(self.optimizer['actor']), 'critic': mk(self.optimizer['critic'])}
-        self._targets = {'actor': _target_bucket(self.model.target_actor, self.optimizer['actor'].bucket),
-                         'critic': _target_bucket(self.model.target_critic, self.optimizer['critic'].bucket)}
-        self.tau, self.gamma = config.tau, config.gamma
         self.actor_update_delay = getattr(config, "actor_update_delay") if self.twin else 1
-        self.use_cuda_graph = getattr(config, "use_cuda_graph", False)
-        self._graphs = {}
         # the logged statistics ride in the tails of the two gradient buckets (the same collective as the gradient)
         self._stats_a = self.optimizer['actor'].bucket.tail[:4]
         self._stats_c = self.optimizer['critic'].bucket.tail[:4]
         self._scratch = _lib.scratch(self.device)
 
-    def _f32(self, x):
-        return torch.as_tensor(x, device=self.device).to(torch.float32).contiguous()
-
-    def _snapshot(self):
-        st = {k: v.snapshot() for k, v in self.optimizer.items()}
-        st.update({"target_" + k: v.flat.clone() for k, v in self._targets.items()})
-        return st
-
-    def _restore(self, st):
-        for k, v in self.optimizer.items():
-            v.restore(st[k])
-        for k, v in self._targets.items():
-            v.flat.copy_(st["target_" + k])
-
     @staticmethod
     def _flat(x):
         return None if x is None else x.reshape(-1).contiguous()
-
-    def _step(self, name, outputs, grads, clip, inputs=None):
-        opt = self.optimizer[name]
-        opt.zero_grad()
-        torch.autograd.backward(outputs, grads, inputs=inputs)
-        if self.world_size > 1:
-            allreduce_sum_(opt.bucket.grad_all)
-        opt.launch(max_norm=clip)
 
     def _device_update(self, obs, act, nxt, rew, ter, actor_step, noise_next=None):
         """Everything of one update that runs on the device; static shapes, no host synchronisation."""
         B = obs.shape[0]
         Bt = B * self.world_size
-        clip = self.grad_clip_norm if self.use_grad_clip else None
         P, F = _lib.ptr, self._flat
 
         # ---- critic step (ddpg_learner.py:45-54, td3_learner.py:46-59)
@@ -94,7 +49,7 @@ class DDPG_Learner(Learner):
         _lib.call("xb_ddpg_critic_loss", P(q1), P(q2), P(tq1), P(tq2), P(rew), P(ter), float(self.gamma), B, Bt, P(dq1),
                   P(dq2), P(backup), P(self._stats_c), P(self._scratch))
         outs, grads = ([q1, q2], [dq1, dq2]) if self.twin else ([q1], [dq1])
-        self._step('critic', outs, grads, clip)
+        self._optimizer_step(self.optimizer['critic'], outs, grads)
 
         # ---- actor step on the updated critic (ddpg_learner.py:56-63, td3_learner.py:63-73)
         if actor_step:
@@ -104,11 +59,8 @@ class DDPG_Learner(Learner):
             _lib.call("xb_ddpg_actor_loss", P(p1), P(p2), B, Bt, P(dp1), P(dp2), P(self._stats_a), P(self._scratch))
             outs, grads = ([p1, p2], [dp1, dp2]) if self.twin else ([p1], [dp1])
             # the reference's p_loss.backward() also fills the critic's gradients; its next zero_grad discards them
-            self._step('actor', outs, grads, clip, inputs=self.optimizer['actor'].bucket.params)
-            # ---- Polyak update of both targets (actor_critic.py:255-261, 313-319)
-            for k, tgt in self._targets.items():
-                live = self.optimizer[k].bucket
-                _lib.call("xb_soft_update", P(tgt.flat), P(live.flat), live.numel, float(self.tau))
+            self._optimizer_step(self.optimizer['actor'], outs, grads, inputs=self.optimizer['actor'].bucket.params)
+            self._soft_update()
         return None
 
     def update(self, sync=True, noise_next=None, **samples):
@@ -125,14 +77,8 @@ class DDPG_Learner(Learner):
             self.optimizer['actor'].prepare()
         noise = None if noise_next is None or not self.twin else self._f32(noise_next)
         args = [obs, act, nxt, rew, ter] + ([] if noise is None else [noise])
-        if self.use_cuda_graph:
-            key = (tuple(obs.shape), actor_step, len(args))
-            if key not in self._graphs:
-                fn = lambda *a, s=actor_step: self._device_update(*a[:5], s, *a[5:])
-                self._graphs[key] = CapturedStep(fn, args, self._snapshot, self._restore)
-            self._graphs[key](*args)
-        else:
-            self._device_update(*args[:5], actor_step, *args[5:])
+        self._device_step((tuple(obs.shape), actor_step, len(args)),
+                          lambda *a: self._device_update(*a[:5], actor_step, *a[5:]), *args)
         self.scheduler['critic'].step()
         if actor_step:
             self.scheduler['actor'].step()
@@ -147,10 +93,7 @@ class DDPG_Learner(Learner):
                 vals["Qvalue"] = sc[1]
             vals.update(actor_lr=self.optimizer['actor'].param_groups[0]['lr'],
                         critic_lr=self.optimizer['critic'].param_groups[0]['lr'])
-            if self.distributed_training:
-                vals = {f"{k}/rank_{self.rank}": v for k, v in vals.items()}
-            info.update(vals)
-            info.update(self.callback.on_update_end(self.iterations, model=self.model, info=info) or {})
+            self._finish_info(info, vals, model=self.model)
         return info
 
 

@@ -9,7 +9,6 @@ the info dict; ``use_cuda_graph`` captures the device part per input shape, as D
 import torch
 
 from ... import _lib
-from ..utils import allreduce_sum_
 from .dqn_learner import DQN_Learner
 
 
@@ -23,11 +22,7 @@ class _DistDQN_Learner(DQN_Learner):
         grad = torch.empty_like(z)
         target_actions = torch.empty(z.shape[0], dtype=torch.int64, device=z.device)
         self._loss(z, zn, act, rew, ter, grad, target_actions)
-        self.optimizer.zero_grad()
-        torch.autograd.backward([z], [grad])
-        if self.world_size > 1:
-            allreduce_sum_(self.optimizer.bucket.grad_all)   # the one collective: gradient + logged statistic
-        self.optimizer.launch(max_norm=self.grad_clip_norm if self.use_grad_clip else None)
+        self._optimizer_step(self.optimizer, [z], [grad])
 
     def _info_values(self):
         """c51_learner.py:65-74 / qrdqn_learner.py:62-71: the reference's keys, Qloss and learning_rate."""

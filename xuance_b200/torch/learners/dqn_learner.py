@@ -8,7 +8,7 @@ the PER sample are ignored, as in the reference (appendix B #8)."""
 import torch
 
 from ... import _lib
-from ..utils import FusedAdam, allreduce_sum_, CapturedStep
+from ..utils import FusedAdam
 from .learner import Learner
 
 
@@ -20,27 +20,13 @@ class DQN_Learner(Learner):
         super().__init__(config, model, callback)
         params = model.eval_parameters() if hasattr(model, "eval_parameters") else model.parameters()
         self.optimizer = FusedAdam(params, self.config.learning_rate, eps=1e-5)
-        self.scheduler = torch.optim.lr_scheduler.LinearLR(self.optimizer, start_factor=1.0,
-                                                           end_factor=self.end_factor_lr_decay,
-                                                           total_iters=self.total_iters)
+        self.scheduler = self._linear_lr(self.optimizer)
         self.gamma = config.gamma
         self.sync_frequency = config.sync_frequency
         self.n_actions = self.model.n_actions
         self._stats = self.optimizer.bucket.tail[:4]       # logged sums ride in the gradient all-reduce (bucket tail)
         self._scratch = _lib.scratch(self.device)
-        self.use_cuda_graph = getattr(config, "use_cuda_graph", False)
-        self._graphs = {}
-
-    def _f32(self, x):
-        return torch.as_tensor(x, device=self.device).to(torch.float32).contiguous()
-
-    def _snapshot(self):
-        return (self.optimizer.snapshot(), [p.detach().clone() for p in self.model.target_parameters()])
-
-    def _restore(self, st):
-        self.optimizer.restore(st[0])
-        for p, q in zip(self.model.target_parameters(), st[1]):
-            p.data.copy_(q)
+        self._graph_tensors = list(self.model.target_parameters())
 
     def _device_update(self, obs, nxt, act, rew, ter):
         """dqn_learner.py:38-52 on the device: no host synchronisation, static shapes (CUDA-graph capturable)."""
@@ -54,11 +40,7 @@ class DQN_Learner(Learner):
         _lib.call("xb_dqn_td_fwd_bwd", _lib.ptr(evalQ), _lib.ptr(targetQ), _lib.ptr(selQ), _lib.ptr(act), _lib.ptr(rew),
                   _lib.ptr(ter), B, A, B * self.world_size, float(self.gamma), _lib.ptr(dq), _lib.ptr(td),
                   _lib.ptr(self._stats), _lib.ptr(self._scratch))
-        self.optimizer.zero_grad()
-        torch.autograd.backward([evalQ], [dq])
-        if self.world_size > 1:
-            allreduce_sum_(self.optimizer.bucket.grad_all)   # the one collective: gradient + logged statistics
-        self.optimizer.launch(max_norm=self.grad_clip_norm if self.use_grad_clip else None)
+        self._optimizer_step(self.optimizer, [evalQ], [dq])
         return td.abs()
 
     def update(self, sync=True, **samples):
@@ -69,24 +51,13 @@ class DQN_Learner(Learner):
         info = self.callback.on_update_start(self.iterations, model=self.model, obs=obs, act=act, next_obs=nxt,
                                              rew=rew, termination=ter) or {}
         self.optimizer.prepare()
-        if self.use_cuda_graph:        # NCCL captures into the graph as in the PPO path
-            key = (tuple(obs.shape), obs.dtype)
-            if key not in self._graphs:
-                self._graphs[key] = CapturedStep(self._device_update, [obs, nxt, act, rew, ter], self._snapshot,
-                                                 self._restore)
-            abs_td = self._graphs[key](obs, nxt, act, rew, ter)
-        else:
-            abs_td = self._device_update(obs, nxt, act, rew, ter)
+        abs_td = self._device_step((tuple(obs.shape), obs.dtype), self._device_update, obs, nxt, act, rew, ter)
         if self.scheduler is not None:
             self.scheduler.step()
         if self.iterations % self.sync_frequency == 0:
             self.model.copy_target()
         if sync:
-            vals = self._info_values()
-            if self.distributed_training:
-                vals = {f"{k}/rank_{self.rank}": v for k, v in vals.items()}
-            info.update(vals)
-            info.update(self.callback.on_update_end(self.iterations, model=self.model, info=info) or {})
+            self._finish_info(info, self._info_values(), model=self.model)
         if self.returns_td:
             return abs_td, info   # |td| stays on the device; PerOffPolicyBuffer.update_priorities takes it as is
         return info

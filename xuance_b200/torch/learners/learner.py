@@ -12,9 +12,12 @@ import torch
 import torch.distributed as dist
 
 from ... import _lib
+from ..utils import allreduce_sum_, CapturedStep
 
 
 class Learner(ABC):
+    rank_suffix = True       # info keys get "/rank_{r}" in distributed runs; the reference's MARL learners log without it
+
     def __init__(self, config, model, callback):
         self.value_normalizer = None
         self.config = config
@@ -49,6 +52,11 @@ class Learner(ABC):
         self.model_dir = getattr(config, "model_dir", "./models")
         self.total_iters = self.estimate_total_iterations()
         self.iterations = 0
+        self.use_cuda_graph = getattr(config, "use_cuda_graph", False)
+        self._graphs = {}
+        # device tensors a graphed update mutates besides the FusedAdam state (target networks, running statistics):
+        # the warm-up runs of a CUDA-graph capture are real, so _snapshot / _restore must cover all of them
+        self._graph_tensors = []
 
     def estimate_total_iterations(self):
         """drl_learner.py:57-62."""
@@ -56,12 +64,64 @@ class Learner(ABC):
         training_frequency = getattr(self.config, "training_frequency", 1)
         return (self.config.running_steps - start_training) // (training_frequency * self.config.parallels)
 
+    # ---------------------------------------------------------------- the update protocol shared by every learner
+    def _f32(self, x):
+        return torch.as_tensor(x, device=self.device).to(torch.float32).contiguous()
+
+    def _linear_lr(self, optimizer, total_iters=None):
+        """The reference's LinearLR schedule from 1 to ``end_factor_lr_decay`` over ``total_iters`` (default: the
+        estimated update count)."""
+        return torch.optim.lr_scheduler.LinearLR(optimizer, start_factor=1.0, end_factor=self.end_factor_lr_decay,
+                                                 total_iters=self.total_iters if total_iters is None else total_iters)
+
+    def _optimizer_step(self, opt, outputs, grads, inputs=None):
+        """Backward of ``outputs`` seeded with ``grads`` into ``opt``'s flat bucket (restricted to ``inputs`` if given),
+        ONE all-reduce of gradient + logged statistics when sharded, then the K7 clip + Adam step."""
+        opt.zero_grad()
+        torch.autograd.backward(outputs, grads, inputs=inputs)
+        if self.world_size > 1:
+            allreduce_sum_(opt.bucket.grad_all)
+        opt.launch(max_norm=self.grad_clip_norm if self.use_grad_clip else None)
+
+    def _device_step(self, key, fn, *args):
+        """Runs ``fn(*args)``, the device half of an update: eagerly, or with ``use_cuda_graph`` as the replay of a graph
+        captured once per ``key`` (``key=None`` runs eagerly).  Returns what ``fn`` returns (a graph's static output)."""
+        if not self.use_cuda_graph or key is None:
+            return fn(*args)
+        if key not in self._graphs:
+            self._graphs[key] = CapturedStep(fn, list(args), self._snapshot, self._restore)
+        return self._graphs[key](*args)
+
+    def _optimizers(self):
+        """Every FusedAdam a device update steps."""
+        return list(self.optimizer.values()) if isinstance(self.optimizer, dict) else [self.optimizer]
+
+    def _snapshot(self):
+        return [o.snapshot() for o in self._optimizers()], [t.detach().clone() for t in self._graph_tensors]
+
+    def _restore(self, st):
+        for o, s in zip(self._optimizers(), st[0]):
+            o.restore(s)
+        with torch.no_grad():
+            for t, s in zip(self._graph_tensors, st[1]):
+                t.copy_(s)
+
+    def _with_rank(self, vals):
+        if self.distributed_training and self.rank_suffix:
+            return {f"{k}/rank_{self.rank}": v for k, v in vals.items()}
+        return vals
+
+    def _finish_info(self, info, vals, **models):
+        """Adds an update's logged values to ``info`` and runs the callback's on_update_end (``models``: the keyword the
+        reference passes the network under, ``model=`` or ``policy=``)."""
+        info.update(self._with_rank(vals))
+        info.update(self.callback.on_update_end(self.iterations, info=info, **models) or {})
+        return info
+
     # ---------------------------------------------------------------- checkpoints (reference format)
     def _opt_state(self):
         if isinstance(self.optimizer, dict):
             return {k: v.state_dict() for k, v in self.optimizer.items()}
-        if isinstance(self.optimizer, list):
-            return [o.state_dict() for o in self.optimizer]
         return self.optimizer.state_dict()
 
     def save_model(self, model_path):
@@ -96,9 +156,6 @@ class Learner(ABC):
                 for k, v in self.optimizer.items():
                     if k in opt:
                         v.load_state_dict(opt[k])
-            elif isinstance(self.optimizer, list):
-                for o, s in zip(self.optimizer, opt):
-                    o.load_state_dict(s)
             elif self.optimizer is not None:
                 self.optimizer.load_state_dict(opt)
         self._restore_rng(ckpt)
@@ -147,9 +204,6 @@ class Learner(ABC):
             if isinstance(self.optimizer, dict):
                 for k, v in self.optimizer.items():
                     v.load_state_dict(opt[k])
-            elif isinstance(self.optimizer, list):
-                for o, st in zip(self.optimizer, opt):
-                    o.load_state_dict(st)
             else:
                 self.optimizer.load_state_dict(opt)
         self._restore_rng(snap)

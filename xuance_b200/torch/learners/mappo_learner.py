@@ -14,11 +14,13 @@ the reference."""
 import torch
 
 from ... import _lib
-from ..utils import FusedAdam, allreduce_sum_, CapturedStep, ValueNorm
+from ..utils import FusedAdam, allreduce_sum_, ValueNorm
 from .learner import Learner
 
 
 class MAPPO_Learner(Learner):
+    rank_suffix = False
+
     def __init__(self, config, agent_grouping, model, callback):
         super().__init__(config, model, callback)
         self.use_parameter_sharing = getattr(config, "use_parameter_sharing", True)
@@ -38,16 +40,15 @@ class MAPPO_Learner(Learner):
         # LearnerMAS.build_optimizer (marl_learner.py:64-76): Adam(eps=1e-5) + LinearLR, stepped only with decay on
         self.optimizer = FusedAdam(self.model.parameters(), lr=self.learning_rate, eps=1e-5,
                                    weight_decay=getattr(config, "weight_decay", 0.0))
-        self.scheduler = torch.optim.lr_scheduler.LinearLR(self.optimizer, start_factor=1.0,
-                                                           end_factor=self.end_factor_lr_decay,
-                                                           total_iters=self.total_iters)
+        self.scheduler = self._linear_lr(self.optimizer)
         self.value_normalizer = ({k: ValueNorm(1, device=self.device) for k in self.group_keys}
                                  if self.use_value_norm else None)
         self._prep = torch.zeros(4, dtype=torch.float64, device=self.device)
         self._stats = self.optimizer.bucket.tail[:8]
         self._scratch = _lib.scratch(self.device)
-        self.use_cuda_graph = getattr(config, "use_cuda_graph", False)
-        self._graphs = {}
+        if self.value_normalizer is not None:
+            self._graph_tensors = [t for v in self.value_normalizer.values()
+                                   for t in (v.running_mean, v.running_mean_sq, v.debiasing_term)]
 
     def estimate_total_iterations(self):
         """marl_learner.py:203-214."""
@@ -56,20 +57,6 @@ class MAPPO_Learner(Learner):
         else:
             update_times = self.config.running_steps // self.config.buffer_size
         return update_times * getattr(self.config, "n_epochs", 1) * getattr(self.config, "n_minibatch", 1)
-
-    def _snapshot(self):
-        vn = [] if self.value_normalizer is None else [t.detach().clone() for v in self.value_normalizer.values()
-                                                       for t in (v.running_mean, v.running_mean_sq, v.debiasing_term)]
-        return (self.optimizer.snapshot(), vn)
-
-    def _restore(self, st):
-        self.optimizer.restore(st[0])
-        if self.value_normalizer is not None:
-            ts = [t for v in self.value_normalizer.values()
-                  for t in (v.running_mean, v.running_mean_sq, v.debiasing_term)]
-            with torch.no_grad():
-                for t, s in zip(ts, st[1]):
-                    t.copy_(s)
 
     def _device_update(self, obs, actions, old_logp, adv, values_old, returns, mask, avail=None, state=None):
         """mappo_learner.py:41-137 on the device (static shapes, no host synchronisation)."""
@@ -95,11 +82,7 @@ class MAPPO_Learner(Learner):
                   float(self.clip_range), float(self.value_clip_range) if self.use_value_clip else 0.0,
                   float(self.huber_delta) if self.use_huber_loss else 0.0, float(self.vf_coef), float(self.ent_coef),
                   _lib.ptr(dlogits), _lib.ptr(dvalue), _lib.ptr(self._stats), _lib.ptr(self._scratch))
-        self.optimizer.zero_grad()
-        torch.autograd.backward([logits, v_pred], [dlogits, dvalue])
-        if self.world_size > 1:
-            allreduce_sum_(self.optimizer.bucket.grad_all)   # gradient + logged statistics in one collective
-        self.optimizer.launch(max_norm=self.grad_clip_norm if self.use_grad_clip else None)
+        self._optimizer_step(self.optimizer, [logits, v_pred], [dlogits, dvalue])
         return None
 
     def _args(self, sample):
@@ -122,22 +105,15 @@ class MAPPO_Learner(Learner):
         args = self._args(sample)
         info = self.callback.on_update_start(self.iterations, model=self.model, batch=sample) or {}
         self.optimizer.prepare()
-        if self.use_cuda_graph:
-            key = tuple(args[0].shape)
-            if key not in self._graphs:
-                self._graphs[key] = CapturedStep(self._device_update, args, self._snapshot, self._restore)
-            self._graphs[key](*args)
-        else:
-            self._device_update(*args)
+        self._device_step(tuple(args[0].shape), self._device_update, *args)
         if self.scheduler is not None and self.use_linear_lr_decay:
             self.scheduler.step()
         if sync:
             s = self._stats.tolist()
             g = self.group_keys[0]
-            info.update({f"{g}/actor_loss": s[0], f"{g}/critic_loss": s[1], f"{g}/entropy": s[2],
-                         f"{g}/predict_value": s[3]})
+            vals = {f"{g}/actor_loss": s[0], f"{g}/critic_loss": s[1], f"{g}/entropy": s[2], f"{g}/predict_value": s[3]}
             if self.use_grad_clip:
-                info["gradient_norm"] = float(self.optimizer.grad_norm.item())
-            info.update({"learning_rate": self.optimizer.param_groups[0]['lr'], "loss": s[4]})
-            info.update(self.callback.on_update_end(self.iterations, model=self.model, info=info) or {})
+                vals["gradient_norm"] = float(self.optimizer.grad_norm.item())
+            vals.update({"learning_rate": self.optimizer.param_groups[0]['lr'], "loss": s[4]})
+            self._finish_info(info, vals, model=self.model)
         return info

@@ -9,7 +9,7 @@ import torch
 
 from ... import _lib
 from ..rl_models.heads import GaussianActorHead
-from ..utils import FusedAdam, allreduce_sum_
+from ..utils import FusedAdam
 from .learner import Learner
 
 
@@ -21,9 +21,7 @@ class PPO_Learner(Learner):
     def __init__(self, config, model, callback):
         super().__init__(config, model, callback)
         self.optimizer = FusedAdam(self.model.parameters(), self.config.learning_rate, eps=1e-5)
-        self.scheduler = torch.optim.lr_scheduler.LinearLR(self.optimizer, start_factor=1.0,
-                                                           end_factor=self.end_factor_lr_decay,
-                                                           total_iters=self._lr_total_iters())
+        self.scheduler = self._linear_lr(self.optimizer, self._lr_total_iters())
         self.vf_coef, self.ent_coef = getattr(config, "vf_coef", 0.0), config.ent_coef
         self.clip_range = getattr(config, "clip_range", 0.0)
         self._stats = self.optimizer.bucket.tail[:8]      # the logged sums travel in the gradient bucket's tail
@@ -31,35 +29,6 @@ class PPO_Learner(Learner):
         # a GaussianActorHead (Box action space) takes the K4G branch of _device_update
         self._gaussian = isinstance(getattr(self.model, "actor", None), GaussianActorHead)
         self._ws = None
-        self._early = None
-        self._hook_early_allreduce()
-
-    def _hook_early_allreduce(self):
-        """Optional (XB_EARLY_ALLREDUCE=1): the bulk of the gradient (the 6400->512 layer and the heads, 98 % of the parameters) is
-        final before the convolution backward starts, so its all-reduce can be issued there (async, on NCCL's stream) and
-        what remains - [statistics | convolution gradients], the front of the bucket - is one small all-reduce at the end.
-        The early piece cannot hide behind the convolution backward: the K12 launches are persistent CTAs that hold every
-        SM, NCCL's CTAs only run at launch boundaries, and the final piece then waits for it.  The default is therefore the
-        single collective issued at the end.  Needs an encoder that reports when those gradients are in place
-        (BoxNatureCNN.grads_ready) and the bucket laid out in parameter order."""
-        import os
-        enc = getattr(getattr(self.model, "representation", None), "_tc", None)       # set by _PixelEncoder.set_compute("tc")
-        if self.world_size <= 1 or enc is None or not hasattr(enc, "grads_ready") or os.environ.get("XB_EARLY_ALLREDUCE", "0") != "1":
-            return
-        bucket = self.optimizer.bucket
-
-        def ready(first_param):
-            if self.world_size <= 1 or self._early is not None:
-                return
-            off = bucket.offset_of(first_param)
-            enc_ids = {id(p) for p in enc.parameters()}
-            late = {id(p) for p in (enc.fc.weight, enc.fc.bias)}
-            for p, o in zip(bucket.params, bucket.offsets):      # everything from `off` on must already be final
-                if (o >= off) != (id(p) in late or id(p) not in enc_ids):
-                    return
-            import torch.distributed as dist
-            self._early = (off, dist.all_reduce(bucket.grad[off:], op=dist.ReduceOp.SUM, async_op=True))
-        enc.grads_ready = ready
 
     def _lr_total_iters(self):
         return self.total_iters
@@ -70,9 +39,6 @@ class PPO_Learner(Learner):
         update_times = self.config.running_steps // buffer_size
         return update_times * self.config.n_epochs * self.config.n_minibatch
 
-    def _f32(self, x):
-        return torch.as_tensor(x, device=self.device).to(torch.float32).contiguous()
-
     def _gauss_ws(self, D):
         """K4G's column-partial workspace, allocated once at the size that fits any row count (D x 2048 doubles, at
         most 1 MiB): captured graphs keep the pointer they were recorded with, so it is never reallocated."""
@@ -81,7 +47,7 @@ class PPO_Learner(Learner):
             self._ws = torch.empty(need, dtype=torch.float64, device=self.device)
         return self._ws
 
-    def _device_update_gauss(self, obs, act, ret, adv, old_logp):
+    def _loss_gauss(self, obs, act, ret, adv, old_logp):
         """The Gaussian-policy branch: K4G gives (dmu, dlog_std, dvalue) and the statistics in one launch."""
         mu, log_std, v_pred = self.model.forward_raw_gauss(obs)
         mu_c, v_c = mu.contiguous(), v_pred.contiguous()
@@ -94,16 +60,16 @@ class PPO_Learner(Learner):
                   _lib.ptr(old_logp), _lib.ptr(adv), _lib.ptr(ret), B, D, B * self.world_size, float(self.clip_range),
                   float(self.vf_coef), float(self.ent_coef), self.loss_kind, _lib.ptr(dmu), _lib.ptr(dlog_std),
                   _lib.ptr(dvalue), _lib.ptr(self._stats), _lib.ptr(self._scratch), _lib.ptr(ws), ws.numel())
-        self.optimizer.zero_grad()
-        torch.autograd.backward([mu_c, v_c, log_std], [dmu, dvalue, dlog_std])
+        return [mu_c, v_c, log_std], [dmu, dvalue, dlog_std]
 
     def _device_update(self, obs, act, ret, adv, old_logp):
-        """ppo_learner.py:43-65 on the device (no host synchronisation, static shapes: CUDA-graph capturable)."""
+        """ppo_learner.py:43-65 on the device (no host synchronisation, static shapes: CUDA-graph capturable):
+        loss -> backward -> [one all-reduce of gradient + statistics] -> K7."""
+        loss = self._loss_gauss if self._gaussian else self._loss_categorical
+        self._optimizer_step(self.optimizer, *loss(obs, act, ret, adv, old_logp))
+
+    def _loss_categorical(self, obs, act, ret, adv, old_logp):
         B = act.shape[0]
-        if self._gaussian:
-            self._device_update_gauss(obs, act, ret, adv, old_logp)
-            self._reduce_and_step()
-            return
         if hasattr(self.model, "forward_raw"):
             logits, v_pred = self.model.forward_raw(obs)
         else:
@@ -118,21 +84,7 @@ class PPO_Learner(Learner):
                   _lib.ptr(adv), _lib.ptr(ret), B, A, B_total, float(self.clip_range), float(self.vf_coef),
                   float(self.ent_coef), self.loss_kind, _lib.ptr(dlogits), _lib.ptr(dvalue), _lib.ptr(self._stats),
                   _lib.ptr(self._scratch))
-        self.optimizer.zero_grad()
-        torch.autograd.backward([logits_c, v_c], [dlogits, dvalue])
-        self._reduce_and_step()
-
-    def _reduce_and_step(self):
-        """[one all-reduce of gradient + statistics] -> K7."""
-        if self.world_size > 1:
-            if self._early is not None:                      # the tail end of the bucket is already being reduced
-                off, work = self._early
-                self._early = None
-                allreduce_sum_(self.optimizer.bucket.grad_all[:self.optimizer.bucket.TAIL + off])
-                work.wait()
-            else:
-                allreduce_sum_(self.optimizer.bucket.grad_all)   # ONE collective: gradient + logged statistics
-        self.optimizer.launch(max_norm=self.grad_clip_norm if self.use_grad_clip else None)
+        return [logits_c, v_c], [dlogits, dvalue]
 
     def host_pre_step(self):
         """Host half before the device update (step counter + 16-byte hyper-parameter upload)."""
@@ -157,20 +109,20 @@ class PPO_Learner(Learner):
         self._device_update(obs, act, ret, adv, old_logp)
         self.host_post_step()
         if sync:
-            info.update(self.materialize_info())
-            info.update(self.callback.on_update_end(self.iterations, policy=self.model, info=info) or {})
+            self._finish_info(info, self._info_values(), policy=self.model)
         return info
 
     def materialize_info(self):
+        """The logged values of the last update, with the rank suffix of a distributed run."""
+        return self._with_rank(self._info_values())
+
+    def _info_values(self):
         """The single device->host read of an update: 8 floats."""
         s = self._stats.tolist()
         lr = self.optimizer.param_groups[0]['lr']
         full = dict(zip(("actor_loss", "critic_loss", "entropy", "learning_rate", "predict_value", "clip_ratio"),
                         (s[0], s[1], s[2], lr, s[3], s[4])))
-        vals = {name: full[name.replace("-", "_")] for name in self.info_names}
-        if self.distributed_training:
-            return {f"{k}/rank_{self.rank}": v for k, v in vals.items()}
-        return vals
+        return {name: full[name.replace("-", "_")] for name in self.info_names}
 
 
 class A2C_Learner(PPO_Learner):

@@ -13,7 +13,7 @@ evidently intended computation.  DESIGN.md "Reference quirks"."""
 import torch
 
 from ... import _lib
-from ..utils import FusedAdam, allreduce_sum_, CapturedStep
+from ..utils import FusedAdam, allreduce_sum_
 from ..utils.flat_bucket import cudnn_rnn_front
 from .learner import Learner
 
@@ -46,6 +46,8 @@ class _SelectFunction(torch.autograd.Function):
 
 
 class QMIX_Learner(Learner):
+    rank_suffix = False
+
     def __init__(self, config, agent_grouping, model, callback):
         super().__init__(config, model, callback)
         self.use_parameter_sharing = getattr(config, "use_parameter_sharing", True)
@@ -60,15 +62,12 @@ class QMIX_Learner(Learner):
         self.optimizer = FusedAdam(self.model.parameters_model, lr=self.learning_rate, eps=1e-5,
                                    weight_decay=getattr(config, "weight_decay", 0.0),
                                    front=cudnn_rnn_front(self.model.individual_q_networks))
-        self.scheduler = torch.optim.lr_scheduler.LinearLR(self.optimizer, start_factor=1.0,
-                                                           end_factor=self.end_factor_lr_decay,
-                                                           total_iters=self.total_iters)
+        self.scheduler = self._linear_lr(self.optimizer)
         dev = self.device
         self._filled_sum = torch.zeros(1, dtype=torch.float32, device=dev)
         self._stats = self.optimizer.bucket.tail[:2]       # logged sums ride in the gradient all-reduce (bucket tail)
         self._scratch = _lib.scratch(dev)
-        self.use_cuda_graph = getattr(config, "use_cuda_graph", False)
-        self._graphs = {}
+        self._graph_tensors = [self._filled_sum]
 
     def estimate_total_iterations(self):
         """marl_learner.py:37-47."""
@@ -83,7 +82,7 @@ class QMIX_Learner(Learner):
 
     def _stacked(self, sample):
         """[B, n, ...] device tensors from a sample dict (uses the buffer's pre-stacked tensors when present)."""
-        f32 = lambda x: torch.as_tensor(x, device=self.device).to(torch.float32).contiguous()
+        f32 = self._f32
         u8 = lambda x: torch.as_tensor(x, device=self.device).to(torch.uint8).contiguous()
         if '_stacked' in sample:
             st = sample['_stacked']
@@ -95,13 +94,6 @@ class QMIX_Learner(Learner):
         out['filled'], out['state'] = f32(sample['filled']), f32(sample['state'])
         out['avail'] = u8(stack(sample['avail_actions'])) if self.use_actions_mask else None
         return out
-
-    def _snapshot(self):
-        return (self.optimizer.snapshot(), self._filled_sum.clone())
-
-    def _restore(self, st):
-        self.optimizer.restore(st[0])
-        self._filled_sum.copy_(st[1])
 
     def _device_update(self, obs, actions, rewards, terminals, agent_mask, filled, state, avail=None):
         """qmix_learner.py:24-95 on the device (no host synchronisation, static shapes: CUDA-graph capturable)."""
@@ -124,11 +116,7 @@ class QMIX_Learner(Learner):
                   _lib.ptr(filled), _lib.ptr(self._filled_sum), B, n, T, float(self.gamma), B * T * self.world_size,
                   _lib.ptr(dq_tot),
                   _lib.ptr(self._stats), _lib.ptr(self._scratch))
-        self.optimizer.zero_grad()
-        torch.autograd.backward([q_tot_eval], [dq_tot])
-        if self.world_size > 1:
-            allreduce_sum_(self.optimizer.bucket.grad_all)   # gradient + logged statistics in one collective
-        self.optimizer.launch(max_norm=self.grad_clip_norm if self.use_grad_clip else None)
+        self._optimizer_step(self.optimizer, [q_tot_eval], [dq_tot])
         return None
 
     def update(self, sample, sync=True):
@@ -139,20 +127,15 @@ class QMIX_Learner(Learner):
         if d['avail'] is not None:
             args.append(d['avail'])
         self.optimizer.prepare()
-        if self.use_cuda_graph:        # the two collectives (sum(filled), gradient bucket) capture into the graph
-            key = tuple(d['obs'].shape)
-            if key not in self._graphs:
-                self._graphs[key] = CapturedStep(self._device_update, args, self._snapshot, self._restore)
-            self._graphs[key](*args)
-        else:
-            self._device_update(*args)
+        # the two collectives (sum(filled), gradient bucket) capture into the graph
+        self._device_step(tuple(d['obs'].shape), self._device_update, *args)
         if self.scheduler is not None:
             self.scheduler.step()
         if sync:
             s = self._stats.tolist()
-            info.update({"learning_rate": self.optimizer.param_groups[0]['lr'], "loss_Q": s[0], "predictQ": s[1]})
+            vals = {"learning_rate": self.optimizer.param_groups[0]['lr'], "loss_Q": s[0], "predictQ": s[1]}
         if self.iterations % self.sync_frequency == 0:
             self.model.copy_target()
         if sync:
-            info.update(self.callback.on_update_end(self.iterations, model=self.model, info=info) or {})
+            self._finish_info(info, vals, model=self.model)
         return info

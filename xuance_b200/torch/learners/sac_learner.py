@@ -3,76 +3,130 @@
 Same three optimiser steps in the same order (actor, critic, alpha), the same LinearLR schedules, soft target
 update and info keys.  The elementwise loss stages and their backward seeds are the K8 kernels, each optimiser is
 a flat-bucket K7 Adam (actor bucket, critic bucket, log_alpha), the Polyak update streams over the critic /
-target-critic buckets once (K7 xb_soft_update).  alpha never leaves the device."""
+target-critic buckets once (K7 xb_soft_update).  alpha never leaves the device.
+
+``_SoftActorCritic_Learner`` holds what SAC and SAC-Discrete (sacdis_learner.py) share: the optimisers, the target
+critic, the temperature state and step, ``update`` and the info dict.  ``_ActorCritic_Learner`` holds the actor / critic
+optimisers and the target buckets that DDPG and TD3 (ddpg_learner.py) share with them."""
 import numpy as np
 import torch
 import torch.nn as nn
 
 from ... import _lib
-from ..utils import FusedAdam, FlatBucket, allreduce_sum_, CapturedStep
+from ..utils import FusedAdam
+from ..utils.flat_bucket import target_bucket
 from .learner import Learner
 
 
-class SAC_Learner(Learner):
+class _ActorCritic_Learner(Learner):
+    """An actor and a critic, each with its own FusedAdam and LinearLR, and a target copy of each network named in
+    ``target_names``, held in a flat array laid out as the live network's bucket."""
+    target_names = ('critic',)
+
     def __init__(self, config, model, callback):
         super().__init__(config, model, callback)
         self.optimizer = {
             'actor': FusedAdam(self.model.actor.parameters(), self.config.learning_rate_actor),
             'critic': FusedAdam(self.model.critic.parameters(), self.config.learning_rate_critic)}
-        mk = lambda o: torch.optim.lr_scheduler.LinearLR(o, start_factor=1.0, end_factor=self.end_factor_lr_decay,
-                                                         total_iters=self.total_iters)
-        self.scheduler = {'actor': mk(self.optimizer['actor']), 'critic': mk(self.optimizer['critic'])}
-        # target critic in its own flat array, same parameter order as the critic bucket
-        self._target_bucket = FlatBucket([p.requires_grad_(True) for p in self.model.target_critic.parameters()])
-        for p in self.model.target_critic.parameters():
-            p.requires_grad_(False)
-            p.grad = None
-        assert self._target_bucket.numel == self.optimizer['critic'].bucket.numel
+        self.scheduler = {k: self._linear_lr(o) for k, o in self.optimizer.items()}
+        self._targets = {k: target_bucket(getattr(self.model, "target_" + k), self.optimizer[k].bucket)
+                         for k in self.target_names}
+        self._graph_tensors = [t.flat for t in self._targets.values()]
         self.tau, self.gamma = config.tau, config.gamma
+
+    def _soft_update(self):
+        """Polyak update of every target (actor_critic.py:155-158, 255-261, 313-319): one K7 launch per target."""
+        for k, tgt in self._targets.items():
+            live = self.optimizer[k].bucket
+            _lib.call("xb_soft_update", _lib.ptr(tgt.flat), _lib.ptr(live.flat), live.numel, float(self.tau))
+
+
+class _SoftActorCritic_Learner(_ActorCritic_Learner):
+    """Subclasses supply ``_actor_critic_steps`` (the actor step, then the critic step), ``_target_entropy`` and
+    ``_graph_key_and_args``."""
+
+    def __init__(self, config, model, callback):
+        super().__init__(config, model, callback)
         self.use_automatic_entropy_tuning = config.use_automatic_entropy_tuning
         if self.use_automatic_entropy_tuning:
-            self.target_entropy = -np.prod(model.actor.action_space.shape).item()
+            self.target_entropy = self._target_entropy()
             self.log_alpha = nn.Parameter(torch.zeros(1, requires_grad=True, device=self.device))
             self.alpha_optimizer = FusedAdam([self.log_alpha], lr=config.learning_rate_actor)
             self._alpha_buf = self.log_alpha.detach().exp()
         else:
             self._alpha_buf = torch.full((1,), float(config.alpha), device=self.device)
         self.alpha = self._alpha_buf
-        self.use_cuda_graph = getattr(config, "use_cuda_graph", False)
-        self._graphs = {}
-        dev = self.device
+        self._graph_tensors.append(self._alpha_buf)
         # the logged sums (and mean(log_pi), which the temperature step needs globally) ride in the tails of the two gradient
         # buckets: TWO collectives per update.  They cannot be one: the reference steps the actor before it evaluates the
         # critic target (sac_learner.py:53-72), so the critic gradient does not exist when the actor's must be reduced.
         self._stats_a = self.optimizer['actor'].bucket.tail[:4]
         self._stats_c = self.optimizer['critic'].bucket.tail[:2]
-        self._scratch = _lib.scratch(dev)
-        self._alpha_loss = torch.zeros(1, dtype=torch.float32, device=dev)
+        self._scratch = _lib.scratch(self.device)
+        self._alpha_loss = torch.zeros(1, dtype=torch.float32, device=self.device)
 
-    def _f32(self, x):
-        return torch.as_tensor(x, device=self.device).to(torch.float32).contiguous()
+    def _optimizers(self):
+        # the temperature optimiser is stepped with the others but, as in the reference, not checkpointed
+        return super()._optimizers() + ([self.alpha_optimizer] if self.use_automatic_entropy_tuning else [])
 
-    def _snapshot(self):
-        st = {k: v.snapshot() for k, v in self.optimizer.items()}
-        st["target"] = self._target_bucket.flat.clone()
+    def _device_update(self, *args):
+        """Everything of one update that runs on the device; no host synchronisation, static shapes."""
+        self._actor_critic_steps(*args)
+        # ---- temperature step (sac_learner.py:74-82, sacdis_learner.py:77-86): d/dlog_alpha of
+        # -mean(log_alpha * (log_pi + H_target)) = -(mean(log_pi) + H_target)
         if self.use_automatic_entropy_tuning:
-            st["alpha_opt"] = self.alpha_optimizer.snapshot()
-        st["alpha"] = self._alpha_buf.clone()
-        return st
+            g = -(self._stats_a[2:3] + self.target_entropy)      # already the global mean: summed with the actor gradient
+            self._alpha_loss.copy_(self.log_alpha.detach() * g)
+            self.alpha_optimizer.zero_grad()
+            self.alpha_optimizer.bucket.grad[:1].copy_(g)
+            self.alpha_optimizer.launch()
+            torch.exp(self.log_alpha.detach(), out=self._alpha_buf)
+        self._soft_update()
+        return None
 
-    def _restore(self, st):
-        for k, v in self.optimizer.items():
-            v.restore(st[k])
-        self._target_bucket.flat.copy_(st["target"])
+    def update(self, sync=True, **samples):
+        self.iterations += 1
+        obs, act = self._f32(samples['obs']), self._f32(samples['actions'])
+        nxt, rew, ter = self._f32(samples['obs_next']), self._f32(samples['rewards']), self._f32(samples['terminals'])
+        info = self.callback.on_update_start(self.iterations, model=self.model, obs=obs, act=act, next_obs=nxt,
+                                             rew=rew, termination=ter) or {}
+        for o in self.optimizer.values():
+            o.prepare()
         if self.use_automatic_entropy_tuning:
-            self.alpha_optimizer.restore(st["alpha_opt"])
-        self._alpha_buf.copy_(st["alpha"])
+            self.alpha_optimizer.prepare()
+        key, args = self._graph_key_and_args([obs, act, nxt, rew, ter], samples)
+        self._device_step(key, self._device_update, *args)
+        self.alpha = self._alpha_buf
+        for sch in self.scheduler.values():
+            sch.step()
+        if sync:
+            sa, sc = self._stats_a.tolist(), self._stats_c.tolist()
+            vals = {"Qloss": sc[0], "Ploss": sa[0], "Qvalue": sa[1],
+                    "actor_lr": self.optimizer['actor'].param_groups[0]['lr'],
+                    "critic_lr": self.optimizer['critic'].param_groups[0]['lr']}
+            if self.use_automatic_entropy_tuning:
+                vals.update(alpha_loss=float(self._alpha_loss), alpha=float(self._alpha_buf))
+            self._finish_info(info, vals, model=self.model)
+        return info
 
-    def _device_update(self, obs, act, nxt, rew, ter, noise_pi=None, noise_next=None):
-        """Everything of sac_learner.py:52-96 that runs on the device; no host synchronisation, static shapes."""
+
+class SAC_Learner(_SoftActorCritic_Learner):
+    def _target_entropy(self):
+        return -np.prod(self.model.actor.action_space.shape).item()
+
+    def _graph_key_and_args(self, args, samples):
+        """``noise_pi`` / ``noise_next`` (standard normal [B, act_dim]) may be supplied for reproducible tests; by default
+        the model draws them as the reference does (Normal.rsample).  With only one of them the update runs eagerly."""
+        noise_pi, noise_next = samples.get('noise_pi'), samples.get('noise_next')
+        if noise_pi is not None or noise_next is not None:
+            args = args + [noise_pi, noise_next]
+        graphed = (noise_pi is None) == (noise_next is None)
+        return ((tuple(args[0].shape), len(args)) if graphed else None), args
+
+    def _actor_critic_steps(self, obs, act, nxt, rew, ter, noise_pi=None, noise_next=None):
+        """sac_learner.py:52-72 on the device."""
         B = obs.shape[0]
         Bt = B * self.world_size
-        clip = self.grad_clip_norm if self.use_grad_clip else None
         alpha = self._alpha_buf
 
         # ---- actor step (sac_learner.py:53-60)
@@ -81,11 +135,8 @@ class SAC_Learner(Learner):
         dlp, dq1, dq2 = torch.empty_like(log_pi), torch.empty_like(q1), torch.empty_like(q2)
         _lib.call("xb_sac_actor_loss", _lib.ptr(log_pi), _lib.ptr(q1), _lib.ptr(q2), _lib.ptr(alpha), B, Bt,
                   _lib.ptr(dlp), _lib.ptr(dq1), _lib.ptr(dq2), _lib.ptr(self._stats_a), _lib.ptr(self._scratch))
-        self.optimizer['actor'].zero_grad()
-        torch.autograd.backward([log_pi, q1, q2], [dlp, dq1, dq2], inputs=self.optimizer['actor'].bucket.params)
-        if self.world_size > 1:
-            allreduce_sum_(self.optimizer['actor'].bucket.grad_all)
-        self.optimizer['actor'].launch(max_norm=clip)
+        self._optimizer_step(self.optimizer['actor'], [log_pi, q1, q2], [dlp, dq1, dq2],
+                             inputs=self.optimizer['actor'].bucket.params)
 
         # ---- critic step (:62-72)
         aq1, aq2 = self.model.Qaction(obs, act)
@@ -97,60 +148,4 @@ class SAC_Learner(Learner):
         _lib.call("xb_sac_critic_loss", _lib.ptr(aq1), _lib.ptr(aq2), _lib.ptr(target_q), _lib.ptr(log_pi_next),
                   _lib.ptr(rew), _lib.ptr(ter), _lib.ptr(alpha), float(self.gamma), B, Bt, _lib.ptr(dq1), _lib.ptr(dq2),
                   _lib.ptr(backup), _lib.ptr(self._stats_c), _lib.ptr(self._scratch))
-        self.optimizer['critic'].zero_grad()
-        torch.autograd.backward([aq1, aq2], [dq1, dq2])
-        if self.world_size > 1:
-            allreduce_sum_(self.optimizer['critic'].bucket.grad_all)
-        self.optimizer['critic'].launch(max_norm=clip)
-
-        # ---- temperature step (:74-82): d/dlog_alpha of -mean(log_alpha*(log_pi+H_target)) = -(mean(log_pi)+H_target)
-        if self.use_automatic_entropy_tuning:
-            mean_lp = self._stats_a[2:3]          # already the global mean: summed with the actor gradient
-            g = -(mean_lp + self.target_entropy)
-            self._alpha_loss.copy_(self.log_alpha.detach() * g)
-            self.alpha_optimizer.zero_grad()
-            self.alpha_optimizer.bucket.grad[:1].copy_(g)
-            self.alpha_optimizer.launch()
-            torch.exp(self.log_alpha.detach(), out=self._alpha_buf)
-
-        # ---- Polyak update of the target critic (actor_critic.py:155-158) over the two flat buckets
-        cb = self.optimizer['critic'].bucket
-        _lib.call("xb_soft_update", _lib.ptr(self._target_bucket.flat), _lib.ptr(cb.flat), cb.numel, float(self.tau))
-        return None
-
-    def update(self, sync=True, noise_pi=None, noise_next=None, **samples):
-        """``noise_pi`` / ``noise_next`` (standard normal [B, act_dim]) may be supplied for reproducible tests; by
-        default the model draws them as the reference does (Normal.rsample)."""
-        self.iterations += 1
-        obs, act = self._f32(samples['obs']), self._f32(samples['actions'])
-        nxt, rew, ter = self._f32(samples['obs_next']), self._f32(samples['rewards']), self._f32(samples['terminals'])
-        info = self.callback.on_update_start(self.iterations, model=self.model, obs=obs, act=act, next_obs=nxt,
-                                             rew=rew, termination=ter) or {}
-        for o in self.optimizer.values():
-            o.prepare()
-        if self.use_automatic_entropy_tuning:
-            self.alpha_optimizer.prepare()
-        graphed = self.use_cuda_graph and (noise_pi is None) == (noise_next is None)
-        if graphed:
-            args = [obs, act, nxt, rew, ter] + ([] if noise_pi is None else [noise_pi, noise_next])
-            key = (tuple(obs.shape), len(args))
-            if key not in self._graphs:
-                self._graphs[key] = CapturedStep(self._device_update, args, self._snapshot, self._restore)
-            self._graphs[key](*args)
-        else:
-            self._device_update(obs, act, nxt, rew, ter, noise_pi, noise_next)
-        self.alpha = self._alpha_buf
-        for sch in self.scheduler.values():
-            sch.step()
-        if sync:
-            sa, sc = self._stats_a.tolist(), self._stats_c.tolist()
-            vals = {"Qloss": sc[0], "Ploss": sa[0], "Qvalue": sa[1],
-                    "actor_lr": self.optimizer['actor'].param_groups[0]['lr'],
-                    "critic_lr": self.optimizer['critic'].param_groups[0]['lr']}
-            if self.use_automatic_entropy_tuning:
-                vals.update(alpha_loss=float(self._alpha_loss), alpha=float(self._alpha_buf))
-            if self.distributed_training:
-                vals = {f"{k}/rank_{self.rank}": v for k, v in vals.items()}
-            info.update(vals)
-            info.update(self.callback.on_update_end(self.iterations, model=self.model, info=info) or {})
-        return info
+        self._optimizer_step(self.optimizer['critic'], [aq1, aq2], [dq1, dq2])

@@ -23,8 +23,6 @@ def cudnn_rnn_front(module):
 
 class FlatBucket:
     TAIL = 32   # float32 slots BEFORE the first gradient: per-update statistics ride in the same all-reduce as the gradient
-                # (in front, so that [statistics | first parameters] stays one contiguous piece when the gradients of the
-                # LAST parameters - final first in a backward pass - are reduced early, see PPO_Learner._early_allreduce)
 
     def __init__(self, params, front=()):
         """``front``: parameters to lay out first (see ``cudnn_rnn_front``); ``self.params`` keeps the caller's order."""
@@ -68,13 +66,6 @@ class FlatBucket:
             return chunk.view(o, h, w, i).permute(0, 3, 1, 2)
         return chunk.view(p.shape)
 
-    def offset_of(self, p):
-        """Element offset of parameter ``p`` inside ``flat`` / ``grad``."""
-        for q, o in zip(self.params, self.offsets):
-            if q is p:
-                return o
-        raise KeyError("parameter is not in this bucket")
-
     def views(self, buf):
         return [self._view(buf, p, o) for p, o in zip(self.params, self.offsets)]
 
@@ -83,3 +74,16 @@ class FlatBucket:
         for p, o in zip(self.params, self.offsets):  # re-attach if someone set .grad to None
             if p.grad is None or p.grad.data_ptr() != self.grad.data_ptr() + 4 * o:
                 p.grad = self._view(self.grad, p, o)
+
+
+def target_bucket(target, live):
+    """A target network's parameters re-homed into their own flat array, in the ``live`` bucket's parameter order and
+    layout, so that one K7 ``xb_soft_update`` streams the Polyak update over the two arrays.  The target's parameters
+    stay frozen (no gradient)."""
+    params = list(target.parameters())
+    bucket = FlatBucket([p.requires_grad_(True) for p in params])
+    for p in params:
+        p.requires_grad_(False)
+        p.grad = None
+    assert bucket.numel == live.numel and bucket.offsets == live.offsets
+    return bucket

@@ -625,8 +625,6 @@ class BoxNatureCNN(TensorCoreNatureCNN):
     plane, 4 channels) and its weight gradient keep the gathered path, with the padded tensors described to it as ordinary
     geometries."""
 
-    grads_ready = None      # optional callable(first_final_parameter), see backward()
-
     def _box_ok(self):
         cs = self.convs
         if len(cs) != 3:
@@ -816,10 +814,6 @@ class BoxNatureCNN(TensorCoreNatureCNN):
                 self.fc.bias.grad.add_(dbfc)
                 dbfc = self.fc.bias.grad
             gfc = [ret(self.fc.weight, dwfc), ret(self.fc.bias, dbfc)]
-            if self.grads_ready is not None and gfc[0] is None and gfc[1] is None:
-                # the Linear layer's gradients (and those of everything after the encoder) are final and in place while the
-                # whole convolution backward is still ahead: a sharded learner starts reducing them now
-                self.grads_ready(self.fc.weight)
             # the Linear layer's data gradient lands straight in conv3's PADDED output-gradient tensor: image b's 6400 values
             # are rows 1 .. H2 of its hp2 rows (a matrix with hp2*W2*N3 elements per row, from column W2*N3); the mask is
             # the plain [B, 6400] activation; the column sums per (h, w, c) are conv3's bias-gradient partials
