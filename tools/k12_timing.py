@@ -62,7 +62,7 @@ def roles():
     sp = tc.wgrad_box_splits(B * P["hp2"], 6, 576, 64)
     report("conv3 weight gradient (box)", lambda: tc.wgrad_box(act2, g3, P["fwd3"], 6, sp))
     report("conv2 weight gradient (gathered)", lambda: enc.be.wgrad(act1, g3.view(Pn, -1, 64), P["wg2"], 64, 32, 4, 4))
-    report("conv1 weight gradient (gathered)", lambda: enc.be.wgrad(x, g1, P["wg1"], 32, 4, 8, 8))
+    report("conv1 weight gradient (TMA windows)", lambda: enc.be.wgrad(x, g1, P["wg1"], 32, 4, 8, 8))
     # the Linear layer 6400 -> 512
     xf, wf = rnd(Pn, B, 6400), rnd(Pn, 512, 6400)
     yf = torch.empty(Pn, B, 512, dtype=torch.bfloat16, device=DEV)

@@ -199,6 +199,37 @@ XB_HD void xb_stage_wgrad(const XbConvGeom &g, const XbUnit *tab, int pt, int64_
         emit_g(xb_canon_off_mn(j * 8, pp, XB_CONV_KC), in_run ? site * g_ld + g_c0 + j * 8 : (int64_t)-1);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Weight gradient from input WINDOWS (conv_tc.cu, conv_tc_kernel_wgrad_win): one A plane, C == 8 (one 16-byte unit per
+// tap), the taps the full KH x KW rectangle in row-major order.  A chunk of 64 consecutive sites touches at most
+// xb_win_rows grid rows R = b * OY + y (all images in one sequence), starting at R0 = chunk_site0 / OX; window slot j holds
+// the KH input rows sy * y + dy[0] .. + KH - 1 of grid row R0 + j, units dx[0] .. dx[0] + win_w - 1 of each, as TMA wrote
+// them (one box per slot, zero outside the input and for grid rows past the last image).  Row (site s, k unit t) of the
+// MN-major A operand is then the 16 bytes at  xb_win_site_off(s) + xb_win_tap_off(t)  of the window: the consumers read
+// their ldmatrix rows from there, where the gathered path stages them with xb_stage_wgrad.
+// ---------------------------------------------------------------------------------------------------------------------
+// units per window row: every tap of every site of a grid row
+XB_HD int xb_win_width(const XbConvGeom &g) { return g.sx * (g.OX - 1) + (g.dx[g.T - 1] - g.dx[0]) + 1; }
+// grid rows one chunk of XB_CONV_KC consecutive sites can touch
+XB_HD int xb_win_rows(const XbConvGeom &g) { return (XB_CONV_KC - 2 + g.OX) / g.OX + 1; }
+// first input row and image of window slot R (grid row R; b >= B past the last image)
+XB_HD void xb_win_box(const XbConvGeom &g, int64_t R, int &b, int &iy0) {
+    int y, x;
+    xb_conv_site(g, R * g.OX, b, y, x);
+    iy0 = y * g.sy + g.dy[0];
+}
+// byte offset of tap unit kcol / 8 within a window slot (rows kcol >= K, which no output keeps, read tap 0)
+XB_HD uint32_t xb_win_tap_off(const XbConvGeom &g, int kcol, int win_w) {
+    const int t = kcol < g.T * g.C ? kcol / g.C : 0;
+    return (uint32_t)(((g.dy[t] - g.dy[0]) * win_w + (g.dx[t] - g.dx[0])) * 16);
+}
+// byte offset of site s's slot and first unit within the window of the chunk whose first grid row is R0
+XB_HD uint32_t xb_win_site_off(const XbConvGeom &g, int64_t s, int64_t R0, uint32_t slot_bytes) {
+    int b, y, x;
+    xb_conv_site(g, s, b, y, x);
+    return (uint32_t)((int64_t)b * g.OY + y - R0) * slot_bytes + (uint32_t)(x * g.sx * 16);
+}
+
 // shared-memory bytes of one pipeline stage: the P planes of A (hi | [mid |] lo) followed by the P planes of W.
 // P = 2: x = hi + lo (|err| <= 2^-16 |x|, 3 products);  P = 3: x = hi + mid + lo (<= 2^-24 |x|, 6 products)
 XB_HD uint32_t xb_conv_stage_bytes(int N, int P = 2) {

@@ -109,6 +109,9 @@ struct ConvParams {
     // weight gradient: sites are cut into `splits` runs of sites_per_split (a multiple of KC)
     int splits;
     int64_t sites_per_split;
+    // conv_tc_kernel_wgrad_win: window slots per chunk, slot pitch in bytes, KH input rows and win_w units per slot
+    int win_rows, win_kh, win_w;
+    uint32_t win_slot;
 };
 
 // 16-byte cp.async with zero-fill.  CA = through L1 (sector sharing between the lanes of a request and reuse of the
@@ -629,6 +632,158 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel(const __grid_consta
     }
 }
 
+// The weight gradient of a raw-pixel first layer (one A plane, C = 8, a full tap rectangle, N = 32, K <= 256; selected by
+// xb_wgrad_gather_tc) with both operands by TMA: work item = one split, ALL K rows, so every site's patches and output
+// gradient are loaded once instead of once per 128-row tile.  Per chunk of 64 sites one elected producer thread loads
+//   * the output gradient: one box {32 columns, 64 sites, PB planes}, 64-byte swizzle ([plane][site][64 B]);
+//   * the input window: win_rows boxes of KH rows x win_w 16-byte units (conv_index.h, xb_win_*), no swizzle;
+// and the consumer warps read their MN-major A fragments with ldmatrix.trans straight from the window (the 16 bytes of a
+// fragment row are one tap unit of one site).  Warpgroup wg owns the m64 row blocks wg and wg + 2 (rows 128 r + 64 wg ..),
+// the rows of the gathered path's tile r, and issues per K step and row block the same n32 wgmmas on the same fragments,
+// B planes and accumulators in the same order, so the partials are bit for bit those of conv_tc_kernel<true, 1, PB, 1>.
+template <int PB>
+__global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel_wgrad_win(const __grid_constant__ ConvParams p) {
+    constexpr int RB = 2;                                    // m64 row blocks per consumer warpgroup
+    constexpr uint32_t G_BYTES = PB * 32 * XB_CONV_KC * 2;   // output-gradient box: 4096 B per plane
+    extern __shared__ __align__(1024) uint8_t smem[];
+    __shared__ __align__(8) uint64_t full_bar[MAX_STAGES], empty_bar[MAX_STAGES];
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const XbConvGeom &g = p.g;
+    const int K = g.T * g.C, S = p.stages;
+    const uint32_t stage_bytes = (G_BYTES + (uint32_t)p.win_rows * p.win_slot + 1023u) & ~1023u;   // as wgrad_win_setup
+    auto chunks_of = [&](int64_t sp) -> int {
+        const int64_t s0 = sp * p.sites_per_split, cnt = (p.M - s0) < p.sites_per_split ? (p.M - s0) : p.sites_per_split;
+        return (int)((cnt + KC - 1) / KC);
+    };
+    if (tid == 0) {
+        for (int s = 0; s < S; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], CONS_WARPS);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+    const uint32_t smem_base = smem_u32(smem);
+    uint32_t t_wait[5] = {0, 0, 0, 0, 0};                   // role timing, slots as in conv_tc_kernel
+    if (p.timing && blockIdx.x < 160 && (tid == 0 || tid == CONS_WARPS * 32)) xb_k12_timing[blockIdx.x][tid == 0 ? 0 : 4] = clock64();
+    auto timed_wait = [&](uint64_t *bar, uint32_t parity, int slot) {
+        if (p.timing) {
+            const uint32_t t0 = clock32();
+            mbar_wait(bar, parity);
+            t_wait[slot] += clock32() - t0;
+        } else {
+            mbar_wait(bar, parity);
+        }
+    };
+
+    if (warp >= CONS_WARPS) {
+        // ------------------------------------------------------------------ producer: one thread issues every copy
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PROD_REGS));
+        if (tid == CONS_WARPS * 32) {
+            const uint32_t bytes = G_BYTES + (uint32_t)(p.win_rows * p.win_kh * p.win_w * 16);
+            uint32_t it = 0;
+            for (int64_t sp = blockIdx.x; sp < p.splits; sp += gridDim.x) {
+                const int n_chunks = chunks_of(sp);
+                for (int kc = 0; kc < n_chunks; ++kc, ++it) {
+                    const int stage = (int)(it % (uint32_t)S);
+                    timed_wait(&empty_bar[stage], ((it / (uint32_t)S) & 1u) ^ 1u, 0);
+                    const uint32_t base = smem_base + (uint32_t)stage * stage_bytes;
+                    const int64_t site0 = sp * p.sites_per_split + (int64_t)kc * KC;
+                    mbar_expect_tx(&full_bar[stage], bytes);
+                    tma_load_3d(base, &p.tm_b, 0, (int)site0, 0, &full_bar[stage]);            // G[site, n], sites >= M zero
+                    const int64_t R0 = xb_div((uint32_t)site0, g.div_ox);      // first grid row of the chunk
+                    for (int j = 0; j < p.win_rows; ++j) {
+                        int b, iy0;
+                        xb_win_box(g, R0 + j, b, iy0);
+                        // 8-byte elements: unit u is elements 2u, 2u + 1
+                        tma_load_3d(base + G_BYTES + (uint32_t)j * p.win_slot, &p.tm_a, 2 * g.dx[0], iy0, b, &full_bar[stage]);
+                    }
+                }
+            }
+        }
+    } else {
+        // ------------------------------------------------------------------ consumers: wgmma issue + epilogue
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONS_REGS));
+        const int wg = warp >> 2;
+        // B: MN-major, 64-byte swizzle, 8-site groups of 512 B (SBO), K step of 16 sites = 1024 B, planes 4096 B apart
+        const uint64_t b_tmpl = make_desc_sw64(0, 0, 512);
+        // this lane's ldmatrix row (see conv_tc_kernel): k row = site 8 (mi >> 1) + lr of the K step, m rows = the 8 K-unit
+        // columns from m_l of the warp's 16 x 16 fragment
+        const int mi = lane >> 3, lr = lane & 7, m_l = 16 * (warp & 3) + 8 * (mi & 1);
+        uint32_t tap_off[RB];
+#pragma unroll
+        for (int r = 0; r < RB; ++r) tap_off[r] = xb_win_tap_off(g, 128 * r + 64 * wg + m_l, p.win_w);
+        const int rbase = 64 * wg + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+        float acc[RB][PB][16];
+        uint32_t it = 0;
+        for (int64_t sp = blockIdx.x; sp < p.splits; sp += gridDim.x) {
+            const int n_chunks = chunks_of(sp);
+            uint32_t scale_d = 0;
+            uint32_t af[KC / 16][RB][4];
+            for (int kc = 0; kc < n_chunks; ++kc, ++it) {
+                const int stage = (int)(it % (uint32_t)S);
+                const uint32_t base = smem_base + (uint32_t)stage * stage_bytes;
+                const int64_t site0 = sp * p.sites_per_split + (int64_t)kc * KC;
+                const int64_t R0 = xb_div((uint32_t)site0, g.div_ox);      // first grid row of the chunk
+                uint32_t site_off[KC / 16];
+#pragma unroll
+                for (int ks = 0; ks < KC / 16; ++ks) site_off[ks] = xb_win_site_off(g, site0 + 16 * ks + 8 * (mi >> 1) + lr, R0, p.win_slot);
+                timed_wait(&full_bar[stage], (it / (uint32_t)S) & 1u, 0);
+                const uint32_t win = base + G_BYTES;
+                // every fragment of the chunk is loaded while no wgmma is in flight (see conv_tc_kernel)
+#pragma unroll
+                for (int ks = 0; ks < KC / 16; ++ks)
+#pragma unroll
+                    for (int r = 0; r < RB; ++r) ldmatrix_x4<1>(af[ks][r], win + site_off[ks] + tap_off[r]);
+                wgmma_fence();
+                const uint64_t b0 = b_tmpl + (uint64_t)(base >> 4);
+#pragma unroll
+                for (int ks = 0; ks < KC / 16; ++ks) {
+#pragma unroll
+                    for (int r = 0; r < RB; ++r)
+#pragma unroll
+                        for (int q = 0; q < PB; ++q)
+                            wgmma_rs_n32<1>(acc[r][q], af[ks][r], b0 + (uint64_t)((ks * 1024 + q * 4096) >> 4), scale_d);
+                    scale_d = 1;
+                }
+                wgmma_commit();
+                timed_wgmma_wait<0>(p.timing, t_wait[3]);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[stage]);
+            }
+            const uint32_t t_epi = p.timing ? clock32() : 0u;
+            // ---- epilogue: partials [splits, K, 32], rows 128 r + rbase (+ 8), accumulator groups added smallest first
+#pragma unroll
+            for (int r = 0; r < RB; ++r)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int kcol = 128 * r + rbase + 8 * h;
+                    if (kcol >= K) continue;
+                    float *row = p.out_f32 + (sp * K + kcol) * 32;
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        float v[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            v[e] = acc[r][PB - 1][4 * i + 2 * h + e];
+#pragma unroll
+                            for (int gq = PB - 2; gq >= 0; --gq) v[e] += acc[r][gq][4 * i + 2 * h + e];
+                        }
+                        *reinterpret_cast<float2 *>(row + 8 * i + cq) = make_float2(v[0], v[1]);
+                    }
+                }
+            if (p.timing) t_wait[4] += clock32() - t_epi;
+        }
+    }
+    if (p.timing && blockIdx.x < 160) {
+        const unsigned long long now = clock64();
+        unsigned long long *o = xb_k12_timing[blockIdx.x];
+        if (tid == 0) o[0] = now - o[0], o[1] = t_wait[0], o[2] = t_wait[3], o[3] = 0, o[7] = t_wait[4];
+        if (tid == CONS_WARPS * 32) o[4] = now - o[4], o[5] = t_wait[0], o[6] = 0;
+    }
+}
+
 // weight-gradient finish: sum the split partials [splits, K, N] in a fixed order and scatter to torch's [N, C, KH, KW]
 // (column k = (kh, kw, c) of the packed layout -> xb_pack_weight_src); accumulate != 0 adds to dw (autograd .grad).
 // A block owns E = 256 / lanes consecutive (k, n) elements - coalesced rows of the partial matrices - and `lanes` threads
@@ -862,16 +1017,31 @@ bool tma_enabled() {
 // bf16 tensor [planes][rows][cols] (cols contiguous, row_stride / plane_stride in elements), tiles {64 cols, box_rows, planes},
 // 128-byte swizzle, zero fill outside [rows, cols]
 bool make_tmap(CUtensorMap *tm, const void *base, int64_t cols, int64_t rows, int planes, int64_t row_stride,
-               int64_t plane_stride, int box_rows) {
+               int64_t plane_stride, int box_rows, int box_cols = 64, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
     EncodeTiledFn enc = encode_tiled_fn();
     if (!enc) return false;
     if (((uintptr_t)base & 15) || (row_stride * 2) % 16 || (plane_stride * 2) % 16 || box_rows > 256) return false;
     const cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)planes};
     const cuuint64_t strides[2] = {(cuuint64_t)row_stride * 2, (cuuint64_t)(planes > 1 ? plane_stride : row_stride * rows) * 2};
-    const cuuint32_t box[3] = {64, (cuuint32_t)box_rows, (cuuint32_t)planes};
+    const cuuint32_t box[3] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows, (cuuint32_t)planes};
     const cuuint32_t estr[3] = {1, 1, 1};
     return enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(base), dims, strides, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// input windows of conv_tc_kernel_wgrad_win: the [B, IH, IW, 8] bf16 plane as [B][IH][2 IW] 8-byte elements (a box row of
+// 16-byte units would exceed the 256-element box limit as bf16), boxes of {2 win_w elements, KH rows, one image}, no swizzle,
+// zero fill outside the input
+bool make_tmap_win(CUtensorMap *tm, const void *base, int B, int IH, int IW, int win_w, int KH) {
+    EncodeTiledFn enc = encode_tiled_fn();
+    if (!enc || ((uintptr_t)base & 15)) return false;
+    const cuuint64_t dims[3] = {(cuuint64_t)IW * 2, (cuuint64_t)IH, (cuuint64_t)B};
+    const cuuint64_t strides[2] = {(cuuint64_t)IW * 16, (cuuint64_t)IH * IW * 16};
+    const cuuint32_t box[3] = {(cuuint32_t)win_w * 2, (cuuint32_t)KH, 1};
+    const cuuint32_t estr[3] = {1, 1, 1};
+    return enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT64, 3, const_cast<void *>(base), dims, strides, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
@@ -965,6 +1135,43 @@ int launch(int pa, int pb, const ConvParams &p, int64_t work, void *stream) {
     if (pa == 2 && pb == 3) return launch_n<WGRAD, 2, 3>(p, work, stream);
     if (pa == 3 && pb == 3) return launch_n<WGRAD, 3, 3>(p, work, stream);
     return XB_EINVAL;
+}
+
+// conv_tc_kernel_wgrad_win takes a weight gradient whose A operand is one plane of 16-byte units (C = 8) read through a full
+// KH x KW tap rectangle in row-major order, with N = n_tile = 32 and 64 <= K <= 256 (two m64 row blocks per consumer
+// warpgroup) - conv1 over raw pixels, 4 channels folded in pixel pairs.  Fills the window fields and the ring of p.
+bool wgrad_win_setup(ConvParams &p, int planes_a, int planes_b, int N, int n_tile) {
+    const XbConvGeom &g = p.g;
+    if (planes_a != 1 || g.C != 8 || N != 32 || n_tile != 32 || g.T % 8 != 0 || g.T * g.C > 2 * TILE_M) return false;
+    int KW = 1;
+    while (KW < g.T && g.dy[KW] == g.dy[0]) ++KW;
+    if (g.T % KW != 0) return false;
+    for (int t = 0; t < g.T; ++t)
+        if (g.dy[t] != g.dy[0] + t / KW || g.dx[t] != g.dx[0] + t % KW) return false;
+    const int KH = g.T / KW, win_w = xb_win_width(g);
+    if (2 * win_w > 256 || KH > 256 || p.M + KC >= ((int64_t)1 << 31)) return false;      // box limits, 32-bit site indices
+    p.win_kh = KH, p.win_w = win_w, p.win_rows = xb_win_rows(g);
+    p.win_slot = ((uint32_t)(KH * win_w * 16) + 127u) & ~127u;             // TMA destinations 128-byte aligned
+    // stage: the output-gradient box (4096 B per plane) + the window slots, 1024-byte aligned (the 64-byte swizzle
+    // pattern of the box repeats every 512 B of absolute address)
+    const uint32_t stage_bytes = ((uint32_t)planes_b * 4096u + (uint32_t)p.win_rows * p.win_slot + 1023u) & ~1023u;
+    int stages = (int)((uint32_t)XB_K12_MAX_DYN_SMEM / stage_bytes);
+    if (stages < 2) return false;
+    p.stages = stages > MAX_STAGES ? MAX_STAGES : stages;
+    p.dyn_smem = (uint32_t)p.stages * stage_bytes;
+    return true;
+}
+
+template <int PB>
+int launch_win(const ConvParams &p, void *stream) {
+    static bool attr = false;
+    if (!attr) {
+        cudaFuncSetAttribute(conv_tc_kernel_wgrad_win<PB>, cudaFuncAttributeMaxDynamicSharedMemorySize, XB_K12_MAX_DYN_SMEM);
+        attr = true;
+    }
+    const int grid = p.splits < xb_sm_count() ? p.splits : xb_sm_count();
+    conv_tc_kernel_wgrad_win<PB><<<grid, THREADS, p.dyn_smem, (cudaStream_t)stream>>>(p);
+    return xb_launch_status();
 }
 
 }  // namespace
@@ -1220,6 +1427,15 @@ extern "C" int xb_wgrad_gather_tc(int planes_a, int planes_b, const void *in, in
     const int64_t per = xb_wgrad_sites_per_split(p.M, splits);
     if (per == 0) return XB_EINVAL;     // too many splits for this many sites
     p.splits = splits, p.sites_per_split = per;
+    if (tma_enabled() && wgrad_win_setup(p, planes_a, planes_b, N, n_tile)) {
+        // both operands by TMA, one work item per split (conv_tc_kernel_wgrad_win)
+        if (!make_tmap_win(&p.tm_a, in, B, IH, IW, p.win_w, p.win_kh) ||
+            !make_tmap(&p.tm_b, g, N, p.M, planes_b, g_ld, g_plane, KC, 32, CU_TENSOR_MAP_SWIZZLE_64B))
+            return XB_EINVAL;
+        if (planes_b == 1) return launch_win<1>(p, stream);
+        if (planes_b == 2) return launch_win<2>(p, stream);
+        return launch_win<3>(p, stream);
+    }
     if (tma_enabled()) {
         // output gradient [planes_b][sites][g_ld]: tiles of {64 columns, 64 sites, all planes} (one 64-column block per plane)
         if (n_tile == 64) p.b_tma = make_tmap(&p.tm_b, g, N, p.M, planes_b, g_ld, g_plane, KC) ? 1 : 0;

@@ -43,6 +43,11 @@ __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr, uint32_t
     return d;
 }
 
+// 64-byte-swizzle descriptor (layout type 2, the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_64B)
+__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+    return (make_desc_sw128(smem_addr, lbo_bytes, sbo_bytes) & ~((uint64_t)3 << 62)) | ((uint64_t)2 << 62);
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
