@@ -442,7 +442,9 @@ int xb_rms_update_normalize(const float *x, int N, int64_t D, float *mean, float
  *                       (128 columns of (t,c), n_tile columns, split).  partials: float32 [splits, T*C, N].  One A plane
  *                       with C = 8, a full tap rectangle in row-major order, N = n_tile = 32 and T*C <= 256 (conv1 over raw
  *                       pixels) runs from TMA input windows instead, one work item per split, with the same partials bit
- *                       for bit; XB_K12_TMA=0 keeps the gathered path.
+ *                       for bit; XB_K12_TMA=0 keeps the gathered path.  So does three planes on each side with C = 32 read
+ *                       as pixel pairs (a KH x 4 tap rectangle in row-major order, even sx and dx[0], even IW), N = n_tile
+ *                       = 64 (conv2 over act1): TMA pair windows, one box per grid row, image and K tile.
  * xb_wgrad_reduce     : dw[N, C, KH, KW] (torch layout) (+)= scale * sum_s partials[s, (kh,kw,c), n], splits added in a fixed
  *                       order; `partials` is scratch: with more than 256 splits groups of rows are folded in place first. */
 int xb_split_bf16(const float *x, int64_t n, int planes, void *out /* bf16 [planes, n] */, void *stream);

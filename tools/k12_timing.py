@@ -61,7 +61,7 @@ def roles():
     report("conv2 data gradient (halo)", lambda: tc.gemm_halo(g3, wd2, P["h_dg2"], out_pl=d1, out_ld=32, relu_mask=act1[0]))
     sp = tc.wgrad_box_splits(B * P["hp2"], 6, 576, 64)
     report("conv3 weight gradient (box)", lambda: tc.wgrad_box(act2, g3, P["fwd3"], 6, sp))
-    report("conv2 weight gradient (gathered)", lambda: enc.be.wgrad(act1, g3.view(Pn, -1, 64), P["wg2"], 64, 32, 4, 4))
+    report("conv2 weight gradient (TMA pairs)", lambda: enc.be.wgrad(act1, g3.view(Pn, -1, 64), P["wg2"], 64, 32, 4, 4))
     report("conv1 weight gradient (TMA windows)", lambda: enc.be.wgrad(x, g1, P["wg1"], 32, 4, 8, 8))
     # the Linear layer 6400 -> 512
     xf, wf = rnd(Pn, B, 6400), rnd(Pn, 512, 6400)

@@ -230,6 +230,41 @@ XB_HD uint32_t xb_win_site_off(const XbConvGeom &g, int64_t s, int64_t R0, uint3
     return (uint32_t)((int64_t)b * g.OY + y - R0) * slot_bytes + (uint32_t)(x * g.sx * 16);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Weight gradient from PIXEL-PAIR windows (conv_tc.cu, conv_tc_kernel_wgrad_pairs): C == 32 input channels read as
+// 64-channel pixel pairs (128 bytes), the taps the full KH x 4 rectangle in row-major order, sx and dx[0] even.  A 128-row
+// K tile mt is then tap row mt: rows (kw, c), kw = 0, 1 in pair x * sx / 2 + dx[0] / 2 and kw = 2, 3 in the next pair.
+// Window slot j of a chunk holds input row sy * y + dy[KW * mt] of grid row R0 + j (all images in one sequence), pairs
+// dx[0] / 2 .. + xb_pwin_width - 1, every plane: [plane][pair][128 B] with TMA's 128-byte swizzle, one box per slot from a
+// tensor map with one dimension per image (zero fill for the rows an image does not have and past the last image).
+// The 16 bytes of row (site s, K rows kcol .. kcol + 7) of plane q of the MN-major A operand are at
+//   xb_sw128(window + xb_pwin_site_off(s) + xb_pwin_tap_off(kcol) + q * xb_pwin_width * 128)
+// where the gathered path stages them with xb_stage_wgrad.
+// ---------------------------------------------------------------------------------------------------------------------
+#define XB_PWIN_KW 4            // taps per tap row: 4 x 32 channels = one 128-row K tile
+// pairs per window row: every tap of every site of a grid row
+XB_HD int xb_pwin_width(const XbConvGeom &g) { return (g.sx * (g.OX - 1) + g.dx[XB_PWIN_KW - 1] - g.dx[0]) / 2 + 1; }
+// input row of window slot R (grid row R) for K tile mt, and its image (b >= B past the last image)
+XB_HD void xb_pwin_box(const XbConvGeom &g, int64_t R, int mt, int &b, int &iy) {
+    int y, x;
+    xb_conv_site(g, R * g.OX, b, y, x);
+    iy = y * g.sy + g.dy[XB_PWIN_KW * mt];
+}
+// byte offset of K rows kcol .. kcol + 7 (one tap, 8 channels) within a pair row, pairs counted from the site's first
+// (kcol within the 128-row tile: taps 0, 1 in the first pair, 2, 3 in the second)
+XB_HD uint32_t xb_pwin_tap_off(const XbConvGeom &g, int kcol) {
+    const int kw = kcol / g.C, d = g.dx[kw] - g.dx[0];
+    return (uint32_t)((d >> 1) * 128 + ((d & 1) * g.C + kcol % g.C) * 2);
+}
+// byte offset of site s's slot and pair within the window of the chunk whose first grid row is R0
+XB_HD uint32_t xb_pwin_site_off(const XbConvGeom &g, int64_t s, int64_t R0, uint32_t slot_bytes) {
+    int b, y, x;
+    xb_conv_site(g, s, b, y, x);
+    return (uint32_t)((int64_t)b * g.OY + y - R0) * slot_bytes + (uint32_t)(x * (g.sx / 2) * 128);
+}
+// the 128-byte swizzle as TMA applies it: the 16-byte unit (bits 4-6) XOR bits 7-9 of the shared-memory address
+XB_HD uint32_t xb_sw128(uint32_t a) { return a ^ (((a >> 7) & 7u) << 4); }
+
 // shared-memory bytes of one pipeline stage: the P planes of A (hi | [mid |] lo) followed by the P planes of W.
 // P = 2: x = hi + lo (|err| <= 2^-16 |x|, 3 products);  P = 3: x = hi + mid + lo (<= 2^-24 |x|, 6 products)
 XB_HD uint32_t xb_conv_stage_bytes(int N, int P = 2) {

@@ -109,7 +109,8 @@ struct ConvParams {
     // weight gradient: sites are cut into `splits` runs of sites_per_split (a multiple of KC)
     int splits;
     int64_t sites_per_split;
-    // conv_tc_kernel_wgrad_win: window slots per chunk, slot pitch in bytes, KH input rows and win_w units per slot
+    // conv_tc_kernel_wgrad_win: window slots per chunk, slot pitch in bytes, KH input rows and win_w units per slot;
+    // conv_tc_kernel_wgrad_pairs: the same with one input row and win_w pixel pairs per slot and plane
     int win_rows, win_kh, win_w;
     uint32_t win_slot;
 };
@@ -139,6 +140,13 @@ __device__ __forceinline__ void tma_load_box(uint32_t dst, const CUtensorMap *tm
     asm volatile(
         "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
         ::"r"(dst), "l"(tm), "r"(c), "r"(w), "r"(ph), "r"(idx), "r"(plane), "r"(smem_u32(bar))
+        : "memory");
+}
+// TMA: one 5-D box at coordinates {c0 .. c4} -> shared memory, completion bytes on an mbarrier
+__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap *tm, int c0, int c1, int c2, int c3, int c4, uint64_t *bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
+        ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "r"(smem_u32(bar))
         : "memory");
 }
 template <int N>
@@ -784,6 +792,162 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel_wgrad_win(const __g
     }
 }
 
+// The weight gradient of a stride-2 layer over a 32-channel activation read as pixel pairs (three planes each side, C = 32,
+// a KH x 4 tap rectangle, N = n_tile = 64; selected by xb_wgrad_gather_tc) with both operands by TMA.  Work items, chunks
+// and wgmmas are the gathered path's: item = (split, 128-row K tile mt) split-major, so the K tiles of a split run on
+// neighbouring CTAs at the same time and share their loads in L2.  Per chunk of 64 sites one elected producer thread loads
+//   * the output gradient: one box {64 columns, 64 sites, 3 planes}, 128-byte swizzle (the gathered path's b_tma box);
+//   * the input window: win_rows boxes {64 channels, win_w pairs, input row sy * y + dy[4 mt] of image b, 3 planes}, 128-byte
+//     swizzle, one per grid row (b, y) the chunk can touch (conv_index.h, xb_pwin_*);
+// and the consumer warps read their MN-major A fragments with ldmatrix.trans straight from the window (a fragment row is 8
+// channels of one site and pair; 8 consecutive sites are 8 consecutive 128-byte pair rows, which the swizzle spreads over
+// all banks).  Each warpgroup issues the gathered path's n64 wgmmas on the same fragments, B planes and accumulators in
+// the same order, so the partials are bit for bit those of conv_tc_kernel<true, 3, 3, 2>.
+__global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel_wgrad_pairs(const __grid_constant__ ConvParams p) {
+    constexpr int PA = 3, PB = 3, NC = 2, N = 32 * NC;
+    constexpr uint32_t G_BYTES = PB * N * KC * 2;            // output-gradient box: 8192 B per plane
+    extern __shared__ __align__(1024) uint8_t smem[];
+    __shared__ __align__(8) uint64_t full_bar[MAX_STAGES], empty_bar[MAX_STAGES];
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const XbConvGeom &g = p.g;
+    const int K = g.T * g.C, S = p.stages, m_tiles = K / TILE_M;
+    const int64_t n_work = (int64_t)p.splits * m_tiles;
+    const uint32_t stage_bytes = G_BYTES + (uint32_t)p.win_rows * p.win_slot;     // as wgrad_pairs_setup
+    const uint32_t pair_plane = (uint32_t)p.win_w * 128u;                          // one plane of a window slot
+    auto chunks_of = [&](int64_t sp) -> int {
+        const int64_t s0 = sp * p.sites_per_split, cnt = (p.M - s0) < p.sites_per_split ? (p.M - s0) : p.sites_per_split;
+        return (int)((cnt + KC - 1) / KC);
+    };
+    if (tid == 0) {
+        for (int s = 0; s < S; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], CONS_WARPS);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+    const uint32_t smem_base = smem_u32(smem);
+    if (smem_base & 1023u) __trap();                         // the 128-byte swizzle pattern repeats every 1024 B
+    uint32_t t_wait[5] = {0, 0, 0, 0, 0};                   // role timing, slots as in conv_tc_kernel
+    if (p.timing && blockIdx.x < 160 && (tid == 0 || tid == CONS_WARPS * 32)) xb_k12_timing[blockIdx.x][tid == 0 ? 0 : 4] = clock64();
+    auto timed_wait = [&](uint64_t *bar, uint32_t parity, int slot) {
+        if (p.timing) {
+            const uint32_t t0 = clock32();
+            mbar_wait(bar, parity);
+            t_wait[slot] += clock32() - t0;
+        } else {
+            mbar_wait(bar, parity);
+        }
+    };
+
+    if (warp >= CONS_WARPS) {
+        // ------------------------------------------------------------------ producer: one thread issues every copy
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PROD_REGS));
+        if (tid == CONS_WARPS * 32) {
+            const uint32_t bytes = G_BYTES + (uint32_t)p.win_rows * (uint32_t)PA * pair_plane;
+            const int p0 = g.dx[0] / 2;                      // first pair of a window row (dx[0] even)
+            uint32_t it = 0;
+            for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
+                const int64_t sp = w / m_tiles;
+                const int mt = (int)(w - sp * m_tiles);
+                const int n_chunks = chunks_of(sp);
+                for (int kc = 0; kc < n_chunks; ++kc, ++it) {
+                    const int stage = (int)(it % (uint32_t)S);
+                    timed_wait(&empty_bar[stage], ((it / (uint32_t)S) & 1u) ^ 1u, 0);
+                    const uint32_t base = smem_base + (uint32_t)stage * stage_bytes;
+                    const int64_t site0 = sp * p.sites_per_split + (int64_t)kc * KC;
+                    mbar_expect_tx(&full_bar[stage], bytes);
+                    tma_load_3d(base, &p.tm_b, 0, (int)site0, 0, &full_bar[stage]);            // G[site, n], sites >= M zero
+                    const int64_t R0 = xb_div((uint32_t)site0, g.div_ox);      // first grid row of the chunk
+                    for (int j = 0; j < p.win_rows; ++j) {
+                        int b, iy;
+                        xb_pwin_box(g, R0 + j, mt, b, iy);
+                        tma_load_5d(base + G_BYTES + (uint32_t)j * p.win_slot, &p.tm_a, 0, p0, iy, b, 0, &full_bar[stage]);
+                    }
+                }
+            }
+        }
+    } else {
+        // ------------------------------------------------------------------ consumers: wgmma issue + epilogue
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONS_REGS));
+        const int wg = warp >> 2;
+        // B as in conv_tc_kernel's weight gradient with b_tma: MN-major, 128-byte swizzle, planes w_plane = 8192 B apart,
+        // K step of 16 sites = 2048 B
+        const uint64_t b_tmpl = make_desc_sw128(0, xb_conv_w_plane_bytes(N), 1024);
+        // this lane's ldmatrix row (see conv_tc_kernel): k row = site 8 (mi >> 1) + lr of the K step, m rows = the 8 K rows
+        // from 64 wg + m_l of the tile
+        const int mi = lane >> 3, lr = lane & 7, m_l = 16 * (warp & 3) + 8 * (mi & 1);
+        const uint32_t tap_off = xb_pwin_tap_off(g, 64 * wg + m_l);
+        const int rbase = 64 * wg + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+        float acc[PB * NC][16];
+        uint32_t it = 0;
+        for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
+            const int64_t sp = w / m_tiles;
+            const int mt = (int)(w - sp * m_tiles);
+            const int n_chunks = chunks_of(sp);
+            uint32_t scale_d = 0;
+            uint32_t af[KC / 16][PA][4];
+            for (int kc = 0; kc < n_chunks; ++kc, ++it) {
+                const int stage = (int)(it % (uint32_t)S);
+                const uint32_t base = smem_base + (uint32_t)stage * stage_bytes;
+                const int64_t site0 = sp * p.sites_per_split + (int64_t)kc * KC;
+                const int64_t R0 = xb_div((uint32_t)site0, g.div_ox);      // first grid row of the chunk
+                const uint32_t win = base + G_BYTES + tap_off;
+                uint32_t row[KC / 16];
+#pragma unroll
+                for (int ks = 0; ks < KC / 16; ++ks) row[ks] = win + xb_pwin_site_off(g, site0 + 16 * ks + 8 * (mi >> 1) + lr, R0, p.win_slot);
+                timed_wait(&full_bar[stage], (it / (uint32_t)S) & 1u, 0);
+                // every fragment of the chunk is loaded while no wgmma is in flight (see conv_tc_kernel)
+#pragma unroll
+                for (int ks = 0; ks < KC / 16; ++ks)
+#pragma unroll
+                    for (int q = 0; q < PA; ++q) ldmatrix_x4<1>(af[ks][q], xb_sw128(row[ks] + (uint32_t)q * pair_plane));
+                wgmma_fence();
+                const uint64_t b0 = b_tmpl + (uint64_t)(base >> 4);
+#pragma unroll
+                for (int ks = 0; ks < KC / 16; ++ks) {
+                    const uint64_t db = b0 + (uint64_t)(ks * (2048 >> 4));
+                    mma_plane<1, PB, NC, 0>(acc, af[ks][0], db, scale_d);
+                    mma_plane<1, PB, NC, 1>(acc, af[ks][1], db, 1u);
+                    mma_plane<1, PB, NC, 2>(acc, af[ks][2], db, 1u);
+                    scale_d = 1;
+                }
+                wgmma_commit();
+                timed_wgmma_wait<0>(p.timing, t_wait[3]);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[stage]);
+            }
+            const uint32_t t_epi = p.timing ? clock32() : 0u;
+            // ---- epilogue: partials [splits, K, 64], rows 128 mt + rbase (+ 8), accumulator groups added smallest first
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float *row = p.out_f32 + (sp * K + 128 * mt + rbase + 8 * h) * N;
+#pragma unroll
+                for (int cc = 0; cc < NC; ++cc)
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        float v[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            v[e] = acc[(PB - 1) * NC + cc][4 * i + 2 * h + e];
+#pragma unroll
+                            for (int gq = PB - 2; gq >= 0; --gq) v[e] += acc[gq * NC + cc][4 * i + 2 * h + e];
+                        }
+                        *reinterpret_cast<float2 *>(row + 32 * cc + 8 * i + cq) = make_float2(v[0], v[1]);
+                    }
+            }
+            if (p.timing) t_wait[4] += clock32() - t_epi;
+        }
+    }
+    if (p.timing && blockIdx.x < 160) {
+        const unsigned long long now = clock64();
+        unsigned long long *o = xb_k12_timing[blockIdx.x];
+        if (tid == 0) o[0] = now - o[0], o[1] = t_wait[0], o[2] = t_wait[3], o[3] = 0, o[7] = t_wait[4];
+        if (tid == CONS_WARPS * 32) o[4] = now - o[4], o[5] = t_wait[0], o[6] = 0;
+    }
+}
+
 // weight-gradient finish: sum the split partials [splits, K, N] in a fixed order and scatter to torch's [N, C, KH, KW]
 // (column k = (kh, kw, c) of the packed layout -> xb_pack_weight_src); accumulate != 0 adds to dw (autograd .grad).
 // A block owns E = 256 / lanes consecutive (k, n) elements - coalesced rows of the partial matrices - and `lanes` threads
@@ -1045,6 +1209,22 @@ bool make_tmap_win(CUtensorMap *tm, const void *base, int B, int IH, int IW, int
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// pixel-pair windows of conv_tc_kernel_wgrad_pairs: the [planes][B][IH][IW][32] bf16 input as {64 channels, IW / 2 pairs,
+// IH rows, B images, planes}, boxes of {64 channels, win_w pairs, one row, one image, every plane}, 128-byte swizzle, zero
+// fill outside the image (an image's last rows never read the next image's first ones)
+bool make_tmap_pairs(CUtensorMap *tm, const void *base, int64_t plane_stride, int planes, int B, int IH, int IW, int win_w) {
+    EncodeTiledFn enc = encode_tiled_fn();
+    if (!enc || ((uintptr_t)base & 15) || (plane_stride * 2) % 16 || IW % 2 || win_w > 256) return false;
+    const cuuint64_t row_b = (cuuint64_t)IW * 64, img_b = (cuuint64_t)IH * row_b;
+    const cuuint64_t dims[5] = {64, (cuuint64_t)IW / 2, (cuuint64_t)IH, (cuuint64_t)B, (cuuint64_t)planes};
+    const cuuint64_t strides[4] = {128, row_b, img_b, planes > 1 ? (cuuint64_t)plane_stride * 2 : img_b * B};
+    const cuuint32_t box[5] = {64, (cuuint32_t)win_w, 1, 1, (cuuint32_t)planes};
+    const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+    return enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void *>(base), dims, strides, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
 // bf16 activation tensor [planes][rows][pixels][channels] (padded-row layout, rows = images x padded rows per image merged),
 // boxes of {64 channels, box_px pixels, box_h rows of ONE row phase, one plane}, 128-byte swizzle
 bool make_tmap_box(CUtensorMap *tm, const void *base, int C, int W, int64_t rows, int planes, int64_t plane_stride, int box_c,
@@ -1172,6 +1352,30 @@ int launch_win(const ConvParams &p, void *stream) {
     const int grid = p.splits < xb_sm_count() ? p.splits : xb_sm_count();
     conv_tc_kernel_wgrad_win<PB><<<grid, THREADS, p.dyn_smem, (cudaStream_t)stream>>>(p);
     return xb_launch_status();
+}
+
+// conv_tc_kernel_wgrad_pairs takes a weight gradient with three planes on each side whose A operand is a 32-channel input
+// read through a full KH x 4 tap rectangle in row-major order with an even column stride and first column (each 128-row
+// K tile is one tap row: two 64-channel pixel pairs per site), with N = n_tile = 64 - conv2 of BoxNatureCNN over act1.
+// Fills the window fields and the ring of p.
+bool wgrad_pairs_setup(ConvParams &p, int planes_a, int planes_b, int N, int n_tile) {
+    const XbConvGeom &g = p.g;
+    if (planes_a != 3 || planes_b != 3 || g.C != 32 || N != 64 || n_tile != 64 || g.T % XB_PWIN_KW != 0) return false;
+    if (g.sx % 2 != 0 || g.dx[0] % 2 != 0 || g.IW % 2 != 0) return false;
+    for (int t = 0; t < g.T; ++t)
+        if (g.dy[t] != g.dy[0] + t / XB_PWIN_KW || g.dx[t] != g.dx[0] + t % XB_PWIN_KW) return false;
+    const int win_w = xb_pwin_width(g);
+    if (win_w <= 0 || win_w > 256 || p.M + KC >= ((int64_t)1 << 31)) return false;      // box limit, 32-bit site indices
+    p.win_kh = 1, p.win_w = win_w, p.win_rows = xb_win_rows(g);
+    // every slot 1024-byte aligned: TMA's swizzle phase of a box is then the same whether it follows the address or the
+    // box's own rows
+    p.win_slot = ((uint32_t)(3 * win_w * 128) + 1023u) & ~1023u;
+    const uint32_t stage_bytes = 3u * xb_conv_w_plane_bytes(64) + (uint32_t)p.win_rows * p.win_slot;
+    int stages = (int)((uint32_t)XB_K12_MAX_DYN_SMEM / stage_bytes);
+    if (stages < 2) return false;
+    p.stages = stages > MAX_STAGES ? MAX_STAGES : stages;
+    p.dyn_smem = (uint32_t)p.stages * stage_bytes;
+    return true;
 }
 
 }  // namespace
@@ -1435,6 +1639,21 @@ extern "C" int xb_wgrad_gather_tc(int planes_a, int planes_b, const void *in, in
         if (planes_b == 1) return launch_win<1>(p, stream);
         if (planes_b == 2) return launch_win<2>(p, stream);
         return launch_win<3>(p, stream);
+    }
+    if (tma_enabled() && wgrad_pairs_setup(p, planes_a, planes_b, N, n_tile)) {
+        // both operands by TMA, the gathered path's work items (split, K tile) (conv_tc_kernel_wgrad_pairs)
+        if (!make_tmap_pairs(&p.tm_a, in, in_plane, planes_a, B, IH, IW, p.win_w) ||
+            !make_tmap(&p.tm_b, g, N, p.M, planes_b, g_ld, g_plane, KC))
+            return XB_EINVAL;
+        static bool attr = false;
+        if (!attr) {
+            cudaFuncSetAttribute(conv_tc_kernel_wgrad_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, XB_K12_MAX_DYN_SMEM);
+            attr = true;
+        }
+        const int64_t work = (int64_t)(T * C / TILE_M) * splits;
+        const int grid = (int)(work < xb_sm_count() ? work : xb_sm_count());
+        conv_tc_kernel_wgrad_pairs<<<grid, THREADS, p.dyn_smem, (cudaStream_t)stream>>>(p);
+        return xb_launch_status();
     }
     if (tma_enabled()) {
         // output gradient [planes_b][sites][g_ld]: tiles of {64 columns, 64 sites, all planes} (one 64-column block per plane)
