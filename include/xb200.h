@@ -145,6 +145,31 @@ int xb_ppo_gauss_loss_fwd_bwd(const float *mu, const float *log_std, const float
                               float *dmu, float *dlog_std, float *dvalue, float *stats, double *scratch, double *ws,
                               int64_t ws_doubles, void *stream);
 
+/* ---------------------------------------------------------------- K4P: fused PPG auxiliary loss fwd+bwd -
+ * ppg_learner.py:114-148 (update_auxiliary_critic) plus the autograd backward of its loss down to the network outputs:
+ *   aux_loss = MSE(v.detach(), aux_v); kl_loss = mean(KL(pi_new || pi_old)); value_loss = MSE(v, R)
+ *   loss = aux_loss + kl_beta * kl_loss + value_loss
+ * dvalue[B] = 2 (v - R) / B_total, daux[B] = 2 (aux_v - v) / B_total (aux_loss reaches aux_v only), means over
+ * B_total >= B rows as K4, so the SUM of the shards' outputs is the global result.  stats[8] = {aux_loss, kl_loss,
+ * value_loss, loss, mean(v), 0, 0, 0}.  scratch as for K4.  One warp per row; no allocation; graph-capturable.
+ * xb_ppg_aux_loss_fwd_bwd (Categorical): logits / old_logits [B, A] raw (each side is log-softmax normalised in the
+ *   kernel, as Categorical(logits=) does), 1 <= A <= 64 (else XB_ERANGE).  dlogits = kl_beta * dKL/dlogits with torch's
+ *   zero-probability rules (a term is +inf where q = 0 and 0 where p = 0, and those terms pass no gradient; a -inf logit
+ *   on either side makes its row's gradient NaN, as autograd's 0 * inf does).  logits, old_logits and dlogits are NULL
+ *   together: then only value_loss is formed (update_critic, ppg_learner.py:90-112: critic-loss = stats[2]).
+ *   aux_value and daux are NULL together (aux_loss = 0).
+ * xb_ppg_aux_gauss_loss_fwd_bwd (DiagGaussian): Normal(mu, exp(log_std)) against Normal(old_mu, exp(old_log_std)),
+ *   mu / old_mu [B, D], log_std / old_log_std [D], 1 <= D <= 64 (else XB_ERANGE); kl_loss is the mean over B_total * D
+ *   terms.  dmu [B, D]; dlog_std [D] = the sum over the local rows (the term depends on the column only: formed as B
+ *   times it in double, bit-identical).  Every pointer is required. */
+int xb_ppg_aux_loss_fwd_bwd(const float *logits, const float *old_logits, const float *value, const float *aux_value,
+                            const float *ret, int64_t B, int A, int64_t B_total, float kl_beta, float *dlogits,
+                            float *dvalue, float *daux, float *stats, double *scratch, void *stream);
+int xb_ppg_aux_gauss_loss_fwd_bwd(const float *mu, const float *log_std, const float *old_mu, const float *old_log_std,
+                                  const float *value, const float *aux_value, const float *ret, int64_t B, int D,
+                                  int64_t B_total, float kl_beta, float *dmu, float *dlog_std, float *dvalue,
+                                  float *daux, float *stats, double *scratch, void *stream);
+
 /* ---------------------------------------------------------------- K4M: fused MAPPO loss fwd+bwd -------
  * Replaces mappo_learner.py:55-113 (one parameter-sharing group, feed-forward actor and critic, Discrete actions) plus
  * the autograd backward of those lines down to (logits, value).  One row = one agent at one env step.

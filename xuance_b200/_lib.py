@@ -36,6 +36,10 @@ _SIGNATURES = {
     "xb_ppo_gauss_ws_doubles": (c_int64, [c_int64, c_int]),
     "xb_ppo_gauss_loss_fwd_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int64, c_int, c_int64, c_float, c_float,
                                           c_float, c_int, _P, _P, _P, _P, _P, _P, c_int64, _P]),
+    "xb_ppg_aux_loss_fwd_bwd": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int, c_int64, c_float, _P, _P, _P, _P, _P,
+                                        _P]),
+    "xb_ppg_aux_gauss_loss_fwd_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int64, c_int, c_int64, c_float, _P, _P,
+                                              _P, _P, _P, _P, _P]),
     "xb_mappo_prepare": (c_int, [_P, _P, c_int64, _P, _P, _P]),
     "xb_value_norm_update": (c_int, [_P, _P, _P, _P, c_int64, c_double, _P, _P]),
     "xb_mappo_loss_fwd_bwd": (c_int, [_P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, c_int64,

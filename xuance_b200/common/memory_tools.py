@@ -169,6 +169,10 @@ class DummyOnPolicyBuffer(Buffer):
     obs_dtype = torch.float32
     _ckpt_tensors = ("_obs", "_act_rows", "_fields")
     _ckpt_host = ("_seg_end_h", "_boot_h", "_covered_h", "start_ids")
+    # the non-scalar auxiliary field that holds the old policy's parameters (PPG): ``sample`` returns it as the batched
+    # distribution the reference's merge_distributions builds - Categorical(logits=rows) for a Discrete action space,
+    # Normal(rows, exp(dist_log_std)) for a Box one
+    DIST_KEY = "old_dist"
 
     def _after_load(self):
         self._gae_dirty = True      # returns / advantages are recomputed from the restored segment bookkeeping
@@ -186,10 +190,10 @@ class DummyOnPolicyBuffer(Buffer):
             raise NotImplementedError("dict observation spaces are outside the hot path (SURVEY.md section 8)")
         self._obs_shape = tuple(obs_shape)
         self._act_shape = tuple(space2shape(self.action_space))
-        self._aux_keys = list((auxiliary_shape or {}).keys())
-        for k in self._aux_keys:
-            if tuple(auxiliary_shape[k]) != ():
-                raise NotImplementedError("only scalar auxiliary infos are on the hot path (e.g. old_logp)")
+        aux_shapes = {k: tuple(v) for k, v in (auxiliary_shape or {}).items()}
+        self._aux_keys = [k for k, v in aux_shapes.items() if v == ()]
+        # non-scalar auxiliary fields: float32 row blocks [N, T, *shape], stored and gathered as the Box action rows are
+        self._aux_row_keys = [k for k, v in aux_shapes.items() if v != ()]
         self._scalar_action = self._act_shape == ()
         names = ["rewards", "terminals"] + (["actions"] if self._scalar_action else []) + ["values"]
         names += ["aux:" + k for k in self._aux_keys]
@@ -202,6 +206,16 @@ class DummyOnPolicyBuffer(Buffer):
         self._obs = self._alloc_rows(self._obs_shape, self.obs_dtype)
         self._act_rows = None if self._scalar_action else self._alloc_rows(self._act_shape, torch.float32)
         self._fields = torch.zeros((len(names), N, T), dtype=torch.float32, device=self.device)
+        self.aux_rows = {k: self._alloc_rows(aux_shapes[k], torch.float32) for k in self._aux_row_keys}
+        self.dist_log_std = None
+        if self.DIST_KEY in self.aux_rows and not self._scalar_action:
+            # the Box policy's log_std snapshot the old_dist rows (its means) were written with: one [D] vector
+            self.dist_log_std = torch.zeros(self._act_shape, dtype=torch.float32, device=self.device)
+        if self._aux_row_keys:
+            for k, t in self.aux_rows.items():
+                setattr(self, "_aux_rows_" + k, t)
+            self._ckpt_tensors = type(self)._ckpt_tensors + tuple("_aux_rows_" + k for k in self._aux_row_keys) + \
+                ("dist_log_std",)
         # GAE bookkeeping: host (pinned) master copies + device mirrors uploaded when dirty
         self._seg_end_h = torch.zeros((N, T), dtype=torch.uint8).pin_memory()
         self._boot_h = torch.zeros((N, T), dtype=torch.float32).pin_memory()
@@ -252,7 +266,9 @@ class DummyOnPolicyBuffer(Buffer):
 
     @property
     def auxiliary_infos(self):
-        return {k: self._fields[self._fid["aux:" + k]] for k in self._aux_keys}
+        infos = {k: self._fields[self._fid["aux:" + k]] for k in self._aux_keys}
+        infos.update(self.aux_rows)
+        return infos
 
     def clear(self):
         """Reference :221-230 re-allocates zeroed arrays; here the cursors and the GAE bookkeeping are reset and
@@ -308,6 +324,9 @@ class DummyOnPolicyBuffer(Buffer):
             self._stage_i ^= 1
         if not self._scalar_action:
             self._store_rows(self._act_rows, acts, t)
+        for k in self._aux_row_keys:       # a row field the caller does not supply at acting time stays as it is
+            if aux_info.get(k) is not None:
+                self._store_rows(self.aux_rows[k], aux_info[k], t)
         self.ptr = (self.ptr + 1) % self.n_size
         self.size = min(self.size + 1, self.n_size)
 
@@ -445,10 +464,29 @@ class DummyOnPolicyBuffer(Buffer):
             "actions": row("actions") if self._scalar_action else self._gather_rows(self._act_rows, idx_t),
             "returns": row("returns"),
             "values": row("values"),
-            "aux_batch": {k: row("aux:" + k) for k in self._aux_keys},
+            "aux_batch": self._aux_batch(row, idx_t),
             "batch_size": idx_t.numel(),
             "advantages": row("advantages"),
         }
+
+    def _aux_batch(self, row, idx_t):
+        batch = {k: row("aux:" + k) for k in self._aux_keys}
+        for k in self._aux_row_keys:
+            rows = self._gather_rows(self.aux_rows[k], idx_t)
+            batch[k] = self._as_distribution(rows) if k == self.DIST_KEY else rows
+        if self.dist_log_std is not None:      # the exact snapshot, not log(exp(.)) of the distribution's scale
+            batch[self.DIST_KEY + "_log_std"] = self.dist_log_std
+        return batch
+
+    def _as_distribution(self, rows):
+        from ..torch.rl_models.distributions import CategoricalDistribution, DiagGaussianDistribution
+        if self._scalar_action:
+            dist = CategoricalDistribution(rows.shape[-1])
+            dist.set_param(logits=rows)
+        else:
+            dist = DiagGaussianDistribution(rows.shape[-1])
+            dist.set_param(rows, self.dist_log_std.exp().expand_as(rows))
+        return dist
 
     def sample(self, indexes, adv_stats=None):
         """reference :267-287.  ``indexes`` are flat slots (env*T+step, as np.arange(buffer_size) shuffled by

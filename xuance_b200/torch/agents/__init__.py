@@ -4,9 +4,10 @@ from .off_policy import OffPolicyAgent
 from .ppo_agent import PPO_Agent
 from .dqn_agent import DQN_Agent, PerDQN_Agent, DuelDQN_Agent
 from .dist_dqn_agent import C51_Agent, QRDQN_Agent
+from .ppg_agent import PPG_Agent
 
 REGISTRY_Agents = {"PPO": PPO_Agent, "PPO_Clip": PPO_Agent, "DQN": DQN_Agent, "PerDQN": PerDQN_Agent, "DuelDQN": DuelDQN_Agent,
-                   "C51DQN": C51_Agent, "QRDQN": QRDQN_Agent}
+                   "C51DQN": C51_Agent, "QRDQN": QRDQN_Agent, "PPG": PPG_Agent}
 try:
     from .sac_agent import SAC_Agent
     REGISTRY_Agents["SAC"] = SAC_Agent

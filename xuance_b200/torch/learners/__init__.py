@@ -7,6 +7,7 @@ from .sacdis_learner import SACDIS_Learner
 from .ddpg_learner import DDPG_Learner, TD3_Learner
 from .qmix_learner import QMIX_Learner
 from .mappo_learner import MAPPO_Learner
+from .ppg_learner import PPG_Learner
 
 REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner, "DQN_Learner": DQN_Learner,
                      "PerDQN_Learner": PerDQN_Learner, "DDQN_Learner": DDQN_Learner, "A2C_Learner": A2C_Learner,
@@ -16,4 +17,4 @@ REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner,
                      "DDPG_Learner": DDPG_Learner, "TD3_Learner": TD3_Learner,
                      "QMIX_Learner": QMIX_Learner,
                      "VDN_Learner": QMIX_Learner,     # vdn_learner.py: the same update with the parameter-free sum mixer
-                     "MAPPO_Learner": MAPPO_Learner}
+                     "MAPPO_Learner": MAPPO_Learner, "PPG_Learner": PPG_Learner}

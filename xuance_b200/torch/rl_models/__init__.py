@@ -8,7 +8,7 @@ from .heads import (CategoricalActorHead, GaussianActorHead, SAC_GaussianActorHe
 from .architectures import (ActorCritic, SharedActorCritic, DeepQNetwork, DuelingDeepQNetwork, GaussianActor, SAC_GaussianActor,
                             TwinActionValueCritic, SoftActorCritic, TwinDiscreteActionValueCritic, SoftActorCriticDiscrete,
                             DeterministicActor, ActionValueCritic, DeterministicActorCritic, TwinDelayedActorCritic,
-                            C51DeepQNetwork, QRDeepQNetwork)
+                            C51DeepQNetwork, QRDeepQNetwork, StateValueCritic, PhasicActorCritic)
 from .qmix import Basic_RNN, AgentFeatureEncoder, DiscreteActionValueCritic, QMIX_Mixer, VDN_mixer, MixingQNetwork
 REGISTRY_Representation["Basic_RNN"] = Basic_RNN
 from .mappo import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic

@@ -522,3 +522,56 @@ class TwinDelayedActorCritic(DeterministicActorCritic):
     def Qpolicy(self, observation):
         q1, q2 = self.Qpolicy_pair(observation)
         return (q1 + q2) / 2.0
+
+
+class StateValueCritic(nn.Module):
+    """critics/base_critics.py:11-43: V(s) = ValueHead(representation(s))."""
+
+    def __init__(self, representation, critic_hidden_size, normalizer=None, initializer=None, activation=None,
+                 device=None, **kwargs):
+        super().__init__()
+        self.representation = representation
+        self.representation_info_shape = representation.output_shapes
+        self.critic_head = ValueHead(feature_dim=self.representation_info_shape['state'][0],
+                                     hidden_size=critic_hidden_size, normalizer=normalizer, initializer=initializer,
+                                     activation=activation, device=device)
+
+    def values(self, observation):
+        """The [B] values alone."""
+        return self.critic_head(self.representation(observation).embeddings)
+
+    def forward(self, observation, **kwargs):
+        rep_out = self.representation(observation, **kwargs)
+        return CriticOutput(representations=rep_out, values=self.critic_head(rep_out.embeddings))
+
+
+class PhasicActorCritic(ActorCritic):
+    """actor_critic.py:75-104: an actor (CategoricalActor or GaussianActor) and two StateValueCritics, each with its own
+    representation, sharing no parameter.  ``forward`` returns the actor's distribution and ``critic``'s values.
+    Parameters are registered actor, critic, aux_critic: ``parameters()`` lists the three groups in that order, the
+    layout the PPG learner's per-group Adam steps by range.  ``forward_raw`` / ``forward_raw_gauss`` give the raw actor
+    outputs and ``critic``'s values, the tensors the fused loss and acting kernels consume."""
+
+    def __init__(self, actor, critic, aux_critic, **kwargs):
+        super().__init__(actor, critic, **kwargs)
+        self.aux_critic = aux_critic
+
+    def logits(self, observation):
+        return self.actor.logits(observation)
+
+    def mu_log_std(self, observation):
+        head = self.actor.actor_head
+        return head.mu(self.actor.representation(observation).embeddings), head.log_std
+
+    def forward_raw(self, observation):
+        """(logits [B, A], values [B])."""
+        return self.logits(observation), self.critic.values(observation)
+
+    def forward_raw_gauss(self, observation):
+        """(mu [B, D], log_std [D], values [B])."""
+        mu, log_std = self.mu_log_std(observation)
+        return mu, log_std, self.critic.values(observation)
+
+    def aux_values(self, observation):
+        """``aux_critic``'s [B] values."""
+        return self.aux_critic.values(observation)

@@ -11,6 +11,7 @@ import torch
 import torch.nn as nn
 
 from .heads import CategoricalActorHead, ValueHead
+from .outputs import StochasticActorOutput
 
 
 class CategoricalActor(nn.Module):
@@ -26,6 +27,12 @@ class CategoricalActor(nn.Module):
                                                hidden_size=actor_hidden_size, action_dim=self.action_dim,
                                                normalizer=normalizer, initializer=initializer, activation=activation,
                                                device=device)
+
+    def forward(self, observation, avail_actions=None, **kwargs):
+        """categorical_actors.py:38-48: the representation's output and the head's CategoricalDistribution."""
+        rep_out = self.representation(observation, **kwargs)
+        return StochasticActorOutput(representations=rep_out,
+                                     distributions=self.actor_head(rep_out.embeddings, avail_actions=avail_actions))
 
     def logits(self, observations, rnn_states=None, return_states=False):
         """Recurrent representations take [S, T, obs] (or [S, obs] for one step) and the state [1, S, H]."""
