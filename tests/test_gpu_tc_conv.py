@@ -1,7 +1,8 @@
 """GPU parity tests of the K12 tensor-core layers (xuance_b200/csrc/conv_tc.cu) against float64 references: operand
 preparation, forward (2 / 3 planes, raw uint8 single plane), data gradient with a given ReLU mask, weight gradient
 (MN-major operands, site splits, column tiles), the Linear layer in all three modes, the whole encoder forward + backward
-next to cuDNN fp32, and a PPO update with compute="tc" next to the fp32 learner.
+next to cuDNN fp32, and a PPO update with compute="tc" next to the fp32 learner.  The assembled encoder is compared with
+float64 layer by layer, at the agents' batch sizes and on every path switch, in tests/test_gpu_k12_encoder.py.
 
 Tolerances.  Operands with 3 planes are exact to 2^-24; what remains is the float32 accumulation of the tensor core, which
 truncates on every addition of a 16-deep product block (results are biased toward zero by up to ~0.5 ulp per K step of
