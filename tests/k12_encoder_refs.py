@@ -47,6 +47,10 @@ stored tensor may have a zero last plane.
 
 ``check`` returns {tensor: max(|kernel - r| / bound)} and raises on any ratio > 1 and on any padding element of the
 persistent padded buffers that is not bitwise zero.
+
+The weight- and bias-gradient bounds above are worst cases over chains of up to 4096 sites and leave room for a lost or
+repeated chunk, split or column-sum row at large B; tests/test_gpu_k12_exact_reductions.py (with tests/k12_exact_refs.py)
+pins those reductions bit for bit on exactly representable operands instead.
 """
 import torch
 import torch.nn.functional as F

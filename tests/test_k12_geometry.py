@@ -187,7 +187,7 @@ def r_pack_conv_weight(w, planes=2, scale=1.0):
 def _epilogue(v, opix, mpix, tile, bias, relu, out_f32, out_pl, out_ld, out_c0, mask, mask_ld, mask_c0, colsum):
     """v [rows, N] float64 of the rows a launch writes; opix / mpix their output / mask pixels, tile their colsum row."""
     N = v.shape[1]
-    cols = torch.arange(N)
+    cols = torch.arange(N, device=v.device)
     if bias is not None:
         v = v + bias.double()
     if relu:
@@ -204,7 +204,7 @@ def _epilogue(v, opix, mpix, tile, bias, relu, out_f32, out_pl, out_ld, out_c0, 
         for q in range(out_pl.shape[0]):
             out_pl[q].view(-1)[idx] = pl[q]
     if colsum is not None:
-        cs = torch.zeros(colsum.shape[0], N, dtype=torch.float64)
+        cs = torch.zeros(colsum.shape[0], N, dtype=torch.float64, device=v.device)
         cs.index_add_(0, tile, v.double())
         colsum.view(-1, N).copy_(cs.float())
 
@@ -212,7 +212,7 @@ def _epilogue(v, opix, mpix, tile, bias, relu, out_f32, out_pl, out_ld, out_c0, 
 def _gathered(x_pl, g):
     """The [M, T*C] A operand of the gathered GEMM ``g`` (float64), input planes in [B, IH, IW, C] element order."""
     x = x_pl.double().sum(0).reshape(g.B, g.IH, g.IW, g.C)
-    ys, xs = torch.arange(g.OY) * g.sy, torch.arange(g.OX) * g.sx
+    ys, xs = torch.arange(g.OY, device=x.device) * g.sy, torch.arange(g.OX, device=x.device) * g.sx
     cols = []
     for dy, dx in zip(g.dy, g.dx):
         iy, ix = ys + dy, xs + dx
@@ -225,7 +225,7 @@ def r_gemm_gather(x_pl, w_pl, geom, bias=None, relu=False, out_f32=None, out_pl=
                   n_tile=None, mask_ld=0, mask_c0=0, colsum=None):
     W = w_pl.double().sum(0)
     out_ld = W.shape[0] if out_ld is None else out_ld
-    m = torch.arange(geom.M)
+    m = torch.arange(geom.M, device=W.device)
     b, y, x = m // (geom.OY * geom.OX), (m // geom.OX) % geom.OY, m % geom.OX
     opix = (b * geom.out_H + y * geom.oys + geom.oy0) * geom.out_W + x * geom.oxs + geom.ox0
     _epilogue(_gathered(x_pl, geom) @ W.t(), opix, opix, m // 128, bias, relu, out_f32, out_pl, out_ld, out_c0, relu_mask,
@@ -236,7 +236,7 @@ def r_gemm_gather(x_pl, w_pl, geom, bias=None, relu=False, out_f32=None, out_pl=
 def _box_rows(x, bg, R):
     """A operand of the box GEMM for merged grid rows R: [len(R), box_px, n_chunks*64], zero outside the tensor."""
     rows, W, _ = x.shape
-    xs = torch.arange(bg.box_px)
+    xs = torch.arange(bg.box_px, device=x.device)
     parts = []
     for c0, w0, r0 in bg.chunks:
         row, px = R * bg.row_step + r0, xs + w0
@@ -249,12 +249,12 @@ def r_gemm_box(x_pl, w_pl, bg, bias=None, relu=False, out_f32=None, out_pl=None,
                n_tile=None, colsum=None):
     W = w_pl.double().sum(0)
     out_ld = W.shape[0] if out_ld is None else out_ld
-    R = torch.arange(bg.B * bg.hp_out)
+    R = torch.arange(bg.B * bg.hp_out, device=W.device)
     b, y = R // bg.hp_out, R % bg.hp_out
     live = (y >= bg.y0) & (y <= bg.y1)
     v = _box_rows(x_pl.double().sum(0).reshape(-1, bg.W, bg.C), bg, R[live]) @ W.t()          # [rows, px, N]
     orow = (b * bg.out_H + (y - bg.y0) * bg.oys + bg.oy0)[live][:, None]
-    ocol = (torch.arange(bg.box_px) * bg.oxs + bg.ox0)[None, :]
+    ocol = (torch.arange(bg.box_px, device=W.device) * bg.oxs + bg.ox0)[None, :]
     mW, mx0 = (bg.mask_W, bg.mask_x0) if bg.mask_W > 0 else (bg.out_W, 0)
     f = lambda t: t.expand(v.shape[:2]).reshape(-1)
     _epilogue(v.reshape(-1, v.shape[-1]), f(orow * bg.out_W + ocol), f(orow * mW + ocol + mx0), f((R[live] // bg.box_h)[:, None]),
@@ -268,11 +268,11 @@ def r_gemm_halo(x_pl, w_pl, hg, bias=None, relu=False, out_f32=None, out_pl=None
     W = w_pl.double().sum(0)
     n_sub = len(hg.subs)
     out_ld = (hg.N if hg.same_cols else W.shape[0]) if out_ld is None else out_ld
-    pos = torch.arange(hg.M)
+    pos = torch.arange(hg.M, device=x.device)
     R, px = pos // hg.halo_w, pos % hg.halo_w + hg.halo_w0
     b, y = R // hg.hp, R % hg.hp
     mW, mx0 = (hg.mask_W, hg.mask_x0) if hg.mask_W > 0 else (hg.out_W, 0)
-    cs = torch.zeros(-(-hg.M // 128) * n_sub, hg.N) if colsum is not None else None
+    cs = torch.zeros(-(-hg.M // 128) * n_sub, hg.N, device=x.device) if colsum is not None else None
     for j, sb in enumerate(hg.subs):
         live = (y >= hg.y0) & (y <= sb["y1"]) & (px >= 0) & (px <= sb["x1"])
         Rl, pl = R[live], px[live]
