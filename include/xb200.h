@@ -292,6 +292,44 @@ int xb_qmix_td(const float *q_tot, const float *q_tot_next, const float *rewards
                const float *filled, const float *filled_sum, int B, int n, int T, float gamma, int64_t rows_total,
                float *dq_tot, float *stats, double *scratch, void *stream);
 
+/* ---------------------------------------------------------------- K9W: Weighted QMIX selection / loss --
+ * Replaces, for one parameter-sharing group with use_rnn=True, wqmix_learner.py:27-129 (_forward_transitions) and
+ * :141-199 (the weighted loss of update) plus their autograd backward down to the agent-network outputs.  Layouts as K9:
+ * q_all / q_cent / q_cent_tgt / q_tgt [B,n,T+1,A] (eval, central, target central and target agent networks), actions /
+ * agent_mask [B,n,T] and filled [B,T] float32, avail (nullable) uint8 [B,n,T+1,avail_ld], non-zero = available.
+ * select_fwd: per (b,i,t), m = agent_mask*filled, g_t = the first maximal index of q_all at t with unavailable actions
+ *           at -1e10 (value_factorization.py:86-91); the next action is g_{t+1} when double_q, else the UNMASKED first
+ *           argmax of q_tgt at t+1 (q_tgt may be NULL when double_q; the reference's use_rnn branch never masks it).
+ *           Writes, agent-minor [B*T, n]: q_eval_taken = q_all[t, a_t]*m, q_cent_taken = q_cent[t, g_t]*m,
+ *           q_next_cent = q_cent_tgt[t+1, next]*m; greedy[B,n,T] = g_t (int32, saved for the backward);
+ *           agree[B*T] = all_i (g_t == a_t and m != 0) (uint8, CW-QMIX's condition_1: a dead or padded agent clears it);
+ *           filled_sum[0] = sum(filled).  One thread per (b,t) row.
+ * select_bwd: dq_all[b,i,t,a_t] = d_eval[row,i]*m and dq_cent[b,i,t,g_t] = d_cent[row,i]*m into pre-zeroed outputs; either
+ *           (d_eval, dq_all) or (d_cent, dq_cent) may be a NULL pair, not both.
+ * loss    : r = mean_i rewards, d = all_i terminals (as xb_qmix_td); y = r + (1-d)*gamma*q_ff_next; td = q_tot - y;
+ *           w = alpha, or 1 where td < 0 (mode XB_WQMIX_OW) / where agree or y > q_ff (XB_WQMIX_CW; agree required);
+ *           loss_Qmix = sum(w*td^2*filled)/filled_sum, loss_central = sum((q_ff-y)^2*filled)/filled_sum.  Writes
+ *           dq_tot = 2*w*td*filled/filled_sum, dq_ff = 2*(q_ff-y)*filled/filled_sum (y and w carry no gradient) and
+ *           stats[4] = {loss_Qmix, loss_central, loss, predictQ = sum(q_tot)/rows_total}.  filled_sum[0] and rows_total >=
+ *           B*T are GLOBAL, so the SUM of the shards' outputs is the global result; deterministic two-level reduction,
+ *           scratch as for K4.
+ * All three: B, n, T, A >= 1 and non-NULL required pointers (else XB_EINVAL); n <= 16, the K9 mixer's limit (else
+ * XB_ERANGE).  No allocation; graph-capturable. */
+#define XB_WQMIX_OW 0
+#define XB_WQMIX_CW 1
+int xb_wqmix_select_fwd(const float *q_all, const float *q_cent, const float *q_cent_tgt, const float *q_tgt,
+                        const float *actions, const float *agent_mask, const float *filled, const uint8_t *avail,
+                        int avail_ld, int B, int n, int T, int A, int double_q, float *q_eval_taken,
+                        float *q_cent_taken, float *q_next_cent, int32_t *greedy, uint8_t *agree, float *filled_sum,
+                        double *scratch, void *stream);
+int xb_wqmix_select_bwd(const float *d_eval, const float *d_cent, const float *actions, const int32_t *greedy,
+                        const float *agent_mask, const float *filled, int B, int n, int T, int A, float *dq_all,
+                        float *dq_cent, void *stream);
+int xb_wqmix_loss_fwd_bwd(const float *q_tot, const float *q_ff, const float *q_ff_next, const float *rewards,
+                          const float *terminals, const float *filled, const uint8_t *agree, const float *filled_sum,
+                          int B, int n, int T, int mode, float alpha, float gamma, int64_t rows_total, float *dq_tot,
+                          float *dq_ff, float *stats, double *scratch, void *stream);
+
 /* Tensor-core forward of the whole mixer (hypernet GEMMs + epilogue in ONE kernel; wgmma with register
  * accumulators, bf16 hi/lo split operands, 3 MMAs per product, fp32 accumulate): q_tot[R] from states[R,S], q[R,n]
  * and the raw Linear parameters of QMIX_Mixer (q_mix_head.py:52-64): w_l1[4] / b_l1[4] are HOST arrays of 4 device

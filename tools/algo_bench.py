@@ -4,7 +4,8 @@ DQN+PER (2^20-transition HBM replay, B=512), SAC (1M replay, B=1024) and QMIX (5
 on one GPU, next to the oracle port of the reference's torch-CPU path on the host; and ``ppo_gauss``, continuous-control
 PPO in the shape of the reference's ppo/mujoco.yaml (train_epochs env-steps/s); ``mappo``, MAPPO in the shape of
 configs/mappo/sc2/5m_vs_6m.yaml (train_epochs env-steps/s); ``mappo_rnn``, recurrent MAPPO in the shape of
-configs/mappo/sc2/3m.yaml (update, eager and graphed); ``sacdis``, SAC-Discrete in the shape of
+configs/mappo/sc2/3m.yaml (update, eager and graphed); ``wqmix``, CW-QMIX in the shape of configs/wqmix/sc2/5m_vs_6m.yaml
+(update, eager and graphed); ``sacdis``, SAC-Discrete in the shape of
 configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (train_epochs, eager and graphed); ``ddpg`` and
 ``td3``, DDPG / TD3 in the shape of the reference's ddpg/mujoco.yaml and td3/mujoco.yaml (sample + update, eager and
 graphed); ``c51`` and ``qrdqn`` on CartPole (Basic_MLP 128, B=256) and SyntheticAtari (Basic_CNN, B=32) shapes (update,
@@ -188,6 +189,43 @@ def bench_qmix(args, Be=32):
         ol = QMIXLearnerOracle(QMIXModelOracle(n, od, A, S), keys, detach_q_eval=False)
         cdt = cpu_timed(lambda: ol.update(ob.sample()), max(args.cpu_iters, 10))
         out.update(cpu_updates_per_s=1 / cdt, cpu_ms_per_update=cdt * 1e3, cpu_threads=torch.get_num_threads(), speedup=cdt / dt)
+    return out
+
+
+def bench_wqmix(args, B=32):
+    """One WQMIX_Learner update in the shape of configs/wqmix/sc2/5m_vs_6m.yaml (5 agents x 72-d, S=98, A=12, T=60, 32
+    episodes, GRU 64, QMIX mixer 32/64, feed-forward mixer 256, action masks, CW-QMIX), eager and graphed, on a device-resident
+    sample; next to the torch-CPU oracle of the same update."""
+    import wqmix_refs as R
+    from oracle_wqmix import WQMIXModelOracle, WQMIXLearnerOracle
+    from test_gpu_wqmix import _product_model
+    from xuance_b200.common import BaseCallback
+    from xuance_b200.torch.learners import REGISTRY_Learners
+    n, od, A, S, T = 5, 72, 12, 98, 60
+    keys = [f"agent_{i}" for i in range(n)]
+    sample = R.fix_sample(np.random.default_rng(0), keys, B=B, T=T, obs_dim=od, A=A, S=S)
+    dev = lambda x: {k: dev(v) for k, v in x.items()} if isinstance(x, dict) else (
+        torch.as_tensor(x, device=DEV) if isinstance(x, np.ndarray) else x)
+    dsample = dev(sample)
+    out = {"config": f"CW-QMIX, 5 agents x 72-d, S=98, A=12, T=60, {B} episodes/update, GRU 64, mixer 32/64, "
+                     f"feed-forward mixer 256, action masks"}
+    for graph in (False, True):
+        torch.manual_seed(0)
+        _, grouping, model = _product_model(n, od, A, S, 64, 32, 64, 256)
+        cfg = Namespace(agent="CWQMIX", alpha=0.1, distributed_training=False, episode_length=T, use_grad_clip=False,
+                        grad_clip_norm=0.5, device=DEV, model_dir="/tmp/x", running_steps=10**7, parallels=8,
+                        use_parameter_sharing=True, use_rnn=True, use_actions_mask=True, learning_rate=7e-4,
+                        sync_frequency=200, double_q=True, n_epochs=1, start_training=0, gamma=0.99,
+                        use_cuda_graph=graph)
+        lrn = REGISTRY_Learners["WQMIX_Learner"](cfg, grouping, model, BaseCallback())
+        dt = timed(lambda: lrn.update(dsample, sync=False), args.iters)
+        out["gpu_ms_per_update_graphed" if graph else "gpu_ms_per_update_eager"] = dt * 1e3
+    out["gpu_agent_steps_per_s_graphed"] = B * T * n / (out["gpu_ms_per_update_graphed"] / 1e3)
+    if not args.no_cpu:
+        ol = WQMIXLearnerOracle(WQMIXModelOracle(n, od, A, S), keys, agent="CWQMIX", detach_q_eval=False)
+        cdt = cpu_timed(lambda: ol.update(sample), max(args.cpu_iters, 5))
+        out.update(cpu_ms_per_update=cdt * 1e3, cpu_threads=torch.get_num_threads(),
+                   speedup_graphed=cdt * 1e3 / out["gpu_ms_per_update_graphed"])
     return out
 
 
@@ -538,6 +576,8 @@ def main():
     if not only or "qmix" in only:
         res["qmix"] = bench_qmix(args)
         res["qmix_4096"] = bench_qmix(Namespace(**{**vars(args), "iters": 20, "no_cpu": True}), Be=1024)
+    if (not only and WORLD == 1) or "wqmix" in only:
+        res["wqmix"] = bench_wqmix(args)
     if (not only and WORLD == 1) or "ppo_gauss" in only:
         res["ppo_gauss"] = bench_ppo_gauss(args)
     if (not only and WORLD == 1) or "mappo" in only:

@@ -95,6 +95,9 @@ _SIGNATURES = {
     "xb_qmix_mix_bwd": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int, c_int, _P, _P, _P, _P, _P]),
     "xb_qmix_td": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, c_int64, _P, _P, _P, _P]),
     "xb_qmix_mix_fused_fwd": (c_int, [_P] * 10 + [c_int64, c_int, c_int, c_int, c_int, _P, _P]),
+    "xb_wqmix_select_fwd": (c_int, [_P] * 8 + [c_int] * 6 + [_P] * 8),
+    "xb_wqmix_select_bwd": (c_int, [_P] * 6 + [c_int] * 4 + [_P] * 3),
+    "xb_wqmix_loss_fwd_bwd": (c_int, [_P] * 8 + [c_int] * 4 + [c_float, c_float, c_int64] + [_P] * 5),
     "xb_powf_libm": (c_int, [_P, c_float, _P, c_int64, _P]),
 }
 _OPTIONAL = {}

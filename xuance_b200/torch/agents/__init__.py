@@ -17,8 +17,11 @@ try:
 except ImportError:
     pass
 from .marl import MARLAgents, OffPolicyMARLAgents, QMIX_Agents, VDN_Agents
+from .wqmix_agents import WQMIX_Agents
 REGISTRY_Agents["QMIX"] = QMIX_Agents
 REGISTRY_Agents["VDN"] = VDN_Agents
+REGISTRY_Agents["OWQMIX"] = WQMIX_Agents
+REGISTRY_Agents["CWQMIX"] = WQMIX_Agents
 from .mappo_agents import OnPolicyMARLAgents, MAPPO_Agents, IPPO_Agents
 REGISTRY_Agents["MAPPO"] = MAPPO_Agents
 REGISTRY_Agents["IPPO"] = IPPO_Agents

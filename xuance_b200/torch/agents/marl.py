@@ -386,7 +386,7 @@ class QMIX_Agents(OffPolicyMARLAgents):
         return QMIX_Mixer(dim_state=self.state_space.shape[0], dim_hidden=self.config.hidden_dim_mixing_net,
                           dim_hypernet_hidden=self.config.hidden_dim_hyper_net, n_agents=self.n_agents, device=self.device)
 
-    def _build_model(self):
+    def _build_q_networks(self):
         q_networks = nn.ModuleDict()
         for group_key, group_agents in self.groups.items():
             ref = group_agents[0]
@@ -395,6 +395,10 @@ class QMIX_Agents(OffPolicyMARLAgents):
                 representation=enc, action_space=self.action_space[ref], critic_hidden_size=self.config.q_hidden_size,
                 normalizer=self.normalize_fn, initializer=self.initializer, activation=self.activation,
                 device=self.device)
+        return q_networks
+
+    def _build_model(self):
+        q_networks = self._build_q_networks()
         mixer = self._build_mixer()
         return MixingQNetwork(grouping=self.agent_grouping, q_networks=q_networks, mixer=mixer, use_rnn=self.use_rnn,
                               device=self.device).to(self.device)

@@ -132,10 +132,14 @@ class QMIX_Learner(Learner):
         if self.scheduler is not None:
             self.scheduler.step()
         if sync:
-            s = self._stats.tolist()
-            vals = {"learning_rate": self.optimizer.param_groups[0]['lr'], "loss_Q": s[0], "predictQ": s[1]}
+            vals = self._info()
         if self.iterations % self.sync_frequency == 0:
             self.model.copy_target()
         if sync:
             self._finish_info(info, vals, model=self.model)
         return info
+
+    def _info(self):
+        """The logged values of the last update (reads the device statistics: one host synchronisation)."""
+        s = self._stats.tolist()
+        return {"learning_rate": self.optimizer.param_groups[0]['lr'], "loss_Q": s[0], "predictQ": s[1]}

@@ -160,6 +160,28 @@ class QMIX_Mixer(nn.Module):
         return _MixFunction.apply(q, w1, b1, w2, b2, self.n_agents, self.dim_hidden).view(-1, 1)
 
 
+class QMIX_FF_Mixer(nn.Module):
+    """q_mix_head.py:98-140: the unconstrained feed-forward mixer of Weighted QMIX,
+    q_tot = ff_net([q, s]) + ff_net_bias(s).  Its layers are torch Linear layers (cuBLAS GEMMs) with torch's default
+    initialisation, as in the reference."""
+
+    def __init__(self, dim_state=0, dim_hidden=32, n_agents=1, device=None):
+        super().__init__()
+        self.device, self.dim_state, self.dim_hidden, self.n_agents = device, dim_state, dim_hidden, n_agents
+        self.dim_input = n_agents + dim_state
+        self.ff_net = nn.Sequential(nn.Linear(self.dim_input, dim_hidden), nn.ReLU(),
+                                    nn.Linear(dim_hidden, dim_hidden), nn.ReLU(),
+                                    nn.Linear(dim_hidden, dim_hidden), nn.ReLU(),
+                                    nn.Linear(dim_hidden, 1)).to(device)
+        self.ff_net_bias = nn.Sequential(nn.Linear(dim_state, dim_hidden), nn.ReLU(),
+                                         nn.Linear(dim_hidden, 1)).to(device)
+
+    def forward(self, values_n, states=None):
+        states = torch.as_tensor(states, dtype=torch.float32, device=self.device).reshape(-1, self.dim_state)
+        inputs = torch.cat([values_n.reshape(-1, self.n_agents), states], dim=-1)
+        return (self.ff_net(inputs) + self.ff_net_bias(states)).view(-1, 1)
+
+
 class VDN_mixer(nn.Module):
     """q_mix_head.py VDN_mixer: Q_tot = sum_i Q_i (no parameters, the global state is ignored)."""
 
@@ -232,4 +254,40 @@ class MixingQNetwork(nn.Module):
         for ep, tp in zip(self.individual_q_networks.parameters(), self.target_individual_q_networks.parameters()):
             tp.data.copy_(ep)
         for ep, tp in zip(self.eval_Qtot.parameters(), self.target_Qtot.parameters()):
+            tp.data.copy_(ep)
+
+
+class WeightedMixingQNetwork(MixingQNetwork):
+    """value_factorization.py:177-318: MixingQNetwork plus the central agent networks (a deep copy of the agent networks,
+    own GRU, on cuDNN like them), the feed-forward mixer and a target copy of each.  Submodules are registered in the
+    reference's order, so its state_dict loads strictly."""
+
+    def __init__(self, grouping, q_networks, mixer, ff_mixer, use_rnn=True, device=None, **kwargs):
+        super().__init__(grouping, q_networks, mixer, use_rnn=use_rnn, device=device, **kwargs)
+        self.individual_q_centralized = deepcopy(q_networks)
+        self.target_individual_q_centralized = deepcopy(self.individual_q_centralized)
+        self.ff_mixer = ff_mixer
+        self.target_ff_mixer = deepcopy(ff_mixer)
+
+    @property
+    def parameters_model(self):
+        return (list(self.individual_q_networks.parameters()) + list(self.eval_Qtot.parameters())
+                + list(self.individual_q_centralized.parameters()) + list(self.ff_mixer.parameters()))
+
+    def q_centralized(self, packed_obs, target=False):
+        """packed_obs [B*n, T+1, obs] -> central Q [B*n, T+1, A] from a zero initial state."""
+        nets = self.target_individual_q_centralized if target else self.individual_q_centralized
+        return nets[self.group_keys[0]](packed_obs)[0]
+
+    def q_feedforward(self, q_taken, states):
+        return self.ff_mixer(q_taken, states)
+
+    def target_q_feedforward(self, q_taken, states):
+        return self.target_ff_mixer(q_taken, states)
+
+    def copy_target(self):
+        super().copy_target()
+        for ep, tp in zip(self.individual_q_centralized.parameters(), self.target_individual_q_centralized.parameters()):
+            tp.data.copy_(ep)
+        for ep, tp in zip(self.ff_mixer.parameters(), self.target_ff_mixer.parameters()):
             tp.data.copy_(ep)
