@@ -450,10 +450,11 @@ int xb_soft_update(float *target, const float *source, int64_t n, float tau, voi
  * xb_categorical_act: CategoricalDistribution over logits[N,A] (modules/distributions.py:128-162), A <= 64.
  *   forced_actions != NULL : a_n = (int)forced_actions[n]          (log_prob / entropy of given actions)
  *   else uniforms != NULL  : a_n = min{i : u_n < p_0+..+p_i}, u in [0,1) (stochastic_sample; inverse CDF in index order,
- *                            last index if rounding leaves the total mass below u_n)
+ *                            the last index with p_i > 0 if rounding leaves the total mass below u_n: a category
+ *                            of probability zero, e.g. a masked action, is never drawn)
  *   else                   : a_n = first argmax_i p_i               (deterministic_sample)
  *   outputs (each nullable, at least one): actions_f32[N] (the float32 the buffers store), actions_i32[N] (for the
- *   host-side env step), logp[N] = log_softmax(logits)[a], entropy[N] = -sum p log p.
+ *   host-side env step), logp[N] = log_softmax(logits)[a], entropy[N] = -sum p log p over p > 0 (finite for -inf logits).
  * xb_gaussian_act: DiagGaussianDistribution(mu[N,D], exp(log_std[D])) (modules/distributions.py:165-197).
  *   forced_actions != NULL : x = forced_actions[N,D]; actions_f32 is not written (log_prob / entropy of given actions)
  *   else noise != NULL     : x = mu + exp(log_std) * noise, noise[N,D] standard normals (stochastic_sample)
@@ -463,6 +464,8 @@ int xb_soft_update(float *target, const float *source, int64_t n, float tau, voi
  * xb_rms_update_normalize: x[N,D] float32.
  *   update != 0: (mean, var)[D] <- parallel-variance merge with the batch moments, float32 in the reference's operation
  *                order; `count` is the running count BEFORE the merge (host state, Python float in the reference).
+ *                The batch sums run row after row, as NumPy reduces axis 0 of an [N, D > 1] batch; for D = 1 NumPy
+ *                sums the single column pairwise once N >= 8, so there the moments may differ in the last bits.
  *   out != NULL: out = clip((x - mean) / (sqrt(var) + eps), -clip_range, clip_range) with the UPDATED statistics
  *                (PPO_Agent.train calls obs_rms.update(obs) and then _process_observation(obs), ppo_agent.py:115-116).
  */

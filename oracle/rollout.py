@@ -55,7 +55,7 @@ def categorical_terms(logits):
     lse = m + np.log(np.exp(z - m).sum(axis=-1, keepdims=True, dtype=np.float32))
     logp = (z - lse).astype(np.float32)
     p = np.exp(logp)
-    return logp, p, -(p * logp).sum(axis=-1, dtype=np.float32)
+    return logp, p, -np.where(p > 0, p * logp, np.float32(0)).sum(axis=-1, dtype=np.float32)   # 0 * -inf adds nothing
 
 
 def categorical_act(logits, uniforms=None, forced_actions=None):
@@ -73,7 +73,8 @@ def categorical_act(logits, uniforms=None, forced_actions=None):
     elif uniforms is not None:
         u = np.asarray(uniforms, np.float32)[:, None]
         hit = u < cdf
-        a = np.where(hit.any(axis=1), hit.argmax(axis=1), A - 1).astype(np.int64)
+        last_pos = A - 1 - (p > 0)[:, ::-1].argmax(axis=1)     # no prefix passed u: the last category with p > 0
+        a = np.where(hit.any(axis=1), hit.argmax(axis=1), last_pos).astype(np.int64)
     else:
         a = p.argmax(axis=1).astype(np.int64)
     return a, logp[np.arange(N), a], ent, cdf

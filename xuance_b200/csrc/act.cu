@@ -8,10 +8,12 @@
 // K10  xb_categorical_act
 // =====================================================================================================
 // torch.distributions.Categorical(logits=z) semantics (modules/distributions.py:128-162):
-//   logp_i = z_i - logsumexp(z), p_i = exp(logp_i), entropy = -sum p_i logp_i,
+//   logp_i = z_i - logsumexp(z), p_i = exp(logp_i), entropy = -sum over p_i > 0 of p_i logp_i (torch clamps the
+//   log-probability of a zero-probability category, so -inf logits leave the entropy finite),
 //   deterministic_sample = argmax_i p_i (first maximal index),
 //   stochastic sample: inverse CDF over p in index order with the caller's uniform u in [0,1)
-//     a = min{ i : u < p_0 + ... + p_i }   (a = last index if rounding leaves the total below u)
+//     a = min{ i : u < p_0 + ... + p_i }   (a = the last index with p_i > 0 if rounding leaves the total below u:
+//     torch.multinomial never draws a zero-probability category, and masked actions sit at the end of the row)
 // The reference draws with torch.multinomial from torch's RNG; a stream that differs by construction, so parity of the
 // draw is defined on supplied uniforms (as for PER, K5) and parity of logp / entropy on the chosen action.
 template <int A_MAX>
@@ -37,7 +39,7 @@ __global__ void __launch_bounds__(128) categorical_act_kernel(const float *__res
         if (i < A) se += expf(z[i] - m);
     const float lse = m + logf(se);
     float ent = 0.f, cdf = 0.f, best_p = -1.f, lp_a = 0.f, lp_best = 0.f, lp_last = 0.f;
-    int a = -1, best = 0;
+    int a = -1, best = 0, last = A - 1;
     const bool sample = uniforms != nullptr && forced == nullptr;
     const float u = sample ? uniforms[n] : 0.f;
     const int want = forced ? (int)forced[n] : -1;
@@ -46,7 +48,11 @@ __global__ void __launch_bounds__(128) categorical_act_kernel(const float *__res
         if (i < A) {
             const float lp = z[i] - lse;
             const float p = expf(lp);
-            ent -= p * lp;
+            if (p > 0.f) {  // 0 * -inf is NaN; every other zero term leaves ent unchanged
+                ent -= p * lp;
+                last = i;
+                lp_last = lp;
+            }
             cdf += p;
             if (sample && a < 0 && u < cdf) {
                 a = i;
@@ -57,7 +63,6 @@ __global__ void __launch_bounds__(128) categorical_act_kernel(const float *__res
                 best = i;
                 lp_best = lp;
             }
-            lp_last = lp;
             if (i == want) lp_a = lp;
         }
     }
@@ -66,8 +71,8 @@ __global__ void __launch_bounds__(128) categorical_act_kernel(const float *__res
     } else if (!sample) {
         a = best;
         lp_a = lp_best;
-    } else if (a < 0) {  // u >= rounded total mass: the last action
-        a = A - 1;
+    } else if (a < 0) {  // u >= rounded total mass: the last action with positive probability
+        a = last;
         lp_a = lp_last;
     }
     if (act_f) act_f[n] = (float)a;
