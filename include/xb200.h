@@ -330,6 +330,55 @@ int xb_wqmix_loss_fwd_bwd(const float *q_tot, const float *q_ff, const float *q_
                           int B, int n, int T, int mode, float alpha, float gamma, int64_t rows_total, float *dq_tot,
                           float *dq_ff, float *stats, double *scratch, void *stream);
 
+/* ---------------------------------------------------------------- K9C: Deep Coordination Graphs (DCG / DCG_S) --
+ * Replaces, for one parameter-sharing group with use_rnn=True, dcg_learner.py:39-88 (act: max-plus belief propagation
+ * and masked arg-max), :90-104 (q_dcg) and the loss of :161-215 plus its autograd backward down to the head outputs.
+ * Layouts: utility outputs f [B,n,T1,A]; payoff outputs pay [2][B,E,T1,A*A], the two orientations ([h_from,h_to] and
+ * [h_to,h_from], coordination_graph.py:90-101) `payoff_ld` elements apart; edges_from / edges_to int32 [E] (the
+ * graph's edge order); avail (nullable) uint8 [B,n,T1,avail_ld], non-zero = available; actions (taken) [B,n,T] float32
+ * and filled [B,T] as K9.  F_e[i][j] = float32((P0[i*A+j] + P1[j*A+i]) / 2), u_v = f_v / n and F_e / E in float64.
+ * greedy : instance r = b*T + t reads step t0 + t (training: T1 = T+1, t0 = 1; acting: T = T1 = 1, t0 = 0).
+ *          U = (u + 0) + 0, messages m_fwd = m_bwd = 0; n_iter times (none when E = 0), Jacobi:
+ *            m_fwd'[e][j] = max_i ((U[from_e][i] - m_bwd[e][i]) + F_e[i][j]),
+ *            m_bwd'[e][i] = max_j ((U[to_e][j] - m_fwd[e][j]) + F_e[i][j]),
+ *            normalize: m -= (sum_a m[a], summed in action order from 0) / A,
+ *            U[v] = (u_v + sum_{e: to_e = v} m_fwd[e]) + sum_{e: from_e = v} m_bwd[e], both sums in edge order from 0;
+ *          actions[r, v] (int32 [B*T, n]) = the first maximal index of U[v] with unavailable actions at -1e10;
+ *          U_out (nullable) float64 [B*T, n, A] = the final U.  Every operation is one IEEE operation in the order
+ *          above (no FMA contraction; divisions correctly rounded), so a float64 restatement is bit-exact.
+ *          One CTA per instance; shared memory 8*(n*A + 2*E*A + E) bytes, plus 8*E*A*A for a table of F_e formed
+ *          once per instance when n_iter > 1 and the total stays within 48 KB (the same values either way).
+ * q_fwd  : per (b,t) row, q_eval = (sum_v u_v[a_v]) + (sum_e F_e[a_from][a_to]) from f_eval / p_eval at step t and
+ *          the taken actions, q_next the same from f_tgt / p_tgt at step t+1 and greedy [B*T, n]; sums in order from
+ *          0; the payoff sum is dropped unless use_payoff (the reference's E == 0 or n_msg_iterations == 0 rule).
+ *          float64 outputs [B*T]; filled_sum[0] = sum(filled).  Heads are [B,n,T+1,A] / [2][B,E,T+1,A*A].
+ * td     : Q = q_eval (+ V(s)), Q' = q_next (+ V(s')) for DCG_S (v, v_next and dv all given or all NULL);
+ *          r = mean_i rewards (float32), d = all_i terminals, y = r + ((1-d)*gamma in float32)*Q'; td = (Q - y)*filled;
+ *          dq = 2*td*filled/filled_sum (float64 [B*T]), dv = float(dq); stats[2] = {loss_Q = sum(td^2)/filled_sum,
+ *          predictQ = sum(Q)/rows_total (padded rows included)}.  filled_sum and rows_total >= B*T are GLOBAL, so the
+ *          SUM of the shards' outputs is the global result; deterministic two-level reduction, scratch as for K4.
+ * q_bwd  : into pre-zeroed df [B,n,T+1,A] and dp [2][B,E,T+1,A*A] (dp_ld apart; NULL unless use_payoff):
+ *          df[b,v,t,a_v] = float(dq/n); dp0[b,e,t,a_from*A+a_to] = dp1[b,e,t,a_to*A+a_from] = float(dq/E)/2.
+ * All four: n >= 1, A >= 1, E >= 0 and the required pointers (else XB_EINVAL); n <= 32, A <= 64, E <= 512 and the
+ * greedy's shared memory within 227 KB (else XB_ERANGE).  No allocation; graph-capturable. */
+#define XB_DCG_MAX_AGENTS 32
+#define XB_DCG_MAX_ACTIONS 64
+#define XB_DCG_MAX_EDGES 512
+#define XB_DCG_MAX_SMEM (227 * 1024)
+int xb_dcg_greedy(const float *f, const float *payoff, int64_t payoff_ld, const int32_t *edges_from,
+                  const int32_t *edges_to, const uint8_t *avail, int avail_ld, int B, int T, int T1, int t0, int n,
+                  int A, int E, int n_iter, int normalize, int32_t *actions, double *U_out, void *stream);
+int xb_dcg_q_fwd(const float *f_eval, const float *p_eval, int64_t p_eval_ld, const float *f_tgt, const float *p_tgt,
+                 int64_t p_tgt_ld, const float *actions, const int32_t *greedy, const float *filled,
+                 const int32_t *edges_from, const int32_t *edges_to, int B, int n, int T, int A, int E, int use_payoff,
+                 double *q_eval, double *q_next, float *filled_sum, double *scratch, void *stream);
+int xb_dcg_td_fwd_bwd(const double *q_eval, const double *q_next, const float *v, const float *v_next,
+                      const float *rewards, const float *terminals, const float *filled, const float *filled_sum, int B,
+                      int n, int T, float gamma, int64_t rows_total, double *dq, float *dv, float *stats,
+                      double *scratch, void *stream);
+int xb_dcg_q_bwd(const double *dq, const float *actions, const int32_t *edges_from, const int32_t *edges_to, int B,
+                 int n, int T, int A, int E, int use_payoff, float *df, float *dp, int64_t dp_ld, void *stream);
+
 /* Tensor-core forward of the whole mixer (hypernet GEMMs + epilogue in ONE kernel; wgmma with register
  * accumulators, bf16 hi/lo split operands, 3 MMAs per product, fp32 accumulate): q_tot[R] from states[R,S], q[R,n]
  * and the raw Linear parameters of QMIX_Mixer (q_mix_head.py:52-64): w_l1[4] / b_l1[4] are HOST arrays of 4 device

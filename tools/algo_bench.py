@@ -5,7 +5,8 @@ on one GPU, next to the oracle port of the reference's torch-CPU path on the hos
 PPO in the shape of the reference's ppo/mujoco.yaml (train_epochs env-steps/s); ``mappo``, MAPPO in the shape of
 configs/mappo/sc2/5m_vs_6m.yaml (train_epochs env-steps/s); ``mappo_rnn``, recurrent MAPPO in the shape of
 configs/mappo/sc2/3m.yaml (update, eager and graphed); ``wqmix``, CW-QMIX in the shape of configs/wqmix/sc2/5m_vs_6m.yaml
-(update, eager and graphed); ``sacdis``, SAC-Discrete in the shape of
+(update, eager and graphed); ``dcg``, DCG in the shape of configs/dcg/sc2/5m_vs_6m.yaml (update, eager and graphed);
+``sacdis``, SAC-Discrete in the shape of
 configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (train_epochs, eager and graphed); ``ddpg`` and
 ``td3``, DDPG / TD3 in the shape of the reference's ddpg/mujoco.yaml and td3/mujoco.yaml (sample + update, eager and
 graphed); ``c51`` and ``qrdqn`` on CartPole (Basic_MLP 128, B=256) and SyntheticAtari (Basic_CNN, B=32) shapes (update,
@@ -223,6 +224,56 @@ def bench_wqmix(args, B=32):
     out["gpu_agent_steps_per_s_graphed"] = B * T * n / (out["gpu_ms_per_update_graphed"] / 1e3)
     if not args.no_cpu:
         ol = WQMIXLearnerOracle(WQMIXModelOracle(n, od, A, S), keys, agent="CWQMIX", detach_q_eval=False)
+        cdt = cpu_timed(lambda: ol.update(sample), max(args.cpu_iters, 5))
+        out.update(cpu_ms_per_update=cdt * 1e3, cpu_threads=torch.get_num_threads(),
+                   speedup_graphed=cdt * 1e3 / out["gpu_ms_per_update_graphed"])
+    return out
+
+
+def bench_dcg(args, B=32):
+    """One DCG_Learner update in the shape of configs/dcg/sc2/5m_vs_6m.yaml (5 agents x 72-d, A=12, T=60, 32 episodes, K13
+    GRU 64, utility / payoff heads 64, FULL graph: E = 10, 8 normalised message iterations, action masks), eager and
+    graphed, on a device-resident sample; next to the torch-CPU oracle of the same update."""
+    import dcg_refs
+    import wqmix_refs as R
+    from oracle_dcg import DCGModelOracle, DCGLearnerOracle
+    import torch.nn as nn
+    from xuance_b200.common import AgentGrouping, BaseCallback, Discrete
+    from xuance_b200.torch.learners import REGISTRY_Learners
+    from xuance_b200.torch.rl_models import (AgentFeatureEncoder, Basic_RNN_K13, DCG_Utility, DCG_Payoff,
+                                             Coordination_Graph, DeepCoordinationGraph)
+    n, od, A, T = 5, 72, 12, 60
+
+    def product_model(H=64):
+        rep = Basic_RNN_K13(input_shape=(od,), initialize=nn.init.orthogonal_, activation=nn.ReLU, device=DEV,
+                            fc_hidden_sizes=[H], recurrent_hidden_size=H)
+        g = Coordination_Graph(n, "FULL", DEV)
+        g.set_coordination_graph()
+        grouping = AgentGrouping.shared(keys)
+        model = DeepCoordinationGraph(grouping, {k: Discrete(A) for k in keys},
+                                      nn.ModuleDict({'shared': AgentFeatureEncoder(rep)}), DCG_Utility(H, H, A, DEV),
+                                      DCG_Payoff(2 * H, H, A, False, 1, DEV), g, use_rnn=True, device=DEV).to(DEV)
+        return grouping, model
+
+    keys = [f"agent_{i}" for i in range(n)]
+    sample = R.fix_sample(np.random.default_rng(0), keys, B=B, T=T, obs_dim=od, A=A, S=4)
+    dev = lambda x: {k: dev(v) for k, v in x.items()} if isinstance(x, dict) else (
+        torch.as_tensor(x, device=DEV) if isinstance(x, np.ndarray) else x)
+    dsample = dev(sample)
+    out = {"config": f"DCG, 5 agents x 72-d, A=12, T=60, {B} episodes/update, GRU 64, heads 64, FULL graph (E=10), "
+                     f"8 normalised iterations, action masks"}
+    for graph in (False, True):
+        torch.manual_seed(0)
+        grouping, model = product_model()
+        cfg = Namespace(agent="DCG", distributed_training=False, episode_length=T, use_grad_clip=False,
+                        grad_clip_norm=0.5, device=DEV, model_dir="/tmp/x", running_steps=10**7, parallels=8,
+                        use_parameter_sharing=True, use_rnn=True, use_actions_mask=True, learning_rate=7e-4,
+                        sync_frequency=200, n_epochs=1, start_training=0, gamma=0.99, use_cuda_graph=graph)
+        lrn = REGISTRY_Learners["DCG_Learner"](cfg, grouping, model, BaseCallback())
+        dt = timed(lambda: lrn.update(dsample, sync=False), args.iters)
+        out["gpu_ms_per_update_graphed" if graph else "gpu_ms_per_update_eager"] = dt * 1e3
+    if not args.no_cpu:
+        ol = DCGLearnerOracle(DCGModelOracle(n, od, A), keys, dcg_refs.graph_edges(n, "FULL"))
         cdt = cpu_timed(lambda: ol.update(sample), max(args.cpu_iters, 5))
         out.update(cpu_ms_per_update=cdt * 1e3, cpu_threads=torch.get_num_threads(),
                    speedup_graphed=cdt * 1e3 / out["gpu_ms_per_update_graphed"])
@@ -578,6 +629,8 @@ def main():
         res["qmix_4096"] = bench_qmix(Namespace(**{**vars(args), "iters": 20, "no_cpu": True}), Be=1024)
     if (not only and WORLD == 1) or "wqmix" in only:
         res["wqmix"] = bench_wqmix(args)
+    if (not only and WORLD == 1) or "dcg" in only:
+        res["dcg"] = bench_dcg(args)
     if (not only and WORLD == 1) or "ppo_gauss" in only:
         res["ppo_gauss"] = bench_ppo_gauss(args)
     if (not only and WORLD == 1) or "mappo" in only:

@@ -372,6 +372,8 @@ def main():
                       xp_.numel() * 2 + g3.numel() * 2, hbm, 2.0 * B * 100 * 64 * K, tpk))
     if want("k13"):
         out["k13"] = k13_bench(R, hbm)
+    if want("dcg"):
+        out["dcg"] = dcg_bench(R)
     print(json.dumps(out))
 
 
@@ -434,6 +436,63 @@ def _k13_bench(R):
                                          and not e.key.startswith(("Memcpy", "Memset")))
         except Exception as exc:     # the timing above stands without the count
             res[name + "_kernels"] = "profiler failed: %s" % exc
+    return res
+
+
+def dcg_bench(R):
+    """K9C xb_dcg_greedy in the shape of configs/dcg/sc2/5m_vs_6m.yaml (5 agents, FULL graph: E = 10, A = 12, 8
+    normalised iterations, action masks) at R = 1920 instances (one training update: 32 episodes x 60 steps) and R = 8
+    (one acting step of 8 environments), against the reference's act() loop (dcg_learner.py:49-88) restated in torch on
+    the same GPU (float64, scatter sums by index_add_)."""
+    import subprocess
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import dcg_refs
+    res = {}
+    try:
+        res["gpu"] = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm",
+                                     "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    except OSError:
+        res["gpu"] = "nvidia-smi unavailable"
+    n, A, it = 5, 12, 8
+    edges = dcg_refs.graph_edges(n, "FULL")
+    E = len(edges)
+    fr = torch.tensor([e[0] for e in edges], dtype=torch.int32, device=DEV)
+    to = torch.tensor([e[1] for e in edges], dtype=torch.int32, device=DEV)
+    frl, tol = fr.long(), to.long()
+    for Rn in (1920, 8):
+        torch.manual_seed(0)
+        f = torch.randn(Rn, n, 1, A, device=DEV)
+        pay = torch.randn(2, Rn, E, 1, A * A, device=DEV)
+        avail = (torch.rand(Rn, n, 1, A, device=DEV) < 0.7).to(torch.uint8)
+        avail[..., 0] = 1
+        acts = torch.empty(Rn, n, dtype=torch.int32, device=DEV)
+        k = lambda: _lib.call("xb_dcg_greedy", _lib.ptr(f), _lib.ptr(pay), pay[0].numel(), _lib.ptr(fr), _lib.ptr(to),
+                              _lib.ptr(avail), A, Rn, 1, 1, 0, n, A, E, it, 1, _lib.ptr(acts), None)
+
+        def loop():
+            P = pay.reshape(2, Rn, E, A, A).clone()
+            P[1] = P[1].transpose(-1, -2).clone()
+            f_ij = P.mean(dim=0).double() / E
+            f_ji = f_ij.transpose(-1, -2).clone()
+            f_i = f.reshape(Rn, n, A).double() / n
+            scat = lambda src, idx: torch.zeros(Rn, n, A, dtype=torch.float64, device=DEV).index_add_(1, idx, src)
+            m_ij = torch.zeros(Rn, E, A, dtype=torch.float64, device=DEV)
+            m_ji = torch.zeros(Rn, E, A, dtype=torch.float64, device=DEV)
+            U = f_i + scat(m_ij, tol) + scat(m_ji, frl)
+            for _ in range(it):
+                jf = (U[:, frl, :] - m_ji).unsqueeze(-1) + f_ij          # both from the old messages (Jacobi)
+                jb = (U[:, tol, :] - m_ij).unsqueeze(-1) + f_ji
+                m_ij, m_ji = jf.max(dim=-2).values, jb.max(dim=-2).values
+                m_ij = m_ij - m_ij.mean(dim=-1, keepdim=True)
+                m_ji = m_ji - m_ji.mean(dim=-1, keepdim=True)
+                U = f_i + scat(m_ij, tol) + scat(m_ji, frl)
+            U = U.clone()
+            U[avail.reshape(Rn, n, A) == 0] = -1e10
+            return U.argmax(dim=-1)
+
+        res[f"R{Rn}_xb_dcg_greedy_us"] = round(timeit(k, R, flush=False), 2)
+        res[f"R{Rn}_torch_loop_us"] = round(timeit(loop, R, flush=False), 2)
+        res[f"R{Rn}_speedup"] = round(res[f"R{Rn}_torch_loop_us"] / res[f"R{Rn}_xb_dcg_greedy_us"], 2)
     return res
 
 

@@ -98,6 +98,10 @@ _SIGNATURES = {
     "xb_wqmix_select_fwd": (c_int, [_P] * 8 + [c_int] * 6 + [_P] * 8),
     "xb_wqmix_select_bwd": (c_int, [_P] * 6 + [c_int] * 4 + [_P] * 3),
     "xb_wqmix_loss_fwd_bwd": (c_int, [_P] * 8 + [c_int] * 4 + [c_float, c_float, c_int64] + [_P] * 5),
+    "xb_dcg_greedy": (c_int, [_P, _P, c_int64, _P, _P, _P] + [c_int] * 10 + [_P, _P, _P]),
+    "xb_dcg_q_fwd": (c_int, [_P, _P, c_int64, _P, _P, c_int64] + [_P] * 5 + [c_int] * 6 + [_P] * 5),
+    "xb_dcg_td_fwd_bwd": (c_int, [_P] * 8 + [c_int] * 3 + [c_float, c_int64] + [_P] * 5),
+    "xb_dcg_q_bwd": (c_int, [_P] * 4 + [c_int] * 6 + [_P, _P, c_int64, _P]),
     "xb_powf_libm": (c_int, [_P, c_float, _P, c_int64, _P]),
 }
 _OPTIONAL = {}

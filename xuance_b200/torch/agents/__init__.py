@@ -22,6 +22,9 @@ REGISTRY_Agents["QMIX"] = QMIX_Agents
 REGISTRY_Agents["VDN"] = VDN_Agents
 REGISTRY_Agents["OWQMIX"] = WQMIX_Agents
 REGISTRY_Agents["CWQMIX"] = WQMIX_Agents
+from .dcg_agents import DCG_Agents
+REGISTRY_Agents["DCG"] = DCG_Agents
+REGISTRY_Agents["DCG_S"] = DCG_Agents
 from .mappo_agents import OnPolicyMARLAgents, MAPPO_Agents, IPPO_Agents
 REGISTRY_Agents["MAPPO"] = MAPPO_Agents
 REGISTRY_Agents["IPPO"] = IPPO_Agents

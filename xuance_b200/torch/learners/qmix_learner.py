@@ -59,15 +59,19 @@ class QMIX_Learner(Learner):
         self.detach_q_eval = getattr(config, "qmix_rnn_detach_q_eval", False)
         self.use_actions_mask = getattr(config, "use_actions_mask", False)
         # LearnerMAS.build_optimizer (marl_learner.py:64-76): one Adam(eps=1e-5) + LinearLR over the trainable set
-        self.optimizer = FusedAdam(self.model.parameters_model, lr=self.learning_rate, eps=1e-5,
-                                   weight_decay=getattr(config, "weight_decay", 0.0),
-                                   front=cudnn_rnn_front(self.model.individual_q_networks))
+        self.optimizer = self._build_optimizer()
         self.scheduler = self._linear_lr(self.optimizer)
         dev = self.device
         self._filled_sum = torch.zeros(1, dtype=torch.float32, device=dev)
         self._stats = self.optimizer.bucket.tail[:2]       # logged sums ride in the gradient all-reduce (bucket tail)
         self._scratch = _lib.scratch(dev)
         self._graph_tensors = [self._filled_sum]
+
+    def _build_optimizer(self):
+        """One FusedAdam over ``parameters_model``, the cuDNN GRU weights first in the bucket (cudnn_rnn_front)."""
+        return FusedAdam(self.model.parameters_model, lr=self.learning_rate, eps=1e-5,
+                         weight_decay=getattr(self.config, "weight_decay", 0.0),
+                         front=cudnn_rnn_front(self.model.individual_q_networks))
 
     def estimate_total_iterations(self):
         """marl_learner.py:37-47."""
@@ -86,14 +90,20 @@ class QMIX_Learner(Learner):
         u8 = lambda x: torch.as_tensor(x, device=self.device).to(torch.uint8).contiguous()
         if '_stacked' in sample:
             st = sample['_stacked']
-            out = {k: f32(st[k]) for k in ('obs', 'actions', 'rewards', 'terminals', 'agent_mask', 'filled', 'state')}
+            out = {k: f32(st[k]) for k in ('obs', 'actions', 'rewards', 'terminals', 'agent_mask', 'filled')}
+            out['state'] = f32(st['state']) if self._uses_global_state() else None
             out['avail'] = u8(st['avail_actions']) if self.use_actions_mask else None
             return out
         stack = lambda d: torch.stack([torch.as_tensor(d[a], device=self.device) for a in self.agent_keys], dim=1)
         out = {k: f32(stack(sample[k])) for k in ('obs', 'actions', 'rewards', 'terminals', 'agent_mask')}
-        out['filled'], out['state'] = f32(sample['filled']), f32(sample['state'])
+        out['filled'] = f32(sample['filled'])
+        out['state'] = f32(sample['state']) if self._uses_global_state() else None
         out['avail'] = u8(stack(sample['avail_actions'])) if self.use_actions_mask else None
         return out
+
+    def _uses_global_state(self):
+        """Whether the update reads the global state (the mixers do; a learner whose replay keeps none says False)."""
+        return True
 
     def _device_update(self, obs, actions, rewards, terminals, agent_mask, filled, state, avail=None):
         """qmix_learner.py:24-95 on the device (no host synchronisation, static shapes: CUDA-graph capturable)."""
