@@ -379,6 +379,74 @@ int xb_dcg_td_fwd_bwd(const double *q_eval, const double *q_next, const float *v
 int xb_dcg_q_bwd(const double *dq, const float *actions, const int32_t *edges_from, const int32_t *edges_to, int B,
                  int n, int T, int A, int E, int use_payoff, float *df, float *dp, int64_t dp_ld, void *stream);
 
+/* ---------------------------------------------------------------- K9Q: QTRAN (QTRAN_base / QTRAN_alt) --
+ * Replaces, for one parameter-sharing group with use_rnn=True, qtran_learner.py:199-371 (update_rnn) except the Q_jt
+ * and V_jt MLPs (cuBLAS through torch), with the action-encoding part of Q_tran / Q_tran_target
+ * (value_factorization.py:354-442, q_mix_head.py:191-211 and :264-292) and the autograd backward of all of it.
+ * Layouts as K9: heads q_all / q_tgt [B,n,T+1,A]; actions, agent_mask (m), rewards, terminals [B,n,T] and filled (f)
+ * [B,T] float32; avail (nullable) uint8 [B,n,T+1,avail_ld], non-zero = available; rows r = b*T + t, R = B*T.
+ * Unavailable actions count as -1e10 in every arg-max; every arg-max and arg-min takes the first extreme index.
+ * select : greedy [B,n,T+1] int32 = the masked arg-max of q_all at every step; next [B,n,T] int32 = greedy at t+1 when
+ *          double_q, else the arg-max of q_tgt at t+1 with the step-(t+1) mask (q_tgt may be NULL when double_q);
+ *          filled_sum[0] = sum(filled).
+ * encode_fwd: D = H + A; for agent i of row r, u_i = [h[b,i,t]*m, onehot(a_i)] (the one-hot is not masked) and
+ *          e_i = W2 relu(W1 u_i + b1) + b2 (the one-hot product is the column W1[:, H+a_i]).  h [B,n,T+1,H] is read at
+ *          steps 0..T-1, the state [B,T+1,S] at step state_t0 + t (0 or 1), the actions from exactly one of act_f
+ *          (float32) and act_i (int32), [B,n,act_T], act_T >= T.  W1, W2 [D,D], b1, b2 [D] (nn.Linear layout).
+ *          mode XB_QTRAN_BASE: x[r] = [state, sum_i e_i], width S+D;  XB_QTRAN_ALT: x[r*n+i] = [state,
+ *          (n-1) e_i, onehot_n(i)], width S+D+n: e_i added n-1 times, as q_mix_head.py:283-285 computes it (the
+ *          mask drops one repeat of agent i's own encoding, not agent i).  Sums run in agent order.
+ *          Actions must lie in [0, A) (the reference's F.one_hot raises otherwise); an action outside it contributes no
+ *          one-hot column here, and to xb_qtran_loss_fwd_bwd it is an out-of-bounds index.  pre (nullable) [R,n,D] = W1 u_i + b1.
+ *          Shared memory 4*(2*D*D + 4*D + n*D) bytes.
+ * encode_bwd: dx as x (the state and id columns carry no gradient); ge_j = dx's encoding columns of row r (base) or
+ *          those of agent-row (r,j) added n-1 times (alt); dz_j = (W2^T ge_j) * (pre > 0); dh[b,j,t] = m * W1[:, :H]^T dz_j
+ *          (step T written as zero); dW1 = sum dz_j u_j^T (the one-hot columns a scatter by action), db1 = sum dz_j,
+ *          dW2 = sum ge_j relu(pre_j)^T, db2 = sum ge_j.  The weight gradients are partial sums over fixed chunks of
+ *          max(128, ceil(R*n/1024)) agent-rows in row order, then added in chunk order: bit-identical from launch to
+ *          launch.  work holds xb_qtran_encode_bwd_work(B, n, T, H, A) = 2*R*n*D + chunks*(2*D*D + 2*D) floats
+ *          (XB_EINVAL if work_floats is smaller): ge and dz1 for every agent-row plus at most 1024 partials, about
+ *          9 MB at B = 32, T = 60, n = 5, H = 64, A = 12 and linear in R*n (2.1 GB at B = 1024, T = 60, n = 32, A = 64,
+ *          the same order as alt's x there).
+ * loss   : r = mean_i rewards, d = all_i terminals (as xb_qmix_td); Q_tot = sum_i q_all[t, a_i]*m and Q_tot_g =
+ *          sum_i q_all[t, g_i]*m (g = greedy at t), in agent order; V = v [R].
+ *          base: qjt, qjt_greedy, qjt_next [R]; y = r + (1-d)*gamma*qjt_next; td = (qjt - y)*f; eo = (Q_tot_g -
+ *          qjt_greedy + V)*f; en = min(Q_tot - qjt + V, 0)*f; den = filled_sum.
+ *          alt: qjt, qjt_greedy, qjt_next [R*n, A]; per (r,i): y = r + (1-d)*gamma*qjt_next[r,i,next_i]; td =
+ *          (qjt[r,i,a_i] - y)*f; eo = (Q_tot_g - qjt_greedy[r,i,g_i] + V)*f; en = min_a (q_all[i,t,a] + sum_{j != i}
+ *          q_all[j,t,a_j]*m_j - qjt[r,i,a] + V)*f over the unmasked row; den = n*filled_sum.
+ *          Each loss is sum(term^2)/den.  Writes dqjt (TD only: qjt is detached in opt and nopt; alt writes whole rows),
+ *          dv [R], and scatters the opt and nopt gradients into pre-zeroed dq_all [B,n,T+1,A] (taken, greedy and, for
+ *          alt, the arg-min entries; coinciding entries add).  stats[5] = {loss_td, loss_opt, loss_nopt, loss =
+ *          loss_td + lambda_opt*loss_opt + lambda_nopt*loss_nopt, Q_joint = sum of the taken qjt / (rows_total, times n
+ *          for alt), padded rows included}.  filled_sum and rows_total >= R are GLOBAL, so the SUM of the shards'
+ *          outputs is the global result; deterministic two-level reduction, scratch as for K4.
+ * All: B, n, T, A (and S, H for the encoder) >= 1, mode in {BASE, ALT} and the required pointers (else XB_EINVAL);
+ * n <= 32, A <= 64, H <= 64 (else XB_ERANGE).  No allocation; graph-capturable. */
+#define XB_QTRAN_BASE 0
+#define XB_QTRAN_ALT 1
+#define XB_QTRAN_MAX_AGENTS 32
+#define XB_QTRAN_MAX_ACTIONS 64
+#define XB_QTRAN_MAX_HIDDEN 64
+int xb_qtran_select(const float *q_all, const float *q_tgt, const uint8_t *avail, int avail_ld, const float *filled,
+                    int B, int n, int T, int A, int double_q, int32_t *greedy, int32_t *next, float *filled_sum,
+                    double *scratch, void *stream);
+int xb_qtran_encode_fwd(int mode, const float *state, int state_t0, const float *h, const float *agent_mask,
+                        const float *act_f, const int32_t *act_i, int act_T, const float *w1, const float *b1,
+                        const float *w2, const float *b2, int B, int n, int T, int S, int H, int A, float *x,
+                        float *pre, void *stream);
+int64_t xb_qtran_encode_bwd_work(int B, int n, int T, int H, int A);
+int xb_qtran_encode_bwd(int mode, const float *dx, const float *h, const float *agent_mask, const float *act_f,
+                        const int32_t *act_i, int act_T, const float *w1, const float *w2, const float *pre, int B,
+                        int n, int T, int S, int H, int A, float *dh, float *dw1, float *db1, float *dw2, float *db2,
+                        float *work, int64_t work_floats, void *stream);
+int xb_qtran_loss_fwd_bwd(int mode, const float *q_all, const float *actions, const int32_t *greedy,
+                          const int32_t *next, const float *agent_mask, const float *filled, const float *rewards,
+                          const float *terminals, const float *qjt, const float *qjt_greedy, const float *qjt_next,
+                          const float *v, const float *filled_sum, int B, int n, int T, int A, float gamma,
+                          float lambda_opt, float lambda_nopt, int64_t rows_total, float *dqjt, float *dv,
+                          float *dq_all, float *stats, double *scratch, void *stream);
+
 /* Tensor-core forward of the whole mixer (hypernet GEMMs + epilogue in ONE kernel; wgmma with register
  * accumulators, bf16 hi/lo split operands, 3 MMAs per product, fp32 accumulate): q_tot[R] from states[R,S], q[R,n]
  * and the raw Linear parameters of QMIX_Mixer (q_mix_head.py:52-64): w_l1[4] / b_l1[4] are HOST arrays of 4 device

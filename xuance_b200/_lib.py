@@ -102,6 +102,11 @@ _SIGNATURES = {
     "xb_dcg_q_fwd": (c_int, [_P, _P, c_int64, _P, _P, c_int64] + [_P] * 5 + [c_int] * 6 + [_P] * 5),
     "xb_dcg_td_fwd_bwd": (c_int, [_P] * 8 + [c_int] * 3 + [c_float, c_int64] + [_P] * 5),
     "xb_dcg_q_bwd": (c_int, [_P] * 4 + [c_int] * 6 + [_P, _P, c_int64, _P]),
+    "xb_qtran_select": (c_int, [_P, _P, _P, c_int, _P] + [c_int] * 5 + [_P] * 5),
+    "xb_qtran_encode_fwd": (c_int, [c_int, _P, c_int, _P, _P, _P, _P, c_int] + [_P] * 4 + [c_int] * 6 + [_P] * 3),
+    "xb_qtran_encode_bwd_work": (c_int64, [c_int] * 5),
+    "xb_qtran_encode_bwd": (c_int, [c_int] + [_P] * 5 + [c_int] + [_P] * 3 + [c_int] * 6 + [_P] * 6 + [c_int64, _P]),
+    "xb_qtran_loss_fwd_bwd": (c_int, [c_int] + [_P] * 13 + [c_int] * 4 + [c_float] * 3 + [c_int64] + [_P] * 6),
     "xb_powf_libm": (c_int, [_P, c_float, _P, c_int64, _P]),
 }
 _OPTIONAL = {}

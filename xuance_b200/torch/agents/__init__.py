@@ -25,6 +25,9 @@ REGISTRY_Agents["CWQMIX"] = WQMIX_Agents
 from .dcg_agents import DCG_Agents
 REGISTRY_Agents["DCG"] = DCG_Agents
 REGISTRY_Agents["DCG_S"] = DCG_Agents
+from .qtran_agents import QTRAN_Agents
+REGISTRY_Agents["QTRAN_base"] = QTRAN_Agents
+REGISTRY_Agents["QTRAN_alt"] = QTRAN_Agents
 from .mappo_agents import OnPolicyMARLAgents, MAPPO_Agents, IPPO_Agents
 REGISTRY_Agents["MAPPO"] = MAPPO_Agents
 REGISTRY_Agents["IPPO"] = IPPO_Agents

@@ -8,6 +8,7 @@ from .ddpg_learner import DDPG_Learner, TD3_Learner
 from .qmix_learner import QMIX_Learner
 from .wqmix_learner import WQMIX_Learner
 from .dcg_learner import DCG_Learner
+from .qtran_learner import QTRAN_Learner
 from .mappo_learner import MAPPO_Learner
 from .ppg_learner import PPG_Learner
 
@@ -20,4 +21,4 @@ REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner,
                      "QMIX_Learner": QMIX_Learner,
                      "VDN_Learner": QMIX_Learner,     # vdn_learner.py: the same update with the parameter-free sum mixer
                      "MAPPO_Learner": MAPPO_Learner, "PPG_Learner": PPG_Learner, "WQMIX_Learner": WQMIX_Learner,
-                     "DCG_Learner": DCG_Learner}
+                     "DCG_Learner": DCG_Learner, "QTRAN_Learner": QTRAN_Learner}

@@ -15,3 +15,4 @@ REGISTRY_Representation["Basic_RNN"] = Basic_RNN
 from .mappo import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic
 from .gru import GRUSequence, gru_sequence, Basic_RNN_K13
 from .dcg import DCG_Utility, DCG_Payoff, Coordination_Graph, DeepCoordinationGraph
+from .qtran import QTRAN_Base, QTRAN_Alt, QTranMixingNetwork
