@@ -127,11 +127,16 @@ def test_continuous_action_replay():
 @pytest.mark.parametrize("alpha", [0.5, 0.6, 0.4, 1.0, 0.25])
 def test_powf_restatement_bit_exact(alpha):
     """The device restatement of glibc powf == numpy's float32 ** python-float (what the reference evaluates for
-    every PER leaf, memory_tools.py:547,596) on 200k priorities incl. tiny / huge / exact-power-of-two inputs."""
+    every PER leaf, memory_tools.py:547,596) on 200k priorities incl. tiny / huge / exact-power-of-two inputs, and one
+    value from every binade from 2^-149 (subnormal) to 2^127 plus both ends of each."""
     from xuance_b200 import _lib
     rng = np.random.default_rng(int(alpha * 100))
     p = np.abs(rng.normal(size=200_000)).astype(np.float32) * np.float32(3.0) + np.float32(1e-8)
     p[:8] = np.array([1e-8, 1.0, 2.0, 0.5, 1e-3, 1e3, 7.0, 0.3333333], np.float32)
+    e = np.arange(-149, 128)
+    binades = np.concatenate([np.ldexp(rng.uniform(1.0, 1.99, e.size), e), np.ldexp(1.0, e),
+                              np.ldexp(2.0 - 2.0 ** -23, e)]).astype(np.float32)
+    p = np.concatenate([p, binades[binades > 0]])
     want = np.array([x ** alpha for x in p], dtype=np.float32)      # numpy scalar power -> libm powf
     d = torch.from_numpy(p).cuda()
     out = torch.empty_like(d)

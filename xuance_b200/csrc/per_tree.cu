@@ -39,8 +39,14 @@ __constant__ unsigned long long EXP2F_TAB[32] = {
     0x3fef5818dcfba487ull, 0x3fef7c97337b9b5full, 0x3fefa4afa2a490daull, 0x3fefd0765b6e4540ull,
 };
 __device__ __forceinline__ float powf_libm(float x, float y) {
-    const uint32_t ix = __float_as_uint(x);
-    if (ix - 0x00800000u >= 0x7f800000u - 0x00800000u) return powf(x, y);  // zero/subnormal/negative/inf/nan
+    uint32_t ix = __float_as_uint(x);
+    if (ix - 0x00800000u >= 0x7f800000u - 0x00800000u) {   // zero, subnormal, negative, inf or nan
+        if (ix == 0u || ix >= 0x7f800000u) return powf(x, y);  // zero/negative/inf/nan: not on the PER path
+        // subnormal: normalised as glibc does, x * 2^23 with the exponent lowered by 23 (it goes negative; the
+        // unsigned wrap cancels in iz = ix - top below)
+        ix = __float_as_uint(__fmul_rn(x, 0x1p23f)) & 0x7fffffffu;
+        ix -= 23u << 23;
+    }
     // log2(x) = log1p(z/c - 1)/ln2 + log2(c) + k
     const uint32_t tmp = ix - 0x3f330000u;
     const int i = (tmp >> 19) & 15;
@@ -61,7 +67,11 @@ __device__ __forceinline__ float powf_libm(float x, float y) {
     q = __fma_rn(pp, r2, q);
     yy = __fma_rn(yy, r4, q);
     const double ylogx = __dmul_rn((double)y, yy);
-    if (fabs(ylogx) >= 126.0) return powf(x, y);  // overflow / underflow handling is not on the PER path
+    if (fabs(ylogx) >= 126.0) {   // glibc's special cases; the rest of this range takes the exp2 path below
+        if (ylogx > 0x1.fffffffd1d571p+6) return __uint_as_float(0x7f800000u);   // x^y rounds to inf
+        if (ylogx <= -150.0) return 0.f;                                          // x^y rounds to 0
+        if (ylogx < -149.0) return 0x1p-149f;                                     // glibc's __math_may_uflowf
+    }
     // exp2(ylogx): x = k/N + r, N = 32
     const double SHIFT = 0x1.8p+47;
     double kd = __dadd_rn(ylogx, SHIFT);

@@ -13,8 +13,13 @@
 //
 // Numerics: the reference computes these layers in fp32.  The tensor pipe takes bf16 here, so every fp32 operand is
 // split x = hi + lo (two bf16 values, |x - hi - lo| <= 2^-16 |x|) and each product is the sum of the three MMAs
-// hi.hi + hi.lo + lo.hi (lo.lo <= 2^-16 relative, the size of the split residual itself) accumulated in fp32: relative error ~1e-5 per layer (a plain bf16 or TF32
-// pass would be ~4e-3 / ~5e-4).  tests/test_gpu_qmix.py pins it against the fp32 oracle.
+// hi.lo + lo.hi + hi.hi (lo.lo <= 2^-16 relative, the size of the split residual itself) accumulated in fp32: relative error
+// ~1e-5 per layer (a plain bf16 or TF32 pass would be ~4e-3 / ~5e-4).  The tensor core truncates each 16-deep block it
+// adds into the accumulator, so the two corrections are issued before the hi.hi chain: their truncation happens at 2^-8
+// of the final magnitude, and hi.hi sees KP/16 full-size adds instead of three times as many.  That cut the measured bias
+// of q_tot (mean signed error over 2^17 rows, in units of the first-order bound) from -3.8e-5 to -1.5e-5 on an H100 SXM
+// (700 W); the rest comes from the hi.hi chain, which one accumulator cannot avoid.  tests/test_gpu_qmix_tc_edges.py
+// pins it against the float64 mixer of tests/qmix_tc_refs.py, with that bias and at the edge shapes.
 #include "tc_common.cuh"
 
 namespace {
@@ -145,20 +150,23 @@ __global__ void __launch_bounds__(TC_THREADS, 1) qmix_mix_tc_kernel(TcParams p) 
                 bulk_g2s(Xraw, p.states + nt * TC_ROWS * S, tile_copy_bytes(nt), &x_bar);
             }
         }
-        // ---- GEMM1: Z[64 x 128] per warpgroup, products (hi,hi) (hi,lo) (lo,hi); lo.lo <= 2^-16 relative is dropped
+        // ---- GEMM1: Z[64 x 128] per warpgroup, products (hi,lo) (lo,hi) (hi,hi); lo.lo <= 2^-16 relative is dropped.
+        // The corrections go first (pp = 0, 1: (pa, pb) = (0, 1), (1, 0)): the tensor core truncates each block it adds
+        // into the accumulator, and so they are truncated at 2^-8 of the final magnitude, not at its full size
         float z[4][16];
         wgmma_fence();
         {
             const uint32_t as[2] = {a1h, a1l}, bs[2] = {smem_u32(B1h), smem_u32(B1l)};
             uint32_t acc = 0;
-            for (int pa = 0; pa < 2; ++pa)
-                for (int pb = 0; pb < 2 - pa; ++pb)
-                    for (int ks = 0; ks < KP1 / 16; ++ks) {   // one MMA = K 16 = two core matrices = 256 B along K
-                        const uint64_t da = make_desc(as[pa] + ks * 256, KP1);
-                        wgmma_n64<0, 0>(z[0], z[1], da, make_desc(bs[pb] + ks * 256, KP1), acc);
-                        wgmma_n64<0, 0>(z[2], z[3], da, make_desc(bs[pb] + 64 * KP1 * 2 + ks * 256, KP1), acc);
-                        acc = 1;
-                    }
+            for (int pp = 0; pp < 3; ++pp) {
+                const int pa = pp == 1, pb = pp == 0;
+                for (int ks = 0; ks < KP1 / 16; ++ks) {   // one MMA = K 16 = two core matrices = 256 B along K
+                    const uint64_t da = make_desc(as[pa] + ks * 256, KP1);
+                    wgmma_n64<0, 0>(z[0], z[1], da, make_desc(bs[pb] + ks * 256, KP1), acc);
+                    wgmma_n64<0, 0>(z[2], z[3], da, make_desc(bs[pb] + 64 * KP1 * 2 + ks * 256, KP1), acc);
+                    acc = 1;
+                }
+            }
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -183,29 +191,29 @@ __global__ void __launch_bounds__(TC_THREADS, 1) qmix_mix_tc_kernel(TcParams p) 
         }
         fence_proxy_async();
         __syncthreads();
-        // ---- GEMM2: W1raw (one 32-column block per agent), W2raw, b2
+        // ---- GEMM2: W1raw (one 32-column block per agent), W2raw, b2; the corrections first, as in GEMM1
         float w1[8][16], w2[16], b2[8];
         wgmma_fence();
         {
             const uint32_t off = (uint32_t)(64 * wg * TC_HH * 2);
             uint32_t acc = 0;
-            for (int pa = 0; pa < 2; ++pa)
-                for (int pb = 0; pb < 2 - pa; ++pb) {
-                    const uint32_t ba = smem_u32(pb ? B2al : B2ah), bb = smem_u32(pb ? B2bl : B2bh), bc = smem_u32(pb ? B2cl : B2ch);
+            for (int pp = 0; pp < 3; ++pp) {
+                const int pa = pp == 1, pb = pp == 0;
+                const uint32_t ba = smem_u32(pb ? B2al : B2ah), bb = smem_u32(pb ? B2bl : B2bh), bc = smem_u32(pb ? B2cl : B2ch);
 #pragma unroll
-                    for (int ks = 0; ks < TC_HH / 16; ++ks) {
-                        const uint32_t a0 = smem_u32(pa ? A2l[0] : A2h[0]) + off + ks * 256;
-                        const uint32_t a1 = smem_u32(pa ? A2l[1] : A2h[1]) + off + ks * 256;
-                        const uint32_t a2 = smem_u32(pa ? A2l[2] : A2h[2]) + off + ks * 256;
+                for (int ks = 0; ks < TC_HH / 16; ++ks) {
+                    const uint32_t a0 = smem_u32(pa ? A2l[0] : A2h[0]) + off + ks * 256;
+                    const uint32_t a1 = smem_u32(pa ? A2l[1] : A2h[1]) + off + ks * 256;
+                    const uint32_t a2 = smem_u32(pa ? A2l[2] : A2h[2]) + off + ks * 256;
 #pragma unroll
-                        for (int i = 0; i < 8; ++i)
-                            if (i < n)
-                                wgmma_n32<0, 0>(w1[i], make_desc(a0, TC_HH), make_desc(ba + i * TC_HH * TC_HH * 2 + ks * 256, TC_HH), acc);
-                        wgmma_n32<0, 0>(w2, make_desc(a1, TC_HH), make_desc(bb + ks * 256, TC_HH), acc);
-                        wgmma_n16<0, 0>(b2, make_desc(a2, TC_HH), make_desc(bc + ks * 256, TC_HH), acc);
-                        acc = 1;
-                    }
+                    for (int i = 0; i < 8; ++i)
+                        if (i < n)
+                            wgmma_n32<0, 0>(w1[i], make_desc(a0, TC_HH), make_desc(ba + i * TC_HH * TC_HH * 2 + ks * 256, TC_HH), acc);
+                    wgmma_n32<0, 0>(w2, make_desc(a1, TC_HH), make_desc(bb + ks * 256, TC_HH), acc);
+                    wgmma_n16<0, 0>(b2, make_desc(a2, TC_HH), make_desc(bc + ks * 256, TC_HH), acc);
+                    acc = 1;
                 }
+            }
         }
         wgmma_commit();
         wgmma_wait<0>();
