@@ -202,6 +202,33 @@ int xb_mappo_loss_fwd_bwd(const float *logits, const uint8_t *avail, int avail_l
                           int64_t R_total, float clip_range, float value_clip_range, float huber_delta, float vf_coef,
                           float ent_coef, float *dlogits, float *dvalue, float *stats, double *scratch, void *stream);
 
+/* ---------------------------------------------------------------- K4V: fused VDAC / IAC loss fwd+bwd --
+ * Replaces vdac_learner.py:53-126 and iac_learner.py:206-254 (one parameter-sharing group, Discrete actions) plus the
+ * autograd backward of those lines down to (logits, value), with the value mixing and its agent reduction fused in.
+ * Rows are agent steps in the episode buffer's (b, i, t) order, r = (b*n + i)*T + t, R = B*n*T (T = 1: feed-forward
+ * batches).  prep and vn come from xb_mappo_prepare / xb_value_norm_update (K4M), unchanged.
+ *     a_loss = -sum(adv * log pi(a) * mask) / M;   e = sum(H * mask) / M;   M = prep[0], the GLOBAL sum of the mask
+ *     masked logits (avail[r, a] == 0) count as -1e10 and get exactly 0 gradient (actor_head.py:40), as in K4M
+ *     c_loss = sum(lc(pred_r) * mask) / M with K4M's value term lc (vn target, Huber or square, inclusive clamp, ties
+ *              split 1/2);   loss = a_loss + vf_coef*c_loss - ent_coef*e
+ * The prediction pred_r of row r depends on mix_mode:
+ *     0 independent (IAC): pred_r = value[r]; dvalue[R].
+ *     1 VDN: value[R] holds V_i; V_tot(b, t) = sum_i V_i (agents in index order); dvalue[R] gets dV_i = dV_tot(b, t).
+ *     2 external mixer (QMIX): value[B*T] is V_tot(b, t) at b*T + t; dvalue[B*T] = dL/dV_tot.
+ *     row_order (modes 1, 2): 0 pairs V_tot(b, t) with rows (b, i, t) for every i; 1 reproduces the reference's
+ *     use_rnn pairing, where row r reads V_tot at index floor(r / n) of the b*T + t order (DESIGN.md section 4); the two
+ *     coincide at T = 1.  dV_tot sums the n rows paired with it, in a fixed order.
+ * stats[8] = {a_loss, c_loss, e, predict_value = sum_r pred_r / R_total (unmasked, as the reference logs it: for VDAC the
+ * mean of V_tot repeated n times), loss, 0, 0, 0}, each the local rows' share (a SUM all-reduce of the shards gives the
+ * global value).  No float atomics: the outputs are bit-identical across launches.  M = 0 gives NaN, as in the
+ * reference.  1 <= A <= 64 and 1 <= n <= 32 (else XB_ERANGE); R must be a multiple of n*T; actions are float32;
+ * old_value may be NULL when value_clip_range <= 0.  scratch as for K4. */
+int xb_vdac_loss_fwd_bwd(const float *logits, const uint8_t *avail, int avail_ld, const float *actions, const float *adv,
+                         const float *value, const float *old_value, const float *ret, const float *mask,
+                         const float *vn, const double *prep, int64_t R, int A, int n, int T, int mix_mode,
+                         int row_order, int64_t R_total, float value_clip_range, float huber_delta, float vf_coef,
+                         float ent_coef, float *dlogits, float *dvalue, float *stats, double *scratch, void *stream);
+
 /* ---------------------------------------------------------------- K5: prioritized-replay trees -------
  * Replaces SumSegmentTree/MinSegmentTree (xuance/common/segtree_tool.py:4-220) and their use in
  * PerOffPolicyBuffer (memory_tools.py:505-598).  One (sum,min) pair PER ENV, float32 nodes, heap layout

@@ -7,6 +7,7 @@ configs/mappo/sc2/5m_vs_6m.yaml (train_epochs env-steps/s); ``mappo_rnn``, recur
 configs/mappo/sc2/3m.yaml (update, eager and graphed); ``wqmix``, CW-QMIX in the shape of configs/wqmix/sc2/5m_vs_6m.yaml
 (update, eager and graphed); ``dcg``, DCG in the shape of configs/dcg/sc2/5m_vs_6m.yaml (update, eager and graphed);
 ``qtran``, QTRAN_alt in the shape of configs/qtran/sc2/5m_vs_6m.yaml (update, eager and graphed);
+``vdac``, VDAC (QMIX mixer) in the shape of configs/vdac/sc2/5m_vs_6m.yaml (update, eager and graphed);
 ``sacdis``, SAC-Discrete in the shape of
 configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (train_epochs, eager and graphed); ``ddpg`` and
 ``td3``, DDPG / TD3 in the shape of the reference's ddpg/mujoco.yaml and td3/mujoco.yaml (sample + update, eager and
@@ -469,6 +470,43 @@ def bench_mappo_rnn(args):
     return out
 
 
+def bench_vdac(args):
+    """VDAC with the QMIX mixer in the shape of configs/vdac/sc2/5m_vs_6m.yaml: one VDAC_Learner.update over its minibatch
+    of 8 episodes x 5 agents x T = 60 (GRU 64, LayerNorm, 12 masked actions, global state 98), eager and as a CUDA graph."""
+    from xuance_b200.common import Box, Discrete
+    from xuance_b200.common.common_tools import get_arguments
+    from xuance_b200.torch.agents import VDAC_Agents
+    B, n, T, od, A, sd = 8, 5, 60, 72, 12, 98
+    keys = ["agent_%d" % i for i in range(n)]
+    rng = np.random.default_rng(0)
+    S = B * n
+    avail = np.zeros((S, T, 12), np.uint8)
+    avail[..., :A] = rng.random((S, T, A)) > 0.3
+    avail[..., 0] = 1
+    lengths = np.tile(rng.integers(20, T + 1, B), n)
+    st = dict(obs=rng.uniform(-1, 1, (S, T, od)).astype(np.float32), actions=np.zeros((S, T), np.float32),
+              advantages=rng.normal(size=(S, T)).astype(np.float32), values=rng.normal(size=(S, T)).astype(np.float32),
+              returns=rng.normal(size=(S, T)).astype(np.float32),
+              agent_mask=(rng.random((S, T)) > 0.05).astype(np.float32),
+              filled=(np.arange(T)[None] < lengths[:, None]).astype(np.float32), avail_actions=avail,
+              state=np.tile(rng.normal(size=(B, T, sd)).astype(np.float32), (n, 1, 1)))
+    sample = {'_stacked': {k: torch.from_numpy(v).to(DEV) for k, v in st.items()}, 'batch_size': B,
+              'sequence_length': T}
+    out = {"config": "VDAC (QMIX mixer) 5m_vs_6m shape: 8 episodes x 5 agents x T = 60 per update, Basic_RNN (fc 64, "
+                     "GRU 64, LayerNorm) actor and critic, 12 masked actions, value clip + ValueNorm + Huber"}
+    for graph in (False, True):
+        cfg = get_arguments("vdac", "sc2", "5m_vs_6m")
+        for k, v in dict(device=DEV, parallels=8, logger=None, model_dir="/tmp/x", use_cuda_graph=graph,
+                         distributed_training=False, episode_length=T).items():
+            setattr(cfg, k, v)
+        torch.manual_seed(0)
+        agent = VDAC_Agents(cfg, None, n, keys, Box(-1, 1, (sd,), np.float32),
+                            {k: Box(-1, 1, (od,), np.float32) for k in keys}, {k: Discrete(A) for k in keys})
+        dt = timed(lambda: agent.learner.update(sample, sync=False), max(5, args.iters // 10), warm=3)
+        out["gpu_ms_per_update_" + ("graph" if graph else "eager")] = dt * 1e3
+    return out
+
+
 def bench_sacdis(args):
     """SAC-Discrete: ``train_epochs(1)`` (one replay sample of 256 rows + one SACDIS_Learner.update) of a SAC_Agent built
     from configs/sac/CartPole-v1.yaml (4-d obs, A = 2, Basic_MLP 128, heads [128], alpha fixed), and the same at A = 18 with
@@ -675,6 +713,8 @@ def main():
         res["mappo"] = bench_mappo(args)
     if (not only and WORLD == 1) or "mappo_rnn" in only:
         res["mappo_rnn"] = bench_mappo_rnn(args)
+    if (not only and WORLD == 1) or "vdac" in only:
+        res["vdac"] = bench_vdac(args)
     if (not only and WORLD == 1) or "sacdis" in only:
         res["sacdis"] = bench_sacdis(args)
     for algo in ("ddpg", "td3"):

@@ -44,6 +44,7 @@ _SIGNATURES = {
     "xb_value_norm_update": (c_int, [_P, _P, _P, _P, c_int64, c_double, _P, _P]),
     "xb_mappo_loss_fwd_bwd": (c_int, [_P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, c_int64,
                                       c_float, c_float, c_float, c_float, c_float, _P, _P, _P, _P, _P]),
+    "xb_vdac_loss_fwd_bwd": (c_int, [_P, _P, c_int] + [_P] * 8 + [c_int64] + [c_int] * 5 + [c_int64] + [c_float] * 4 + [_P] * 5),
     "xb_per_insert": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_float, _P]),
     "xb_per_sample": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int64, c_float, _P, _P, _P, _P]),
     "xb_per_update": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, _P]),

@@ -448,19 +448,6 @@ extern "C" int xb_value_norm_update(float *running_mean, float *running_mean_sq,
     return xb_launch_status();
 }
 
-// nn.HuberLoss(reduction='none', delta) forward and d/d(input) at d = input - target (aten huber / huber_backward);
-// delta <= 0 selects (input - target)^2.
-__device__ __forceinline__ void value_loss(float d, float delta, float &l, float &g) {
-    if (delta > 0.f) {
-        const float z = fabsf(d);
-        l = z < delta ? __fmul_rn(__fmul_rn(0.5f, z), z) : __fmul_rn(delta, __fsub_rn(z, __fmul_rn(0.5f, delta)));
-        g = d <= -delta ? -delta : (d >= delta ? delta : d);
-    } else {
-        l = __fmul_rn(d, d);
-        g = 2.f * d;
-    }
-}
-
 template <int A_MAX>
 __global__ void __launch_bounds__(256, 1) mappo_loss_kernel(
     const float *__restrict__ logits, const uint8_t *__restrict__ avail, int avail_ld,

@@ -62,6 +62,19 @@ __device__ __forceinline__ void block_sum_d(double (&v)[K], double *smem) {
     }
 }
 
+// nn.HuberLoss(reduction='none', delta) forward and d/d(input) at d = input - target (aten huber / huber_backward);
+// delta <= 0 selects (input - target)^2.  The value term of K4M and K4V.
+__device__ __forceinline__ void value_loss(float d, float delta, float &l, float &g) {
+    if (delta > 0.f) {
+        const float z = fabsf(d);
+        l = z < delta ? __fmul_rn(__fmul_rn(0.5f, z), z) : __fmul_rn(delta, __fsub_rn(z, __fmul_rn(0.5f, delta)));
+        g = d <= -delta ? -delta : (d >= delta ? delta : d);
+    } else {
+        l = __fmul_rn(d, d);
+        g = 2.f * d;
+    }
+}
+
 // Deterministic grid reduction: every block deposits K partial sums, the last block to arrive (ticket counter)
 // adds them in block order and calls fin(total[K]).  scratch layout: [K][XB_MAX_PARTIALS] doubles then the
 // int32 ticket at scratch[K_MAX*XB_MAX_PARTIALS] (K_MAX = 8).  gridDim.x <= XB_MAX_PARTIALS.

@@ -31,3 +31,6 @@ REGISTRY_Agents["QTRAN_alt"] = QTRAN_Agents
 from .mappo_agents import OnPolicyMARLAgents, MAPPO_Agents, IPPO_Agents
 REGISTRY_Agents["MAPPO"] = MAPPO_Agents
 REGISTRY_Agents["IPPO"] = IPPO_Agents
+from .vdac_agents import VDAC_Agents, IAC_Agents
+REGISTRY_Agents["VDAC"] = VDAC_Agents
+REGISTRY_Agents["IAC"] = IAC_Agents

@@ -92,6 +92,10 @@ class OnPolicyMARLAgents(MARLAgents):
         s = torch.as_tensor(np.asarray(state, np.float32), device=self.device)
         return s.repeat_interleave(self.n_agents, dim=0)          # rows are env-major, agent-minor
 
+    def _critic_values(self, obs_d, state, n_envs, rnn_states=None, return_states=False):
+        """The values of the acting rows [n_envs * n_agents] (and the new critic states with return_states)."""
+        return self.model.values(obs_d, self._states(state, n_envs), rnn_states=rnn_states, return_states=return_states)
+
     @torch.no_grad()
     def get_actions(self, obs_list, state=None, avail_actions_list=None, rnn_states_actor=None,
                     rnn_states_critic=None, test_mode=False, deterministic=False, **kwargs):
@@ -114,10 +118,9 @@ class OnPolicyMARLAgents(MARLAgents):
                   _lib.ptr(out[1]), None)
         if not test_mode:
             if self.use_rnn:
-                out[2], rnn_states_critic = self.model.values(obs_d, self._states(state, n_envs),
-                                                              rnn_states=rnn_states_critic, return_states=True)
+                out[2], rnn_states_critic = self._critic_values(obs_d, state, n_envs, rnn_states_critic, True)
             else:
-                out[2] = self.model.values(obs_d, self._states(state, n_envs))
+                out[2] = self._critic_values(obs_d, state, n_envs)
         host = out.cpu().numpy().reshape(3, n_envs, len(K))
         actions_list = [{k: int(host[0, e, i]) for i, k in enumerate(K)} for e in range(n_envs)]
         log_pi, values = {}, {}
@@ -136,7 +139,7 @@ class OnPolicyMARLAgents(MARLAgents):
         if self.use_rnn:      # the critic rows of env i (on_policy_marl.py:337-344)
             n = len(self.agent_keys)
             h = rnn_states_critic[:, i_env * n:(i_env + 1) * n]
-        v = self.model.values(torch.from_numpy(obs).to(self.device), self._states(st, 1), rnn_states=h).cpu().numpy()
+        v = self._critic_values(torch.from_numpy(obs).to(self.device), st, 1, h).cpu().numpy()
         return None, {k: v[i] for i, k in enumerate(self.agent_keys)}
 
     def init_rnn_states(self, n_envs):

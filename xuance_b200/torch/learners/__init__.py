@@ -10,6 +10,7 @@ from .wqmix_learner import WQMIX_Learner
 from .dcg_learner import DCG_Learner
 from .qtran_learner import QTRAN_Learner
 from .mappo_learner import MAPPO_Learner
+from .vdac_learner import VDAC_Learner, IAC_Learner
 from .ppg_learner import PPG_Learner
 
 REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner, "DQN_Learner": DQN_Learner,
@@ -21,4 +22,5 @@ REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner,
                      "QMIX_Learner": QMIX_Learner,
                      "VDN_Learner": QMIX_Learner,     # vdn_learner.py: the same update with the parameter-free sum mixer
                      "MAPPO_Learner": MAPPO_Learner, "PPG_Learner": PPG_Learner, "WQMIX_Learner": WQMIX_Learner,
-                     "DCG_Learner": DCG_Learner, "QTRAN_Learner": QTRAN_Learner}
+                     "DCG_Learner": DCG_Learner, "QTRAN_Learner": QTRAN_Learner,
+                     "VDAC_Learner": VDAC_Learner, "IAC_Learner": IAC_Learner}

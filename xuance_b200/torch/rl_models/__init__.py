@@ -16,3 +16,4 @@ from .mappo import CategoricalActor, CentralizedStateValueCritic, MultiAgentActo
 from .gru import GRUSequence, gru_sequence, Basic_RNN_K13
 from .dcg import DCG_Utility, DCG_Payoff, Coordination_Graph, DeepCoordinationGraph
 from .qtran import QTRAN_Base, QTRAN_Alt, QTranMixingNetwork
+from .vdac import IndependentActorCritic, ValueDecompositionActorCritic
