@@ -568,6 +568,26 @@ int xb_gru_seq_fwd(const float *xg, const float *w_hh, const float *b_hh, const 
 int xb_gru_seq_bwd(const float *dy, const float *dhT, const float *w_hh, const float *gates, const float *y,
                    const float *h0, int64_t S, int T, int H, float *dxg, float *dgh, float *dh0, void *stream);
 
+/* ---------------------------------------------------------------- K13L: LSTM sequence kernels ---------
+ * The recurrence of a one-layer torch.nn.LSTM (gate order i, f, g, o) over S independent sequences of T steps, as
+ * DRQN's recurrent Q head runs it (RecurrentQValueHead, rl_models/heads/q_head.py:126-175).  xg[S, T, 4H] is the
+ * projected input x W_ih^T + b_ih (a cuBLAS GEMM the caller runs for all T at once); w_hh[4H, H], b_hh[4H] are torch's
+ * weight_hh_l0 / bias_hh_l0; h0, c0 [S, H] are nullable (zeros).  Per step, with pre = xg + (W_hh h + b_hh),
+ *     i = sigmoid(pre_i), f = sigmoid(pre_f), g = tanh(pre_g), o = sigmoid(pre_o), c' = f c + i g, h' = o tanh(c').
+ * fwd: writes y[S, T, H] (every h'), hT, cT [S, H] and, when gates != NULL (training), gates[S, T, 5H] = {i, f, g, o, c'}.
+ * bwd: from dy[S, T, H] and nullable dhT, dcT [S, H], with the forward's gates and c0, writes dxg[S, T, 4H], the gradient
+ *      of the pre-activations.  All four are plain sums of xg and W_hh h + b_hh, so dxg is also the gradient of
+ *      W_hh h + b_hh: dW_ih, db_ih, dx, dW_hh = sum dxg^T h_{t-1} and db_hh = sum dxg follow by GEMMs / sums.  When
+ *      dh0 / dc0 != NULL, writes dh0, dc0 [S, H].
+ * float32 on the CUDA cores with accurate expf / tanhf; one CTA of 4H threads walks all T steps of 4 sequences.  W_hh
+ * stays on chip: the first 32 k-entries of each thread's column in registers, the rest in shared memory (192 KB of the
+ * 256 KB at H = 128).  No atomics: every sequence's result is bit-identical from launch to launch and whichever CTA
+ * owns it.  1 <= H <= 128, T >= 1, S >= 1, and NULL required pointers, are XB_EINVAL. */
+int xb_lstm_seq_fwd(const float *xg, const float *w_hh, const float *b_hh, const float *h0, const float *c0, int64_t S,
+                    int T, int H, float *y, float *hT, float *cT, float *gates, void *stream);
+int xb_lstm_seq_bwd(const float *dy, const float *dhT, const float *dcT, const float *w_hh, const float *gates,
+                    const float *c0, int64_t S, int T, int H, float *dxg, float *dh0, float *dc0, void *stream);
+
 /* ---------------------------------------------------------------- K7: flat-bucket optimiser step -----
  * Replaces clip_grad_norm_ + torch.optim.Adam.step on the learner's parameters (ppo_learner.py:61-65;
  * Adam eps=1e-5, no weight decay, no amsgrad) over ONE flat float32 bucket (params/grads/exp_avg/exp_avg_sq

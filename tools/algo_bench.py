@@ -12,7 +12,8 @@ configs/mappo/sc2/3m.yaml (update, eager and graphed); ``wqmix``, CW-QMIX in the
 configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (train_epochs, eager and graphed); ``ddpg`` and
 ``td3``, DDPG / TD3 in the shape of the reference's ddpg/mujoco.yaml and td3/mujoco.yaml (sample + update, eager and
 graphed); ``c51`` and ``qrdqn`` on CartPole (Basic_MLP 128, B=256) and SyntheticAtari (Basic_CNN, B=32) shapes (update,
-eager and graphed).  Prints one JSON object.
+eager and graphed); ``drqn``, DRQN in the shape of configs/drqn/classic_control/CartPole-v1.yaml (update, eager and
+graphed).  Prints one JSON object.
 
     python tools/algo_bench.py [--iters 200] [--cpu-iters 5] [--no-cpu] [--graph]
     torchrun --nnodes=1 --nproc-per-node G --master-addr 127.0.0.1 tools/algo_bench.py --no-cpu --graph    (G GPUs)
@@ -674,6 +675,39 @@ def bench_dist_dqn(args, algo):
     return res
 
 
+def bench_drqn(args, repeats=3):
+    """DRQN in the shape of configs/drqn/classic_control/CartPole-v1.yaml: one DRQN_Learner.update over B = 8 windows of
+    L = 50 steps (Basic_MLP 128, LSTM 128, 2 actions), eager and as a CUDA graph, each repeated ``repeats`` times, next to
+    the torch-CPU oracle's update (nn.LSTM on the host) on the same shape."""
+    import subprocess
+    from xuance_b200.common import Box, Discrete
+    from xuance_b200.common.common_tools import get_arguments
+    from xuance_b200.torch.agents import DRQN_Agent
+    from oracle_drqn import DRQNOracle, DRQNLearnerOracle
+    B, L, od, A = 8, 50, 4, 2
+    rng = np.random.default_rng(0)
+    sample = {"obs": torch.from_numpy(rng.standard_normal((B, L + 1, od)).astype(np.float32)).to(DEV),
+              "actions": torch.from_numpy(rng.integers(0, A, (B, L)).astype(np.float32)).to(DEV),
+              "rewards": torch.ones(B, L, device=DEV), "terminals": torch.zeros(B, L, device=DEV), "batch_size": B}
+    out = {"config": "DRQN CartPole-v1 shape: B = 8 windows x L = 50, Basic_MLP 128, LSTM 128, 2 actions",
+           "gpu": subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                                 capture_output=True, text=True).stdout.strip()}
+    for graph in (False, True):
+        cfg = get_arguments("drqn", "classic_control", "CartPole-v1")
+        for k, v in dict(device=DEV, logger=None, model_dir="/tmp/x", use_cuda_graph=graph, episode_length=500).items():
+            setattr(cfg, k, v)
+        agent = DRQN_Agent(cfg, observation_space=Box(-np.inf, np.inf, (od,), np.float32), action_space=Discrete(A))
+        out["gpu_ms_per_update_" + ("graph" if graph else "eager")] = [
+            round(timed(lambda: agent.learner.update(sync=False, **sample), args.iters, warm=5) * 1e3, 4)
+            for _ in range(repeats)]
+    if not args.no_cpu:
+        ol = DRQNLearnerOracle(DRQNOracle("LSTM", 128, od, 128, A))
+        cs = {k: v.cpu() for k, v in sample.items() if k != "batch_size"}
+        out["cpu_ms_per_update"] = round(cpu_timed(lambda: ol.update(**cs), max(args.cpu_iters, 3)) * 1e3, 3)
+        out["cpu_threads"] = torch.get_num_threads()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=200)
@@ -723,6 +757,8 @@ def main():
     for algo in ("c51", "qrdqn"):
         if (not only and WORLD == 1) or algo in only:
             res[algo] = bench_dist_dqn(args, algo)
+    if (not only and WORLD == 1) or "drqn" in only:
+        res["drqn"] = bench_drqn(args)
     res["cuda_graph"] = bool(args.graph)
     res["n_gpus"] = WORLD
     if RANK == 0:

@@ -4,7 +4,7 @@ shapes (SURVEY.md section 7 "hard parts": at the named PPO shape K2/K4/K5 move <
 bandwidth fraction is also reported at a scaled shape).  CUDA events on the launching stream, >= 3 warm-ups, L2
 flushed between timed launches (256 MB memset).  Prints one JSON object.
 
-    python tools/kernel_bench.py [--only k2,k4] [--reps 20]      (k12 / k12box / k3p: the tensor-core encoder layers, gathered and TMA-box / halo variants; k13: the GRU sequence kernels against cuDNN)
+    python tools/kernel_bench.py [--only k2,k4] [--reps 20]      (k12 / k12box / k3p: the tensor-core encoder layers, gathered and TMA-box / halo variants; k13: the GRU sequence kernels against cuDNN; k13l: the LSTM sequence kernels against cuDNN)
 """
 import argparse
 import json
@@ -372,9 +372,50 @@ def main():
                       xp_.numel() * 2 + g3.numel() * 2, hbm, 2.0 * B * 100 * 64 * K, tpk))
     if want("k13"):
         out["k13"] = k13_bench(R, hbm)
+    if want("k13l"):
+        out["k13l"] = k13l_bench(R)
     if want("dcg"):
         out["dcg"] = dcg_bench(R)
     print(json.dumps(out))
+
+
+def k13l_bench(R, repeats=3):
+    """K13L at DRQN's shapes: training (S = 8 sequences of T = 50, H = 128, input 128, configs/drqn CartPole-v1), acting
+    (S = 10, T = 1) and a larger S = 640: a whole LSTM forward + backward (input projection and weight-gradient GEMMs
+    included) through lstm_sequence against nn.LSTM on cuDNN (forward only for acting), both in IEEE fp32.  Each timing
+    is repeated ``repeats`` times, alternating the two, so the spread is visible."""
+    import subprocess
+    import torch.nn as nn
+    from xuance_b200.torch.rl_models import lstm_sequence
+    saved = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        res = {"gpu": subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm",
+                                      "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()}
+        H = I = 128
+        torch.manual_seed(0)
+        lstm = nn.LSTM(I, H, batch_first=True, device=DEV)
+        for name, S, T, train in (("train", 8, 50, True), ("act", 10, 1, False), ("large", 640, 50, True)):
+            x = torch.randn(S, T, I, device=DEV, requires_grad=train)
+            dy = torch.randn(S, T, H, device=DEV)
+
+            def step(mine):
+                if not train:
+                    with torch.no_grad():
+                        return lstm_sequence(lstm, x)[0] if mine else lstm(x)[0]
+                x.grad = None
+                lstm.zero_grad(set_to_none=True)
+                yy = lstm_sequence(lstm, x)[0] if mine else lstm(x)[0]
+                yy.backward(dy)
+            ours, cudnn = [], []
+            for _ in range(repeats):
+                ours.append(round(timeit(lambda: step(True), R), 2))
+                cudnn.append(round(timeit(lambda: step(False), R), 2))
+            res[name] = {"shape": f"S={S} T={T} H={H} I={I}" + (" fwd+bwd" if train else " fwd"), "k13l_us": ours,
+                         "cudnn_us": cudnn, "speedup_median": round(float(np.median(cudnn) / np.median(ours)), 2)}
+        return res
+    finally:        # IEEE fp32 for this comparison only
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = saved
 
 
 def k13_bench(R, hbm):

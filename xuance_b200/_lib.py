@@ -90,6 +90,8 @@ _SIGNATURES = {
     "xb_ddpg_actor_loss": (c_int, [_P, _P, c_int64, c_int64, _P, _P, _P, _P, _P]),
     "xb_gru_seq_fwd": (c_int, [_P, _P, _P, _P, c_int64, c_int, c_int, _P, _P, _P, _P]),
     "xb_gru_seq_bwd": (c_int, [_P, _P, _P, _P, _P, _P, c_int64, c_int, c_int, _P, _P, _P, _P]),
+    "xb_lstm_seq_fwd": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int, c_int, _P, _P, _P, _P, _P]),
+    "xb_lstm_seq_bwd": (c_int, [_P, _P, _P, _P, _P, _P, c_int64, c_int, c_int, _P, _P, _P, _P]),
     "xb_qmix_select_fwd": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     "xb_qmix_select_bwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
     "xb_qmix_mix_fwd": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int, c_int, _P, _P]),

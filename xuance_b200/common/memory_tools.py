@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from .. import _lib
-from .spaces import space2shape
+from .spaces import space2shape, is_discrete
 
 
 def _as_device(x, device, dtype=None):
@@ -724,3 +724,103 @@ class PerOffPolicyBuffer(DummyOffPolicyBuffer):
         pr = pr.to(device=self.device, dtype=torch.float32).contiguous()
         _lib.call("xb_per_update", _lib.ptr(self._it_sum), _lib.ptr(self._it_min), _lib.ptr(self._max_priority),
                   _lib.ptr(idx_t), _lib.ptr(pr), self.n_envs, self._it_capacity, self._k, float(self._alpha))
+
+
+# =====================================================================================================
+# Episode replay for recurrent off-policy learners (DRQN)
+# =====================================================================================================
+class RecurrentOffPolicyBuffer(Buffer):
+    """Device-resident mirror of RecurrentOffPolicyBuffer and EpisodeBuffer (reference memory_tools.py:145-179,
+    390-468).  ``buffer_size`` counts transitions, the ring counts episodes: ``n_size = buffer_size // n_envs`` slots, as
+    the reference's ``deque(maxlen=n_size)``.
+
+    Each env stages its running episode in ``episode_length + 1`` device rows: row 0 holds the first observation and row
+    t + 1 holds the observation after step t with that step's (action, reward, terminal).  ``begin`` writes row 0,
+    ``put`` writes one row of every env in one ``xb_rollout_store_at`` launch at each env's own step, and ``store(i)``
+    copies env i's finished episode into the next ring slot with its length.  ``sample`` draws on the host in the
+    reference's order (episodes with replacement, one shared window length, one start per episode) and gathers the
+    windows with K3: obs [B, L+1, obs], actions / rewards / terminals [B, L]."""
+
+    FIELDS = ("actions", "rewards", "terminals")
+    _ckpt_tensors = ("_obs", "_fields", "_stage_obs", "_stage_fields")
+    _ckpt_host = ("_len", "_stage_len")
+
+    def __init__(self, observation_space, action_space, auxiliary_shape, n_envs, buffer_size, batch_size,
+                 episode_length, lookup_length, device="cuda:0"):
+        super().__init__(observation_space, action_space, auxiliary_shape, n_envs, buffer_size, device)
+        if not is_discrete(action_space):
+            raise ValueError("RecurrentOffPolicyBuffer stores Discrete actions")
+        obs_shape = space2shape(self.observation_space)
+        if isinstance(obs_shape, dict):
+            raise NotImplementedError("dict observation spaces are outside the hot path")
+        self.batch_size, self.episode_length, self.lookup_length = batch_size, int(episode_length), lookup_length
+        self._obs_dim = int(np.prod(obs_shape))
+        self._obs_shape = tuple(obs_shape)
+        R, F = self.episode_length + 1, len(self.FIELDS)
+        self._obs = torch.zeros((self.n_size, R, self._obs_dim), dtype=torch.float32, device=self.device)
+        self._fields = torch.zeros((F, self.n_size, R), dtype=torch.float32, device=self.device)
+        self._len = np.zeros(self.n_size, np.int64)
+        self._stage_obs = torch.zeros((n_envs, R, self._obs_dim), dtype=torch.float32, device=self.device)
+        self._stage_fields = torch.zeros((F, n_envs, R), dtype=torch.float32, device=self.device)
+        self._stage_len = np.zeros(n_envs, np.int64)
+
+    def can_sample(self):
+        return self.size >= self.batch_size
+
+    def clear(self, *args):
+        self.ptr, self.size = 0, 0
+
+    def _store_at(self, steps, obs, scal=None):
+        st = torch.from_numpy(steps.astype(np.int32)).to(self.device)
+        o = _as_device(np.asarray(obs, np.float32).reshape(self.n_envs, self._obs_dim), self.device, torch.float32)
+        s = None if scal is None else _as_device(scal, self.device, torch.float32)
+        _lib.call("xb_rollout_store_at", _lib.ptr(self._stage_obs), _lib.ptr(o), self._obs_dim * 4,
+                  _lib.ptr(self._stage_fields if s is not None else None), _lib.ptr(s), 0 if s is None else len(self.FIELDS),
+                  self.n_envs, self.episode_length + 1, _lib.ptr(st))
+
+    def begin(self, obs, envs=None):
+        """Starts a new episode at ``obs`` [n_envs, obs] for the envs in ``envs`` (None: all)."""
+        sel = np.zeros(self.n_envs, bool)
+        sel[slice(None) if envs is None else list(envs)] = True
+        self._stage_len[sel] = 0
+        self._store_at(np.where(sel, 0, -1), obs)
+
+    def put(self, next_obs, acts, rews, terminals):
+        """EpisodeBuffer.put for every env: one transition (next obs, action, reward, terminal) per env."""
+        if (self._stage_len >= self.episode_length).any():
+            raise RuntimeError("RecurrentOffPolicyBuffer: an episode ran past episode_length = %d steps"
+                               % self.episode_length)
+        self._stage_len += 1
+        scal = np.stack([np.asarray(x, np.float32).reshape(self.n_envs) for x in (acts, rews, terminals)])
+        self._store_at(self._stage_len, next_obs, scal)
+
+    def store(self, i):
+        """reference :433-436: env i's staged episode -> the ring (the oldest episode drops out once it is full)."""
+        n = int(self._stage_len[i])
+        self._obs[self.ptr, :n + 1].copy_(self._stage_obs[i, :n + 1])
+        self._fields[:, self.ptr, :n + 1].copy_(self._stage_fields[:, i, :n + 1])
+        self._len[self.ptr] = n
+        self.ptr = (self.ptr + 1) % self.n_size
+        self.size = min(self.size + 1, self.n_size)
+
+    def sample(self):
+        """reference :438-468, drawing from NumPy's global RNG in the reference's order."""
+        B = self.batch_size
+        pos = np.random.choice(self.size, B)                          # deque positions, oldest first
+        slots = (self.ptr - self.size + pos) % self.n_size
+        lens = self._len[slots]
+        L = int(min(self.episode_length, lens.min(), self.lookup_length))
+        starts = np.array([np.random.randint(0, n - L + 1) for n in lens], np.int64)
+        base = slots.astype(np.int64) * (self.episode_length + 1) + starts
+        obs_idx = self._index_tensor((base[:, None] + np.arange(L + 1)).reshape(-1))
+        scal_idx = self._index_tensor((base[:, None] + 1 + np.arange(L)).reshape(-1))
+        obs = torch.empty((B, L + 1, self._obs_dim), dtype=torch.float32, device=self.device)
+        _lib.call("xb_gather_rows", _lib.ptr(self._obs), _lib.ptr(obs_idx), B * (L + 1), self._obs_dim * 4,
+                  _lib.ptr(obs))
+        F = len(self.FIELDS)
+        out = torch.empty((F, B * L), dtype=torch.float32, device=self.device)
+        _lib.call("xb_gather_scalars", _lib.ptr(self._fields), self.n_size * (self.episode_length + 1),
+                  _lib.ptr(scal_idx), B * L, F, _lib.ptr(out), -1, None, None)
+        out = out.view(F, B, L)
+        return {"obs": obs.view((B, L + 1) + self._obs_shape), "actions": out[0], "rewards": out[1],
+                "terminals": out[2], "batch_size": B}

@@ -12,6 +12,7 @@ from .qtran_learner import QTRAN_Learner
 from .mappo_learner import MAPPO_Learner
 from .vdac_learner import VDAC_Learner, IAC_Learner
 from .ppg_learner import PPG_Learner
+from .drqn_learner import DRQN_Learner
 
 REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner, "DQN_Learner": DQN_Learner,
                      "PerDQN_Learner": PerDQN_Learner, "DDQN_Learner": DDQN_Learner, "A2C_Learner": A2C_Learner,
@@ -23,4 +24,5 @@ REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner,
                      "VDN_Learner": QMIX_Learner,     # vdn_learner.py: the same update with the parameter-free sum mixer
                      "MAPPO_Learner": MAPPO_Learner, "PPG_Learner": PPG_Learner, "WQMIX_Learner": WQMIX_Learner,
                      "DCG_Learner": DCG_Learner, "QTRAN_Learner": QTRAN_Learner,
-                     "VDAC_Learner": VDAC_Learner, "IAC_Learner": IAC_Learner}
+                     "VDAC_Learner": VDAC_Learner, "IAC_Learner": IAC_Learner,
+                     "DRQN_Learner": DRQN_Learner}

@@ -1,5 +1,5 @@
 from .layers import mlp_block, cnn_block, ActivationFunctions
-from .outputs import (ModelOutput, RepresentationOutput, ActionOutput, StochasticActorOutput, TwinCriticOutput,
+from .outputs import (ModelOutput, RNN_State, RepresentationOutput, ActionOutput, StochasticActorOutput, TwinCriticOutput,
                       DeterministicActorOutput, CriticOutput)
 from .distributions import CategoricalDistribution, DiagGaussianDistribution, ActivatedDiagGaussianDistribution
 from .representations import Basic_Identical, Basic_MLP, Basic_CNN, AC_CNN_Atari, REGISTRY_Representation
@@ -17,3 +17,5 @@ from .gru import GRUSequence, gru_sequence, Basic_RNN_K13
 from .dcg import DCG_Utility, DCG_Payoff, Coordination_Graph, DeepCoordinationGraph
 from .qtran import QTRAN_Base, QTRAN_Alt, QTranMixingNetwork
 from .vdac import IndependentActorCritic, ValueDecompositionActorCritic
+from .lstm import LSTMSequence, lstm_sequence
+from .drqn import RecurrentQValueHead, DeepRecurrentQNetwork

@@ -4,6 +4,12 @@ from typing import Any, Optional
 
 
 @dataclass
+class RNN_State:
+    hidden_states: Any = None
+    cell_states: Any = None
+
+
+@dataclass
 class RepresentationOutput:
     embeddings: Any
     rnn_states: Any = None
