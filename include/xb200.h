@@ -229,6 +229,41 @@ int xb_vdac_loss_fwd_bwd(const float *logits, const uint8_t *avail, int avail_ld
                          int row_order, int64_t R_total, float value_clip_range, float huber_delta, float vf_coef,
                          float ent_coef, float *dlogits, float *dvalue, float *stats, double *scratch, void *stream);
 
+/* ---------------------------------------------------------------- K4C: COMA critic input, loss fwd+bwd, acting --
+ * Replaces coma_learner.py:53-137, the critic-input assembly of centralized_critics.py:259-286 and the epsilon-mixed
+ * acting of actor_critic.py:279-295 / coma_agents.py:226-258 (one parameter-sharing group, Discrete actions).  Rows are
+ * agent steps in the episode buffer's (b, i, t) order, r = (b*n + i)*T + t, R = B*n*T.  Actions are float32 integers.
+ * xb_coma_critic_input: out[R, S + F + n*A] with row r = [state[b, t, 0..S) | feat[r, 0..F) | joint one-hot of the n
+ *     agents' actions at (b, t), agent-major, with agent i's own A-block zeroed] from state [B,T,S], feat [R,F] and
+ *     actions [B,n,T].  Copies and 0 / 1 only, so the rows are bit-exact; an action outside [0, A) sets no bit.  Its
+ *     backward is the feature slice of the output gradient (no kernel).  1 <= A <= 64, 1 <= n <= 32 (else XB_ERANGE).
+ * xb_coma_loss_fwd_bwd: logits[R,A] with avail[R, avail_ld] (uint8, nullable: use_actions_mask), q[R,A] the critic's
+ *     Q, eps[1] (DEVICE scalar: a captured graph stays valid while epsilon decays), M = prep[0] from xb_mappo_prepare
+ *     (the GLOBAL sum of the mask):
+ *     p = softmax(z), z = logits with unavailable entries at -1e10;  q_mix = (1 - eps) p + eps / A;
+ *     pi = q_mix * av / sum(q_mix * av)  (av = 1 without avail);  baseline = sum_a pi_a Q_a;
+ *     adv = Q[a] - baseline (detached);  loss_a = -sum(adv * log pi[a] * mask) / M;
+ *     loss_c = sum(((Q[a] - ret) * mask)^2) / M
+ *     dlogits[R,A] = d loss_a / d logits, exactly 0 at unavailable entries; a taken action with pi[a] = 0 gives
+ *     log pi[a] = -inf and NaN at the row's available entries, as autograd of the reference does.
+ *     dq[R,A] = d loss_c / d Q, nonzero only at the taken action.
+ *     stats[8] = {loss_a, loss_c, advantage = sum(adv) / R_total (unmasked, as the reference logs it), 0, 0, 0, 0, 0},
+ *     each the local rows' share (a SUM all-reduce of the shards gives the global value).  No float atomics: outputs
+ *     are bit-identical across launches.  M = 0 gives NaN, as in the reference.  1 <= A <= 64 (else XB_ERANGE).
+ *     scratch as for K4.
+ * xb_coma_act: the acting distribution over logits[N,A]: pi = q_mix / sum(q_mix) with eps[1] on the device (eps NULL:
+ *     no mix, the reference's test_mode).  uniforms != NULL: a = min{i : u < pi_0 + .. + pi_i} (the last index with
+ *     pi_i > 0 if rounding leaves the total below u); else the first arg-max of pi.  After the mix an unavailable action
+ *     has probability eps / A and can be drawn, as in the reference.  Outputs (each nullable, at least one):
+ *     actions_f32[N], actions_i32[N], logp[N] = log pi[a].  A <= 64 (else XB_ERANGE). */
+int xb_coma_critic_input(const float *state, const float *feat, const float *actions, int B, int n, int T, int S, int F,
+                         int A, float *out, void *stream);
+int xb_coma_loss_fwd_bwd(const float *logits, const uint8_t *avail, int avail_ld, const float *q, const float *actions,
+                         const float *ret, const float *mask, const float *eps, const double *prep, int64_t R, int A,
+                         int64_t R_total, float *dlogits, float *dq, float *stats, double *scratch, void *stream);
+int xb_coma_act(const float *logits, const uint8_t *avail, int avail_ld, const float *eps, const float *uniforms, int N,
+                int A, float *actions_f32, int32_t *actions_i32, float *logp, void *stream);
+
 /* ---------------------------------------------------------------- K5: prioritized-replay trees -------
  * Replaces SumSegmentTree/MinSegmentTree (xuance/common/segtree_tool.py:4-220) and their use in
  * PerOffPolicyBuffer (memory_tools.py:505-598).  One (sum,min) pair PER ENV, float32 nodes, heap layout

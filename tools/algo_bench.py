@@ -13,7 +13,8 @@ configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (tr
 ``td3``, DDPG / TD3 in the shape of the reference's ddpg/mujoco.yaml and td3/mujoco.yaml (sample + update, eager and
 graphed); ``c51`` and ``qrdqn`` on CartPole (Basic_MLP 128, B=256) and SyntheticAtari (Basic_CNN, B=32) shapes (update,
 eager and graphed); ``drqn``, DRQN in the shape of configs/drqn/classic_control/CartPole-v1.yaml (update, eager and
-graphed).  Prints one JSON object.
+graphed); ``coma``, COMA in the shape of configs/coma/sc2/5m_vs_6m.yaml (update, eager and graphed).  Prints one JSON
+object.
 
     python tools/algo_bench.py [--iters 200] [--cpu-iters 5] [--no-cpu] [--graph]
     torchrun --nnodes=1 --nproc-per-node G --master-addr 127.0.0.1 tools/algo_bench.py --no-cpu --graph    (G GPUs)
@@ -708,6 +709,63 @@ def bench_drqn(args, repeats=3):
     return out
 
 
+def bench_coma(args):
+    """COMA in the shape of configs/coma/sc2/5m_vs_6m.yaml: one COMA_Learner.update over its minibatch of 8 episodes x 5
+    agents x T = 60 (fc 64, GRU 64, LayerNorm actor and critic encoders, critic MLP 128-128 over the 98 + 64 + 5 * 12
+    counterfactual input, 12 actions), eager and as a CUDA graph, next to the torch-CPU oracle's update (nn.GRU on the
+    host) on the same model and sample."""
+    import copy
+    import subprocess
+    from xuance_b200.common import Box, Discrete
+    from xuance_b200.common.common_tools import get_arguments
+    from xuance_b200.torch.agents import COMA_Agents
+    from oracle_coma import COMALearnerOracle
+    B, n, T, od, A, sd = 8, 5, 60, 72, 12, 98
+    keys = ["agent_%d" % i for i in range(n)]
+    rng = np.random.default_rng(0)
+    S = B * n
+    lengths = np.tile(rng.integers(20, T + 1, B), n)
+    st = dict(obs=rng.uniform(-1, 1, (S, T, od)).astype(np.float32),
+              actions=rng.integers(0, A, (S, T)).astype(np.float32),
+              advantages=rng.normal(size=(S, T)).astype(np.float32), values=rng.normal(size=(S, T)).astype(np.float32),
+              returns=rng.normal(size=(S, T)).astype(np.float32),
+              agent_mask=(rng.random((S, T)) > 0.05).astype(np.float32),
+              filled=(np.arange(T)[None] < lengths[:, None]).astype(np.float32),
+              state=np.tile(rng.normal(size=(B, T, sd)).astype(np.float32), (n, 1, 1)))
+    sample = {'_stacked': {k: torch.from_numpy(v).to(DEV) for k, v in st.items()}, 'batch_size': B,
+              'sequence_length': T}
+    out = {"config": "COMA 5m_vs_6m shape: 8 episodes x 5 agents x T = 60 per update, Basic_RNN (fc 64, GRU 64, "
+                     "LayerNorm) actor and critic encoders, critic MLP 128-128, 12 actions, epsilon 0.5",
+           "gpu": subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                                 capture_output=True, text=True).stdout.strip()}
+    model = None
+    for graph in (False, True):
+        cfg = get_arguments("coma", "sc2", "5m_vs_6m")
+        for k, v in dict(device=DEV, parallels=8, logger=None, model_dir="/tmp/x", use_cuda_graph=graph,
+                         distributed_training=False, episode_length=T).items():
+            setattr(cfg, k, v)
+        torch.manual_seed(0)
+        agent = COMA_Agents(cfg, None, n, keys, Box(-1, 1, (sd,), np.float32),
+                            {k: Box(-1, 1, (od,), np.float32) for k in keys}, {k: Discrete(A) for k in keys})
+        if model is None:
+            model = copy.deepcopy(agent.model)
+        dt = timed(lambda: agent.learner.update(sample, 0.5, sync=False), max(5, args.iters // 10), warm=3)
+        out["gpu_ms_per_update_" + ("graph" if graph else "eager")] = dt * 1e3
+    if not args.no_cpu:
+        ol = COMALearnerOracle(model, (n, False, 0.5), cfg=vars(cfg))
+        t = {k: torch.from_numpy(v) for k, v in st.items()}
+        b = dict(obs=t['obs'].reshape(n, B, T, od).transpose(0, 1).reshape(S, T, od),
+                 **{k: t[f].reshape(n, B, T).transpose(0, 1).reshape(-1) for k, f in
+                    (("actions", "actions"), ("returns", "returns"))},
+                 mask=(t['agent_mask'] * t['filled']).reshape(n, B, T).transpose(0, 1).reshape(-1),
+                 avail=None, state=t['state'][:B], B=B, n=n, T=T)
+        cdt = cpu_timed(lambda: ol.update(b, 0.5), max(args.cpu_iters, 3))
+        out.update(cpu_ms_per_update=cdt * 1e3, cpu_threads=torch.get_num_threads(),
+                   speedup_eager=cdt * 1e3 / out["gpu_ms_per_update_eager"],
+                   speedup_graph=cdt * 1e3 / out["gpu_ms_per_update_graph"])
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=200)
@@ -759,6 +817,8 @@ def main():
             res[algo] = bench_dist_dqn(args, algo)
     if (not only and WORLD == 1) or "drqn" in only:
         res["drqn"] = bench_drqn(args)
+    if (not only and WORLD == 1) or "coma" in only:
+        res["coma"] = bench_coma(args)
     res["cuda_graph"] = bool(args.graph)
     res["n_gpus"] = WORLD
     if RANK == 0:

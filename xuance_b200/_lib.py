@@ -45,6 +45,9 @@ _SIGNATURES = {
     "xb_mappo_loss_fwd_bwd": (c_int, [_P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, c_int64,
                                       c_float, c_float, c_float, c_float, c_float, _P, _P, _P, _P, _P]),
     "xb_vdac_loss_fwd_bwd": (c_int, [_P, _P, c_int] + [_P] * 8 + [c_int64] + [c_int] * 5 + [c_int64] + [c_float] * 4 + [_P] * 5),
+    "xb_coma_critic_input": (c_int, [_P, _P, _P] + [c_int] * 6 + [_P, _P]),
+    "xb_coma_loss_fwd_bwd": (c_int, [_P, _P, c_int] + [_P] * 6 + [c_int64, c_int, c_int64] + [_P] * 5),
+    "xb_coma_act": (c_int, [_P, _P, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P]),
     "xb_per_insert": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_float, _P]),
     "xb_per_sample": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int64, c_float, _P, _P, _P, _P]),
     "xb_per_update": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_float, _P]),

@@ -37,3 +37,5 @@ REGISTRY_Agents["IPPO"] = IPPO_Agents
 from .vdac_agents import VDAC_Agents, IAC_Agents
 REGISTRY_Agents["VDAC"] = VDAC_Agents
 REGISTRY_Agents["IAC"] = IAC_Agents
+from .coma_agents import COMA_Agents
+REGISTRY_Agents["COMA"] = COMA_Agents

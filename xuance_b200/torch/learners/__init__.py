@@ -11,6 +11,7 @@ from .dcg_learner import DCG_Learner
 from .qtran_learner import QTRAN_Learner
 from .mappo_learner import MAPPO_Learner
 from .vdac_learner import VDAC_Learner, IAC_Learner
+from .coma_learner import COMA_Learner
 from .ppg_learner import PPG_Learner
 from .drqn_learner import DRQN_Learner
 
@@ -25,4 +26,4 @@ REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner,
                      "MAPPO_Learner": MAPPO_Learner, "PPG_Learner": PPG_Learner, "WQMIX_Learner": WQMIX_Learner,
                      "DCG_Learner": DCG_Learner, "QTRAN_Learner": QTRAN_Learner,
                      "VDAC_Learner": VDAC_Learner, "IAC_Learner": IAC_Learner,
-                     "DRQN_Learner": DRQN_Learner}
+                     "DRQN_Learner": DRQN_Learner, "COMA_Learner": COMA_Learner}

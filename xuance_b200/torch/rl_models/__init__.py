@@ -19,3 +19,4 @@ from .qtran import QTRAN_Base, QTRAN_Alt, QTranMixingNetwork
 from .vdac import IndependentActorCritic, ValueDecompositionActorCritic
 from .lstm import LSTMSequence, lstm_sequence
 from .drqn import RecurrentQValueHead, DeepRecurrentQNetwork
+from .coma import CounterfactualCentralizedCritic, CounterfactualMultiAgentActorCritic
