@@ -509,6 +509,39 @@ int xb_qtran_loss_fwd_bwd(int mode, const float *q_all, const float *actions, co
                           float lambda_opt, float lambda_nopt, int64_t rows_total, float *dqjt, float *dv,
                           float *dq_all, float *stats, double *scratch, void *stream);
 
+/* ---------------------------------------------------------------- K9I: IQL per-agent masked double-Q TD ----
+ * Replaces, for one parameter-sharing group with use_rnn=True, iql_learner.py:37-142 (_forward_transitions and the loss
+ * of update) plus the autograd backward of those lines down to the agent-network outputs.  Layouts as K9: q_all / q_tgt
+ * [B,n,T+1,A] (eval and target heads); actions, rewards, terminals, agent_mask [B,n,T] and filled [B,T] float32; avail
+ * (nullable) uint8 [B,n,T+1,avail_ld], non-zero = available.  Every (b,i,t) is its own loss row: rewards and terminals are
+ * the agent's own (no team reward, no all-agents terminal) and there is no mixer.
+ * prepare: msum[0] (float64) = sum(agent_mask * filled) over the B*n*T local rows (deterministic two-level reduction);
+ *          SUM-all-reduce it when the minibatch is sharded.
+ * td     : per row, m = agent_mask*filled (float32); g = the first maximal index of q_all at t+1 with unavailable actions
+ *          at -1e10 (value_factorization.py:86-91); q_next = q_tgt at t+1 with unavailable actions at -1e10, gathered at
+ *          g (double_q) or max-reduced; y = r + (1-d)*gamma*q_next, one float32 operation at a time in that order (no
+ *          FMA), so g, q_next and y are bit-exact against the reference's float32 expression; td = (q_all[t, a] - y)*m.
+ *          Writes the WHOLE dq_all [B,n,T+1,A] (no memset needed): (1/M)*(2*td)*m at the taken action, as autograd of
+ *          sum(td^2)/M forms it, zero elsewhere and on step T; and stats[2] = {loss_Q = sum(td^2)/M, predictQ =
+ *          sum(q_all[t, a])/rows_total over every row, masked or not, as the reference's .mean()}, each the local rows'
+ *          share.  M = msum[0] and rows_total >= B*n*T are GLOBAL, so a shard's dq rows are bit-equal to the whole-batch
+ *          launch and the SUM of the shards' statistics is the global value.  M = 0 gives 0/0 = NaN, as the reference.
+ *          Optional outputs (each nullable), [B,n,T]: next_actions (int32, g; written with or without double_q), q_next,
+ *          target (y).  An action outside [0, A) gets no gradient and makes the statistics NaN (the reference's gather
+ *          raises).  Tiles of 128 rows of q_all and q_tgt are staged through 2*129*(A|1)*4 bytes of shared memory; the
+ *          reduction is deterministic (scratch as for K4): outputs are bit-identical across launches.
+ * Both: B, n, T, A >= 1, avail_ld >= A and the required pointers (else XB_EINVAL); td: n <= 32, A <= 64 (else
+ * XB_ERANGE).  No allocation; graph-capturable. */
+#define XB_IQL_MAX_AGENTS 32
+#define XB_IQL_MAX_ACTIONS 64
+int xb_iql_prepare(const float *agent_mask, const float *filled, int B, int n, int T, double *msum, double *scratch,
+                   void *stream);
+int xb_iql_td_fwd_bwd(const float *q_all, const float *q_tgt, const float *actions, const float *rewards,
+                      const float *terminals, const float *agent_mask, const float *filled, const uint8_t *avail,
+                      int avail_ld, const double *msum, int B, int n, int T, int A, int double_q, float gamma,
+                      int64_t rows_total, float *dq_all, float *stats, double *scratch, int32_t *next_actions,
+                      float *q_next, float *target, void *stream);
+
 /* Tensor-core forward of the whole mixer (hypernet GEMMs + epilogue in ONE kernel; wgmma with register
  * accumulators, bf16 hi/lo split operands, 3 MMAs per product, fp32 accumulate): q_tot[R] from states[R,S], q[R,n]
  * and the raw Linear parameters of QMIX_Mixer (q_mix_head.py:52-64): w_l1[4] / b_l1[4] are HOST arrays of 4 device

@@ -7,6 +7,7 @@ configs/mappo/sc2/5m_vs_6m.yaml (train_epochs env-steps/s); ``mappo_rnn``, recur
 configs/mappo/sc2/3m.yaml (update, eager and graphed); ``wqmix``, CW-QMIX in the shape of configs/wqmix/sc2/5m_vs_6m.yaml
 (update, eager and graphed); ``dcg``, DCG in the shape of configs/dcg/sc2/5m_vs_6m.yaml (update, eager and graphed);
 ``qtran``, QTRAN_alt in the shape of configs/qtran/sc2/5m_vs_6m.yaml (update, eager and graphed);
+``iql``, IQL in the shape of configs/iql/sc2/5m_vs_6m.yaml (update, eager and graphed);
 ``vdac``, VDAC (QMIX mixer) in the shape of configs/vdac/sc2/5m_vs_6m.yaml (update, eager and graphed);
 ``sacdis``, SAC-Discrete in the shape of
 configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (train_epochs, eager and graphed); ``ddpg`` and
@@ -313,6 +314,41 @@ def bench_qtran(args, B=32):
         out["gpu_ms_per_update_graphed" if graph else "gpu_ms_per_update_eager"] = dt * 1e3
     if not args.no_cpu:
         orc = QTRANOracle(model, total_iters=10**6)
+        cdt = cpu_timed(lambda: orc.update(sample), max(args.cpu_iters, 5))
+        out.update(cpu_ms_per_update=cdt * 1e3, cpu_threads=torch.get_num_threads(),
+                   speedup_graphed=cdt * 1e3 / out["gpu_ms_per_update_graphed"])
+    return out
+
+
+def bench_iql(args, B=32):
+    """One IQL_Learner update in the shape of configs/iql/sc2/5m_vs_6m.yaml (5 agents x 72-d, A=12, T=60, 32 episodes,
+    K13 GRU 64, Q head 64, double-Q, action masks), eager and graphed, on a device-resident sample; next to the torch-CPU
+    float64 oracle of the same update."""
+    import wqmix_refs as R
+    from oracle_iql import IQLOracle, build_model
+    from xuance_b200.common import BaseCallback
+    from xuance_b200.torch.learners import REGISTRY_Learners
+    n, od, A, T = 5, 72, 12, 60
+    keys = [f"agent_{i}" for i in range(n)]
+    sample = R.fix_sample(np.random.default_rng(0), keys, B=B, T=T, obs_dim=od, A=A, S=4)
+    dev = lambda x: {k: dev(v) for k, v in x.items()} if isinstance(x, dict) else (
+        torch.as_tensor(x, device=DEV) if isinstance(x, np.ndarray) else x)
+    dsample = dev(sample)
+    out = {"config": f"IQL, 5 agents x 72-d, A=12, T=60, {B} episodes/update, GRU 64, Q head 64, double-Q, "
+                     f"action masks"}
+    for graph in (False, True):
+        torch.manual_seed(0)
+        _, grouping, model = build_model(n, od, A, 64, DEV)
+        cfg = Namespace(agent="IQL", distributed_training=False, episode_length=T, use_grad_clip=False,
+                        grad_clip_norm=0.5, device=DEV, model_dir="/tmp/x", running_steps=10**7, parallels=8,
+                        use_parameter_sharing=True, use_rnn=True, use_actions_mask=True, learning_rate=7e-4,
+                        sync_frequency=200, n_epochs=1, start_training=0, gamma=0.99, double_q=True,
+                        use_cuda_graph=graph)
+        lrn = REGISTRY_Learners["IQL_Learner"](cfg, grouping, model, BaseCallback())
+        dt = timed(lambda: lrn.update(dsample, sync=False), args.iters)
+        out["gpu_ms_per_update_graphed" if graph else "gpu_ms_per_update_eager"] = dt * 1e3
+    if not args.no_cpu:
+        orc = IQLOracle(model, total_iters=10**6)
         cdt = cpu_timed(lambda: orc.update(sample), max(args.cpu_iters, 5))
         out.update(cpu_ms_per_update=cdt * 1e3, cpu_threads=torch.get_num_threads(),
                    speedup_graphed=cdt * 1e3 / out["gpu_ms_per_update_graphed"])
@@ -799,6 +835,8 @@ def main():
         res["dcg"] = bench_dcg(args)
     if (not only and WORLD == 1) or "qtran" in only:
         res["qtran"] = bench_qtran(args)
+    if (not only and WORLD == 1) or "iql" in only:
+        res["iql"] = bench_iql(args)
     if (not only and WORLD == 1) or "ppo_gauss" in only:
         res["ppo_gauss"] = bench_ppo_gauss(args)
     if (not only and WORLD == 1) or "mappo" in only:

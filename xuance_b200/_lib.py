@@ -113,6 +113,8 @@ _SIGNATURES = {
     "xb_qtran_encode_bwd_work": (c_int64, [c_int] * 5),
     "xb_qtran_encode_bwd": (c_int, [c_int] + [_P] * 5 + [c_int] + [_P] * 3 + [c_int] * 6 + [_P] * 6 + [c_int64, _P]),
     "xb_qtran_loss_fwd_bwd": (c_int, [c_int] + [_P] * 13 + [c_int] * 4 + [c_float] * 3 + [c_int64] + [_P] * 6),
+    "xb_iql_prepare": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, _P]),
+    "xb_iql_td_fwd_bwd": (c_int, [_P] * 8 + [c_int, _P] + [c_int] * 5 + [c_float, c_int64] + [_P] * 7),
     "xb_powf_libm": (c_int, [_P, c_float, _P, c_int64, _P]),
 }
 _OPTIONAL = {}

@@ -31,6 +31,8 @@ REGISTRY_Agents["DCG_S"] = DCG_Agents
 from .qtran_agents import QTRAN_Agents
 REGISTRY_Agents["QTRAN_base"] = QTRAN_Agents
 REGISTRY_Agents["QTRAN_alt"] = QTRAN_Agents
+from .iql_agents import IQL_Agents
+REGISTRY_Agents["IQL"] = IQL_Agents
 from .mappo_agents import OnPolicyMARLAgents, MAPPO_Agents, IPPO_Agents
 REGISTRY_Agents["MAPPO"] = MAPPO_Agents
 REGISTRY_Agents["IPPO"] = IPPO_Agents

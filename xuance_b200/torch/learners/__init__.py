@@ -9,6 +9,7 @@ from .qmix_learner import QMIX_Learner
 from .wqmix_learner import WQMIX_Learner
 from .dcg_learner import DCG_Learner
 from .qtran_learner import QTRAN_Learner
+from .iql_learner import IQL_Learner
 from .mappo_learner import MAPPO_Learner
 from .vdac_learner import VDAC_Learner, IAC_Learner
 from .coma_learner import COMA_Learner
@@ -24,6 +25,6 @@ REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner,
                      "QMIX_Learner": QMIX_Learner,
                      "VDN_Learner": QMIX_Learner,     # vdn_learner.py: the same update with the parameter-free sum mixer
                      "MAPPO_Learner": MAPPO_Learner, "PPG_Learner": PPG_Learner, "WQMIX_Learner": WQMIX_Learner,
-                     "DCG_Learner": DCG_Learner, "QTRAN_Learner": QTRAN_Learner,
+                     "DCG_Learner": DCG_Learner, "QTRAN_Learner": QTRAN_Learner, "IQL_Learner": IQL_Learner,
                      "VDAC_Learner": VDAC_Learner, "IAC_Learner": IAC_Learner,
                      "DRQN_Learner": DRQN_Learner, "COMA_Learner": COMA_Learner}

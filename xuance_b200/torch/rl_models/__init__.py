@@ -10,7 +10,7 @@ from .architectures import (ActorCritic, SharedActorCritic, DeepQNetwork, Duelin
                             DeterministicActor, ActionValueCritic, DeterministicActorCritic, TwinDelayedActorCritic,
                             C51DeepQNetwork, QRDeepQNetwork, StateValueCritic, PhasicActorCritic)
 from .qmix import (Basic_RNN, AgentFeatureEncoder, DiscreteActionValueCritic, QMIX_Mixer, VDN_mixer, MixingQNetwork,
-                   QMIX_FF_Mixer, WeightedMixingQNetwork)
+                   QMIX_FF_Mixer, WeightedMixingQNetwork, IndependentMixer)
 REGISTRY_Representation["Basic_RNN"] = Basic_RNN
 from .mappo import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic
 from .gru import GRUSequence, gru_sequence, Basic_RNN_K13

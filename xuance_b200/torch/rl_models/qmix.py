@@ -192,6 +192,14 @@ class VDN_mixer(nn.Module):
         return values_n.reshape(values_n.shape[0] if values_n.dim() == 2 else -1, -1).sum(dim=-1, keepdim=True)
 
 
+class IndependentMixer(nn.Module):
+    """q_mix_head.py IndependentMixer: independent Q-learning, the agents' values pass through (no parameters).  IQL's
+    update never calls it: its loss is per agent (K9I)."""
+
+    def forward(self, values_n, states=None):
+        return values_n
+
+
 class MixingQNetwork(nn.Module):
     """value_factorization.py:17-174 for one shared group: eval/target agent networks + eval/target mixers."""
 
