@@ -170,6 +170,43 @@ int xb_ppg_aux_gauss_loss_fwd_bwd(const float *mu, const float *log_std, const f
                                   int64_t B_total, float kl_beta, float *dmu, float *dlog_std, float *dvalue,
                                   float *daux, float *stats, double *scratch, void *stream);
 
+/* ---------------------------------------------------------------- K4N: fused NPG loss fwd+bwd ---------
+ * npg_learner.py:37-43 plus the two backward seeds the update needs (no B_total: NPG runs on one GPU):
+ *   log pi_b = Categorical(logits).log_prob(a) or sum_j Normal(mu_j, exp(log_std_j)).log_prob(x_j)
+ *   a_loss = -mean(adv * log pi); c_loss = mean((v - R)^2)
+ * Writes the loss seed d a_loss / d outputs, the score seed d(sum_b log pi_b) / d outputs, dvalue[B] = 2 (v - R) / B,
+ * stats[8] = {a_loss, c_loss, mean(v), sum log pi, 0, 0, 0, 0} and *logp_sum = sum log pi in fp64 (K7N's kappa).
+ * One warp per row; fixed-order reductions (bit-identical from launch to launch); no allocation; graph-capturable.
+ * actions are float32.  scratch as for K4.
+ * xb_npg_loss_fwd_bwd (Categorical): logits [B, A], 1 <= A <= 64 (else XB_ERANGE); dlogits / dscore [B, A].
+ * xb_npg_gauss_loss_fwd_bwd (DiagGaussian): mu / actions [B, D], log_std [D], 1 <= D <= 64 (else XB_ERANGE); dmu / smu
+ *   [B, D] (loss / score seeds), dlog_std / slog_std [D] their column sums over B.  ws: >= xb_npg_gauss_ws_doubles(B, D)
+ *   doubles (2 D min(ceil(B / 8), 2048)) for the per-block column partials, added in block order; ws_doubles is its
+ *   size (XB_EINVAL if too small). */
+int xb_npg_loss_fwd_bwd(const float *logits, const float *value, const float *actions, const float *adv,
+                        const float *ret, int64_t B, int A, float *dlogits, float *dscore, float *dvalue,
+                        float *stats, double *logp_sum, double *scratch, void *stream);
+int64_t xb_npg_gauss_ws_doubles(int64_t B, int D);
+int xb_npg_gauss_loss_fwd_bwd(const float *mu, const float *log_std, const float *value, const float *actions,
+                              const float *adv, const float *ret, int64_t B, int D, float *dmu, float *dlog_std,
+                              float *smu, float *slog_std, float *dvalue, float *stats, double *logp_sum,
+                              double *scratch, double *ws, int64_t ws_doubles, void *stream);
+
+/* ---------------------------------------------------------------- K7N: NPG natural gradient ------------
+ * npg_learner.py:54-62 and 100-113 in closed form.  For each segment i (one actor parameter tensor) of the flat
+ * gradient g, with s the score gradient in the same layout, kappa = *logp_sum / horizon and the reference's
+ * F = kappa s s^T + lam I, Sherman-Morrison gives, in place:
+ *   g <- (g - s * kappa (s.g) / (lam + kappa s.s)) / lam
+ * The dot products accumulate in fp64: one partial per chunk of 4096 elements, folded in chunk order (bit-identical from
+ * launch to launch).  Two launches, no host synchronisation; a zero denominator is not guarded.
+ * xb_npg_segment_table (host only): table[3 * nseg] = {offset, length, first chunk} from the segments' element
+ *   offsets and lengths (length >= 1); returns the chunk count, or XB_EINVAL.  Upload the table once.
+ * xb_npg_natural_grad: table on the device, nchunks as returned; ws >= 2 * nchunks doubles; horizon > 0, lam > 0. */
+int64_t xb_npg_segment_table(const int64_t *offsets, const int64_t *lengths, int nseg, int64_t *table);
+int xb_npg_natural_grad(float *g, const float *s, const int64_t *table, int nseg, int64_t nchunks,
+                        const double *logp_sum, double horizon, double lam, double *ws, int64_t ws_doubles,
+                        void *stream);
+
 /* ---------------------------------------------------------------- K4M: fused MAPPO loss fwd+bwd -------
  * Replaces mappo_learner.py:55-113 (one parameter-sharing group, feed-forward actor and critic, Discrete actions) plus
  * the autograd backward of those lines down to (logits, value).  One row = one agent at one env step.

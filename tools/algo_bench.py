@@ -14,8 +14,9 @@ configs/sac/CartPole-v1.yaml and at 18 actions with automatic entropy tuning (tr
 ``td3``, DDPG / TD3 in the shape of the reference's ddpg/mujoco.yaml and td3/mujoco.yaml (sample + update, eager and
 graphed); ``c51`` and ``qrdqn`` on CartPole (Basic_MLP 128, B=256) and SyntheticAtari (Basic_CNN, B=32) shapes (update,
 eager and graphed); ``drqn``, DRQN in the shape of configs/drqn/classic_control/CartPole-v1.yaml (update, eager and
-graphed); ``coma``, COMA in the shape of configs/coma/sc2/5m_vs_6m.yaml (update, eager and graphed).  Prints one JSON
-object.
+graphed); ``coma``, COMA in the shape of configs/coma/sc2/5m_vs_6m.yaml (update, eager and graphed); ``npg``, NPG in
+the shapes of configs/npg/classic_control/{CartPole,Pendulum}-v1.yaml (update, eager and graphed, next to the reference's
+dense float32 inverse restated on the GPU).  Prints one JSON object.
 
     python tools/algo_bench.py [--iters 200] [--cpu-iters 5] [--no-cpu] [--graph]
     torchrun --nnodes=1 --nproc-per-node G --master-addr 127.0.0.1 tools/algo_bench.py --no-cpu --graph    (G GPUs)
@@ -802,6 +803,82 @@ def bench_coma(args):
     return out
 
 
+def _gpu_identity():
+    """The card's name and power limit, read next to the measurement."""
+    import subprocess
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(LOCAL)],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.TimeoutExpired):
+        q = "nvidia-smi unavailable"
+    return {"device": torch.cuda.get_device_name(LOCAL), "nvidia_smi": q}
+
+
+def bench_npg(args, repeats=3):
+    """One NPG_Learner update in the shapes of the shipped configs: CartPole-v1 (Basic_MLP 128, actor / critic 128, 2
+    actions, 10 envs x 256 steps in 8 minibatches: B = 320) and Pendulum-v1 (Basic_MLP 256, actor 256, critic 256, 1 action
+    component, 10 x 128 in one minibatch: B = 1280), eager and graphed, on device-resident samples, repeated ``repeats``
+    times.  Next to it, the reference's natural gradient of ONE CartPole-shape minibatch restated on the GPU: per actor
+    tensor a dense float32 P x P F = kappa s s^T + 1e-3 I, torch.linalg.inv(F) and F^-1 g (the largest P is 16384)."""
+    from xuance_b200.common import Box, Discrete
+    from xuance_b200.common.common_tools import get_arguments
+    from xuance_b200.torch.agents import REGISTRY_Agents
+    out = {"gpu": _gpu_identity()}
+    shapes = {"cartpole": ("CartPole-v1", Box(-5, 5, (4,), np.float32), Discrete(2)),
+              "pendulum": ("Pendulum-v1", Box(-8, 8, (3,), np.float32), Box(-2, 2, (1,), np.float32))}
+    for name, (env_id, obs_space, act_space) in shapes.items():
+        res = {}
+        for graph in (False, True):
+            cfg = get_arguments("npg", "classic_control", env_id,
+                                parser_args=Namespace(device=DEV, use_cuda_graph=graph, model_dir="/tmp/xb_npg_bench"))
+            torch.manual_seed(0)
+            agent = REGISTRY_Agents["NPG"](cfg, None, obs_space, act_space)
+            B = agent.batch_size
+            rng = np.random.default_rng(0)
+            acts = (rng.normal(size=(B, 1)) * 0.4) if isinstance(act_space, Box) else rng.integers(0, 2, B)
+            s = {"obs": torch.as_tensor(rng.normal(size=(B,) + obs_space.shape), dtype=torch.float32, device=DEV),
+                 "actions": torch.as_tensor(acts, dtype=torch.float32, device=DEV),
+                 "returns": torch.as_tensor(rng.normal(size=B), dtype=torch.float32, device=DEV),
+                 "advantages": torch.as_tensor(rng.normal(size=B), dtype=torch.float32, device=DEV)}
+            lrn = agent.learner
+            key = "gpu_ms_per_update_graphed" if graph else "gpu_ms_per_update_eager"
+            res[key] = [timed(lambda: lrn.update(sync=False, **s), args.iters) * 1e3 for _ in range(repeats)]
+            res["B"], res["actor_params"] = B, [p.numel() for p in agent.model.actor.parameters()]
+        out[name] = res
+        if name == "cartpole":
+            out["cartpole_dense_inverse_restatement"] = _npg_dense_restatement(agent, s, repeats)
+    return out
+
+
+def _npg_dense_restatement(agent, s, repeats):
+    """The reference's F^-1 g (npg_learner.py:100-113) for one minibatch, restated on the GPU in float32 (the reference
+    itself runs this on whatever device the learner uses): one dense inverse per actor tensor."""
+    model, H = agent.model, agent.config.horizon_size
+    params = list(model.actor.parameters())
+    logits = model.logits(s["obs"])
+    logp = torch.distributions.Categorical(logits=logits).log_prob(s["actions"].long())
+    scores = [x.reshape(-1) for x in torch.autograd.grad(logp.sum(), params, retain_graph=True)]
+    grads = [x.reshape(-1) for x in torch.autograd.grad(-(s["advantages"] * logp).mean(), params)]
+    kappa = logp.sum().item() / H
+
+    def step():
+        for sc, g in zip(scores, grads):
+            F = torch.outer(sc, sc) * kappa + 1e-3 * torch.eye(sc.numel(), device=DEV)
+            torch.linalg.inv(F) @ g
+    step()
+    torch.cuda.synchronize()
+    times = []
+    for _ in range(repeats):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        step()
+        e1.record()
+        torch.cuda.synchronize()
+        times.append(e0.elapsed_time(e1))
+    return {"what": "restatement of the reference's dense float32 inverse, one CartPole-shape minibatch (B = %d)"
+            % s["actions"].shape[0], "largest_P": max(x.numel() for x in scores), "gpu_ms_per_minibatch": times}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=200)
@@ -857,6 +934,8 @@ def main():
         res["drqn"] = bench_drqn(args)
     if (not only and WORLD == 1) or "coma" in only:
         res["coma"] = bench_coma(args)
+    if (not only and WORLD == 1) or "npg" in only:
+        res["npg"] = bench_npg(args)
     res["cuda_graph"] = bool(args.graph)
     res["n_gpus"] = WORLD
     if RANK == 0:

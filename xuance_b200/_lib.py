@@ -40,6 +40,11 @@ _SIGNATURES = {
                                         _P]),
     "xb_ppg_aux_gauss_loss_fwd_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int64, c_int, c_int64, c_float, _P, _P,
                                               _P, _P, _P, _P, _P]),
+    "xb_npg_loss_fwd_bwd": (c_int, [_P] * 5 + [c_int64, c_int] + [_P] * 7),
+    "xb_npg_gauss_ws_doubles": (c_int64, [c_int64, c_int]),
+    "xb_npg_gauss_loss_fwd_bwd": (c_int, [_P] * 6 + [c_int64, c_int] + [_P] * 9 + [c_int64, _P]),
+    "xb_npg_segment_table": (c_int64, [_P, _P, c_int, _P]),
+    "xb_npg_natural_grad": (c_int, [_P, _P, _P, c_int, c_int64, _P, c_double, c_double, _P, c_int64, _P]),
     "xb_mappo_prepare": (c_int, [_P, _P, c_int64, _P, _P, _P]),
     "xb_value_norm_update": (c_int, [_P, _P, _P, _P, c_int64, c_double, _P, _P]),
     "xb_mappo_loss_fwd_bwd": (c_int, [_P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, c_int64,

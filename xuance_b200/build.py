@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libxb200.so")
 STAMP = os.path.join(HERE, ".libxb200.stamp")
-SOURCES = ["api.cu", "rollout.cu", "losses.cu", "per_tree.cu", "optim.cu", "sac.cu", "ddpg.cu", "dist_dqn.cu", "ppg.cu", "gru.cu", "lstm.cu", "qmix_mix.cu", "qmix_tc.cu", "wqmix.cu", "dcg.cu", "qtran.cu", "iql.cu", "vdac.cu", "coma.cu", "act.cu", "conv_tc.cu", "obs_planes.cu"]
+SOURCES = ["api.cu", "rollout.cu", "losses.cu", "per_tree.cu", "optim.cu", "sac.cu", "ddpg.cu", "dist_dqn.cu", "ppg.cu", "npg.cu", "gru.cu", "lstm.cu", "qmix_mix.cu", "qmix_tc.cu", "wqmix.cu", "dcg.cu", "qtran.cu", "iql.cu", "vdac.cu", "coma.cu", "act.cu", "conv_tc.cu", "obs_planes.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--use_fast_math=false", "-ftz=false", "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v",
               "--expt-relaxed-constexpr", "--expt-extended-lambda"]

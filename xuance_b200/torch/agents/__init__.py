@@ -5,12 +5,14 @@ from .ppo_agent import PPO_Agent
 from .dqn_agent import DQN_Agent, PerDQN_Agent, DuelDQN_Agent
 from .dist_dqn_agent import C51_Agent, QRDQN_Agent
 from .ppg_agent import PPG_Agent
+from .npg_agent import NPG_Agent
 # DRQN_Agent is constructed directly, DRQN_Agent(config, envs): adding it to REGISTRY_Agents (and so to get_runner) is a
 # separate change, because the registry's keys are pinned by the C51 / QR-DQN tests
 from .drqn_agent import DRQN_Agent
 
 REGISTRY_Agents = {"PPO": PPO_Agent, "PPO_Clip": PPO_Agent, "DQN": DQN_Agent, "PerDQN": PerDQN_Agent, "DuelDQN": DuelDQN_Agent,
-                   "C51DQN": C51_Agent, "QRDQN": QRDQN_Agent, "PPG": PPG_Agent}
+                   "C51DQN": C51_Agent, "QRDQN": QRDQN_Agent, "PPG": PPG_Agent,
+                   "NPG": NPG_Agent}
 try:
     from .sac_agent import SAC_Agent
     REGISTRY_Agents["SAC"] = SAC_Agent

@@ -14,6 +14,7 @@ from .mappo_learner import MAPPO_Learner
 from .vdac_learner import VDAC_Learner, IAC_Learner
 from .coma_learner import COMA_Learner
 from .ppg_learner import PPG_Learner
+from .npg_learner import NPG_Learner
 from .drqn_learner import DRQN_Learner
 
 REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner, "DQN_Learner": DQN_Learner,
@@ -24,7 +25,7 @@ REGISTRY_Learners = {"PPO_Learner": PPO_Learner, "PPOCLIP_Learner": PPO_Learner,
                      "DDPG_Learner": DDPG_Learner, "TD3_Learner": TD3_Learner,
                      "QMIX_Learner": QMIX_Learner,
                      "VDN_Learner": QMIX_Learner,     # vdn_learner.py: the same update with the parameter-free sum mixer
-                     "MAPPO_Learner": MAPPO_Learner, "PPG_Learner": PPG_Learner, "WQMIX_Learner": WQMIX_Learner,
+                     "MAPPO_Learner": MAPPO_Learner, "PPG_Learner": PPG_Learner, "NPG_Learner": NPG_Learner, "WQMIX_Learner": WQMIX_Learner,
                      "DCG_Learner": DCG_Learner, "QTRAN_Learner": QTRAN_Learner, "IQL_Learner": IQL_Learner,
                      "VDAC_Learner": VDAC_Learner, "IAC_Learner": IAC_Learner,
                      "DRQN_Learner": DRQN_Learner, "COMA_Learner": COMA_Learner}

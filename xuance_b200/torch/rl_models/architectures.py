@@ -14,7 +14,9 @@ from .outputs import ModelOutput, StochasticActorOutput, TwinCriticOutput, Deter
 
 
 class ActorCritic(nn.Module):
-    """actor_critic.py:8-37 (separate actor / critic modules each owning a representation)."""
+    """actor_critic.py:8-37 (separate actor / critic modules each owning a representation).  ``logits`` / ``mu_log_std``
+    and ``forward_raw`` / ``forward_raw_gauss`` give the raw actor outputs (a CategoricalActor's logits, a GaussianActor's
+    mu and log_std) and a StateValueCritic's values, the tensors the fused loss and acting kernels consume."""
 
     def __init__(self, actor, critic, **kwargs):
         super().__init__()
@@ -28,6 +30,22 @@ class ActorCritic(nn.Module):
     def act(self, observation, deterministic=False, **kwargs):
         d = self.actor(observation, **kwargs).distributions
         return d.deterministic_sample() if deterministic else d.stochastic_sample()
+
+    def logits(self, observation):
+        return self.actor.logits(observation)
+
+    def mu_log_std(self, observation):
+        head = self.actor.actor_head
+        return head.mu(self.actor.representation(observation).embeddings), head.log_std
+
+    def forward_raw(self, observation):
+        """(logits [B, A], values [B])."""
+        return self.logits(observation), self.critic.values(observation)
+
+    def forward_raw_gauss(self, observation):
+        """(mu [B, D], log_std [D], values [B])."""
+        mu, log_std = self.mu_log_std(observation)
+        return mu, log_std, self.critic.values(observation)
 
 
 class SharedActorCritic(nn.Module):
@@ -549,28 +567,11 @@ class PhasicActorCritic(ActorCritic):
     """actor_critic.py:75-104: an actor (CategoricalActor or GaussianActor) and two StateValueCritics, each with its own
     representation, sharing no parameter.  ``forward`` returns the actor's distribution and ``critic``'s values.
     Parameters are registered actor, critic, aux_critic: ``parameters()`` lists the three groups in that order, the
-    layout the PPG learner's per-group Adam steps by range.  ``forward_raw`` / ``forward_raw_gauss`` give the raw actor
-    outputs and ``critic``'s values, the tensors the fused loss and acting kernels consume."""
+    layout the PPG learner's per-group Adam steps by range.  The raw-output methods are ActorCritic's."""
 
     def __init__(self, actor, critic, aux_critic, **kwargs):
         super().__init__(actor, critic, **kwargs)
         self.aux_critic = aux_critic
-
-    def logits(self, observation):
-        return self.actor.logits(observation)
-
-    def mu_log_std(self, observation):
-        head = self.actor.actor_head
-        return head.mu(self.actor.representation(observation).embeddings), head.log_std
-
-    def forward_raw(self, observation):
-        """(logits [B, A], values [B])."""
-        return self.logits(observation), self.critic.values(observation)
-
-    def forward_raw_gauss(self, observation):
-        """(mu [B, D], log_std [D], values [B])."""
-        mu, log_std = self.mu_log_std(observation)
-        return mu, log_std, self.critic.values(observation)
 
     def aux_values(self, observation):
         """``aux_critic``'s [B] values."""
