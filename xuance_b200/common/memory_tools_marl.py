@@ -21,14 +21,16 @@ def _pad4(n):
     return (n + 3) // 4 * 4
 
 
-class MARL_OffPolicyBuffer_RNN:
-    def __init__(self, agent_keys, state_space=None, obs_space=None, act_space=None, n_envs=1, buffer_size=1,
-                 batch_size=1, max_episode_steps=1, device="cuda:0", **kwargs):
-        assert buffer_size % n_envs == 0, "buffer_size must be divisible by the number of envs (parallels)"
+class _MARLBuffer:
+    """The construction every multi-agent buffer shares: one parameter-sharing group (all agents with the same
+    observation and action shapes), Discrete actions (each subclass refuses a Box with its ``BOX_REFUSAL``) and
+    storage on a CUDA device."""
+    BOX_REFUSAL = None
+
+    def __init__(self, agent_keys, state_space, obs_space, act_space, n_envs, buffer_size, device, **kwargs):
         self.agent_keys = list(agent_keys)
         self.n_agents = len(self.agent_keys)
-        self.n_envs, self.buffer_size, self.batch_size = n_envs, buffer_size, batch_size
-        self.max_eps_len = max_episode_steps
+        self.n_envs, self.buffer_size = n_envs, buffer_size
         self.state_space = state_space
         self.store_global_state = state_space is not None
         self.use_actions_mask = kwargs.get("use_actions_mask", False)
@@ -39,7 +41,7 @@ class MARL_OffPolicyBuffer_RNN:
         if any(self.obs_shape[k] != self.obs_shape[k0] or self.act_shape[k] != self.act_shape[k0] for k in self.agent_keys):
             raise NotImplementedError("heterogeneous agents are outside the hot-path scope (one parameter-sharing group)")
         if self.act_shape[k0] != ():
-            raise NotImplementedError("QMIX uses discrete actions")
+            raise NotImplementedError(self.BOX_REFUSAL)
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError("xuance_b200 buffers are device-resident: device must be CUDA (no CPU fallback)")
@@ -48,6 +50,72 @@ class MARL_OffPolicyBuffer_RNN:
         self._obs_dim = int(np.prod(self.obs_shape[k0]))
         self._state_dim = int(np.prod(space2shape(state_space))) if self.store_global_state else 0
         self._n_act = int(self.avail_actions_shape[k0][0]) if self.use_actions_mask else 0
+
+    def _gather_rows(self, src, idx_t):
+        """K3: src[idx_t] for rows of src.shape[1:]."""
+        out = torch.empty((idx_t.numel(),) + tuple(src.shape[1:]), dtype=src.dtype, device=self.device)
+        row_bytes = int(np.prod(src.shape[1:])) * src.element_size()
+        _lib.call("xb_gather_rows", _lib.ptr(src), _lib.ptr(idx_t), idx_t.numel(), row_bytes, _lib.ptr(out))
+        return out
+
+
+class _MARLOnPolicyBuffer(_MARLBuffer):
+    """What the two on-policy buffers share: the scalar fields, the (env, agent) rows, the GAE launch and the per-agent
+    split of a sample."""
+    FIELDS = ('actions', 'rewards', 'values', 'log_pi_old', 'terminals', 'agent_mask', 'returns', 'advantages')
+    STORED = 6   # the fields store() writes; returns / advantages come from finish_path
+
+    def __init__(self, agent_keys, state_space, obs_space, act_space, n_envs, buffer_size, use_gae, use_advnorm, gamma,
+                 gae_lam, device, **kwargs):
+        super().__init__(agent_keys, state_space, obs_space, act_space, n_envs, buffer_size, device, **kwargs)
+        self.use_gae, self.use_advantage_norm = use_gae, use_advnorm
+        self.gamma, self.gae_lambda = gamma, gae_lam
+        self._rows = self.n_envs * self.n_agents
+
+    def _per_agent(self, d, dtype=np.float32):
+        """{agent: [n_envs, ...]} -> [n_envs * n_agents, ...] (env-major, agent-minor)."""
+        return np.stack([np.asarray(d[k], dtype=dtype) for k in self.agent_keys], axis=1).reshape(self._rows, -1)
+
+    def _gae(self, rows, seg_end, boot, start, cov, agent_grouping, value_normalizer):
+        """``xb_gae_scan_vn`` over the agent rows ``rows`` of ``field()``: advantages and returns of the path that ends
+        where ``seg_end`` marks it (bootstrapping from ``boot``), on the steps [start, cov) of each row (start None: 0),
+        with the values denormalised by the group's ValueNorm state as it is now."""
+        vn = None
+        if value_normalizer is not None:
+            groups = {agent_grouping.agent_to_group[k] for k in self.agent_keys} if agent_grouping is not None \
+                else set(value_normalizer)
+            if len(groups) != 1:
+                raise NotImplementedError("one parameter-sharing group")
+            vn = value_normalizer[groups.pop()]
+        vp = vn.state_pointers() if vn is not None else (None, None, None)
+        f = lambda name: _lib.ptr(self.field(name)[rows])
+        _lib.call("xb_gae_scan_vn", f('rewards'), f('values'), f('terminals'), _lib.ptr(seg_end), _lib.ptr(boot),
+                  _lib.ptr(start), _lib.ptr(cov), f('advantages'), f('returns'), self.n_agents,
+                  self.field('rewards').shape[1], float(self.gamma),
+                  float(self.gae_lambda if self.gae_lambda is not None else 0.0), 1 if self.use_gae else 0, *vp)
+
+    def _split(self, st, B):
+        """The agent-major stacked sample (row k * B + b is agent k of sample b) as per-agent views under the
+        reference's keys; the per-sample ``filled`` and ``state`` keep agent 0's rows."""
+        out = {}
+        for key, v in st.items():
+            if key == 'avail_actions':
+                v = v[..., :self._n_act]
+            if key in ('terminals', 'agent_mask', 'avail_actions', 'filled'):
+                v = v.bool()
+            out[key] = v[:B] if key in ('filled', 'state') else {a: v[i * B:(i + 1) * B]
+                                                                 for i, a in enumerate(self.agent_keys)}
+        return out
+
+
+class MARL_OffPolicyBuffer_RNN(_MARLBuffer):
+    BOX_REFUSAL = "QMIX uses discrete actions"
+
+    def __init__(self, agent_keys, state_space=None, obs_space=None, act_space=None, n_envs=1, buffer_size=1,
+                 batch_size=1, max_episode_steps=1, device="cuda:0", **kwargs):
+        assert buffer_size % n_envs == 0, "buffer_size must be divisible by the number of envs (parallels)"
+        super().__init__(agent_keys, state_space, obs_space, act_space, n_envs, buffer_size, device, **kwargs)
+        self.batch_size, self.max_eps_len = batch_size, max_episode_steps
         self.clear()
         self.clear_episodes()
 
@@ -143,14 +211,6 @@ class MARL_OffPolicyBuffer_RNN:
         self.size = min(self.size + 1, self.buffer_size)
         ep['filled'][i_env] = 0
 
-    def _gather(self, key, idx_t):
-        src = self._dev[key]
-        row_shape = tuple(src.shape[1:])
-        row_bytes = int(np.prod(row_shape)) * src.element_size()
-        out = torch.empty((idx_t.numel(),) + row_shape, dtype=src.dtype, device=self.device)
-        _lib.call("xb_gather_rows", _lib.ptr(src), _lib.ptr(idx_t), idx_t.numel(), row_bytes, _lib.ptr(out))
-        return out
-
     # ---- reference :971-996
     def sample(self, batch_size=None, episode_choices=None):
         assert self.size > 0, "You need to first store experience data into the buffer!"
@@ -160,7 +220,7 @@ class MARL_OffPolicyBuffer_RNN:
             episode_choices = np.random.choice(self.size, batch_size)
         idx_t = torch.from_numpy(np.asarray(episode_choices, dtype=np.int64)).to(self.device)
         T, A = self.max_eps_len, self._n_act
-        st = {k: self._gather(k, idx_t) for k in self._dev}
+        st = {k: self._gather_rows(v, idx_t) for k, v in self._dev.items()}
         st['terminals'] = st['terminals'][:, :, :T].bool()
         st['agent_mask'] = st['agent_mask'][:, :, :T].bool()
         st['filled'] = st['filled'][:, :T].bool()
@@ -175,7 +235,7 @@ class MARL_OffPolicyBuffer_RNN:
         return out
 
 
-class MARL_OnPolicyBuffer:
+class MARL_OnPolicyBuffer(_MARLOnPolicyBuffer):
     """On-policy multi-agent rollout - mirror of MARL_OnPolicyBuffer (xuance/common/memory_tools_marl.py:63-270):
     ``store(**step_data)``, ``finish_path(i_env, agent_grouping, value_next, value_normalizer)``, ``sample(indexes)``,
     ``clear``, ``full``, ``ptr / size / start_ids``, same constructor arguments and sample keys.
@@ -186,38 +246,14 @@ class MARL_OnPolicyBuffer:
     ValueNorm state as it is at that moment (the reference's per-step Python loop, :208-236).  ``sample`` gathers the
     minibatch agent-major (row k * B + b is agent k of sample b) with K3 and normalises the advantages per agent over
     the minibatch, as the reference does per agent key (:255-258)."""
-    FIELDS = ('actions', 'rewards', 'values', 'log_pi_old', 'terminals', 'agent_mask', 'returns', 'advantages')
-    STORED = 6   # the fields store() writes; returns / advantages come from finish_path
+    BOX_REFUSAL = "MARL_OnPolicyBuffer: Box action spaces (Gaussian MAPPO) are not supported"
 
     def __init__(self, agent_keys, state_space=None, obs_space=None, act_space=None, n_envs=1, buffer_size=1,
                  use_gae=False, use_advnorm=False, gamma=None, gae_lam=None, device="cuda:0", **kwargs):
         assert buffer_size % n_envs == 0, "buffer_size must be divisible by the number of envs (parallels)"
-        self.agent_keys = list(agent_keys)
-        self.n_agents = len(self.agent_keys)
-        self.n_envs, self.buffer_size = n_envs, buffer_size
+        super().__init__(agent_keys, state_space, obs_space, act_space, n_envs, buffer_size, use_gae, use_advnorm,
+                         gamma, gae_lam, device, **kwargs)
         self.n_size = buffer_size // n_envs
-        self.state_space = state_space
-        self.store_global_state = state_space is not None
-        self.use_actions_mask = kwargs.get("use_actions_mask", False)
-        self.avail_actions_shape = kwargs.get("avail_actions_shape", None)
-        self.use_gae, self.use_advantage_norm = use_gae, use_advnorm
-        self.gamma, self.gae_lambda = gamma, gae_lam
-        k0 = self.agent_keys[0]
-        obs_shape = {k: tuple(space2shape(obs_space[k])) for k in self.agent_keys}
-        act_shape = {k: tuple(space2shape(act_space[k])) for k in self.agent_keys}
-        if any(obs_shape[k] != obs_shape[k0] or act_shape[k] != act_shape[k0] for k in self.agent_keys):
-            raise NotImplementedError("heterogeneous agents are outside the hot-path scope (one parameter-sharing group)")
-        if act_shape[k0] != ():
-            raise NotImplementedError("MARL_OnPolicyBuffer: Box action spaces (Gaussian MAPPO) are not supported")
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("xuance_b200 buffers are device-resident: device must be CUDA (no CPU fallback)")
-        _lib.load()
-        _lib.use_device(self.device)
-        self._obs_dim = int(np.prod(obs_shape[k0]))
-        self._state_dim = int(np.prod(space2shape(state_space))) if self.store_global_state else 0
-        self._n_act = int(self.avail_actions_shape[k0][0]) if self.use_actions_mask else 0
-        self._rows = self.n_envs * self.n_agents
         self._scratch = _lib.scratch(self.device)
         self.clear()
 
@@ -255,10 +291,6 @@ class MARL_OnPolicyBuffer:
         """[n_envs * n_agents, n_size] device view of a scalar field (row = env * n_agents + agent)."""
         return self._scal[self.FIELDS.index(name)]
 
-    def _per_agent(self, d, dtype=np.float32):
-        """{agent: [n_envs, ...]} -> [n_envs * n_agents, ...] (env-major, agent-minor)."""
-        return np.stack([np.asarray(d[k], dtype=dtype) for k in self.agent_keys], axis=1).reshape(self._rows, -1)
-
     # ---- reference :175-184
     def store(self, **step_data):
         t, R = self.ptr, self._rows
@@ -288,7 +320,7 @@ class MARL_OnPolicyBuffer:
         beg = int(self.start_ids[i_env])
         end = self.n_size if self.full else self.ptr
         if end > beg:
-            n, T = self.n_agents, self.n_size
+            n = self.n_agents
             rows = slice(i_env * n, (i_env + 1) * n)
             self._seg_end[rows, end - 1] = 1
             self._boot[rows, end - 1] = [np.float32(value_next[k]) for k in self.agent_keys]
@@ -296,25 +328,9 @@ class MARL_OnPolicyBuffer:
             self._boot_d[rows].copy_(torch.from_numpy(self._boot[rows]))
             self._start_d[rows].fill_(beg)
             self._cov_d[rows].fill_(end)
-            vn = None
-            if value_normalizer is not None:
-                groups = {agent_grouping.agent_to_group[k] for k in self.agent_keys} if agent_grouping is not None \
-                    else set(value_normalizer)
-                if len(groups) != 1:
-                    raise NotImplementedError("one parameter-sharing group")
-                vn = value_normalizer[groups.pop()]
-            vp = vn.state_pointers() if vn is not None else (None, None, None)
-            f = lambda name: _lib.ptr(self.field(name)[rows])
-            _lib.call("xb_gae_scan_vn", f('rewards'), f('values'), f('terminals'), _lib.ptr(self._seg_end_d[rows]),
-                      _lib.ptr(self._boot_d[rows]), _lib.ptr(self._start_d[rows]), _lib.ptr(self._cov_d[rows]),
-                      f('advantages'), f('returns'), n, T, float(self.gamma),
-                      float(self.gae_lambda if self.gae_lambda is not None else 0.0), 1 if self.use_gae else 0, *vp)
+            self._gae(rows, self._seg_end_d[rows], self._boot_d[rows], self._start_d[rows], self._cov_d[rows],
+                      agent_grouping, value_normalizer)
         self.start_ids[i_env] = self.ptr
-
-    def _gather_rows(self, src, idx_t, row_bytes, shape, dtype):
-        out = torch.empty(shape, dtype=dtype, device=self.device)
-        _lib.call("xb_gather_rows", _lib.ptr(src), _lib.ptr(idx_t), idx_t.numel(), row_bytes, _lib.ptr(out))
-        return out
 
     # ---- reference :242-270
     def sample(self, indexes=None):
@@ -335,27 +351,13 @@ class MARL_OnPolicyBuffer:
                 _lib.call("xb_gather_scalars", _lib.ptr(adv_plane), self._rows * T, _lib.ptr(slot_t[k * B:]), B, 1,
                           _lib.ptr(scal[ia, k * B:]), 0, _lib.ptr(stats), _lib.ptr(self._scratch))
         st = {name: scal[i] for i, name in enumerate(self.FIELDS)}
-        st['obs'] = self._gather_rows(self._obs, slot_t, self._obs_dim * 4, (n * B, self._obs_dim), torch.float32)
+        st['obs'] = self._gather_rows(self._obs.flatten(0, 1), slot_t)         # one gathered row per (row, step) slot
         if self.use_actions_mask:
-            a4 = _pad4(self._n_act)
-            st['avail_actions'] = self._gather_rows(self._avail, slot_t, a4, (n * B, a4), torch.uint8)
+            st['avail_actions'] = self._gather_rows(self._avail.flatten(0, 1), slot_t)
         if self.store_global_state:
             s_idx = torch.from_numpy(np.tile(env * T + step, n)).to(self.device)
-            st['state'] = self._gather_rows(self._state, s_idx, self._state_dim * 4, (n * B, self._state_dim),
-                                            torch.float32)
-        out = {}
-        for key, v in st.items():
-            if key == 'state':
-                out[key] = v[:B]
-            elif key == 'avail_actions':
-                out[key] = {a: v[i * B:(i + 1) * B, :self._n_act].bool() for i, a in enumerate(self.agent_keys)}
-            elif key in ('terminals', 'agent_mask'):
-                out[key] = {a: v[i * B:(i + 1) * B].bool() for i, a in enumerate(self.agent_keys)}
-            else:
-                out[key] = {a: v[i * B:(i + 1) * B] for i, a in enumerate(self.agent_keys)}
-        out['batch_size'] = B
-        out['_stacked'] = st
-        return out
+            st['state'] = self._gather_rows(self._state.flatten(0, 1), s_idx)
+        return dict(self._split(st, B), batch_size=B, _stacked=st)
 
     # ---- checkpoint (the reference does not save its rollout)
     def state_dict(self):
@@ -381,7 +383,7 @@ class MARL_OnPolicyBuffer:
         self.ptr, self.size, self.start_ids = int(sd["ptr"]), int(sd["size"]), np.array(sd["start_ids"])
 
 
-class MARL_OnPolicyBuffer_RNN:
+class MARL_OnPolicyBuffer_RNN(_MARLOnPolicyBuffer):
     """Episode-major on-policy rollout for recurrent MAPPO - mirror of MARL_OnPolicyBuffer_RNN
     (xuance/common/memory_tools_marl.py:273-515): same constructor arguments, keys, ``ptr / size / full``, ``clear /
     clear_episodes / store / store_episodes / finish_path / sample``.  ``buffer_size`` counts episodes.
@@ -393,38 +395,15 @@ class MARL_OnPolicyBuffer_RNN:
     never zeroed between episodes, so the padded tail of an env's second episode still holds its first episode's data.
     ``sample`` gathers whole episodes with K3 into sequence-major ``[B*n, T, .]`` (sequence k*B + b is agent k of
     episode b) and does not normalise advantages (the reference's recurrent ``sample`` does not either)."""
-    FIELDS = MARL_OnPolicyBuffer.FIELDS
-    STORED = MARL_OnPolicyBuffer.STORED
+    BOX_REFUSAL = "MARL_OnPolicyBuffer_RNN: Box action spaces (Gaussian MAPPO) are not supported"
 
     def __init__(self, agent_keys, state_space=None, obs_space=None, act_space=None, n_envs=1, buffer_size=1,
                  max_episode_steps=1, use_gae=False, use_advnorm=False, gamma=None, gae_lam=None, device="cuda:0",
                  **kwargs):
-        self.agent_keys = list(agent_keys)
-        self.n_agents = len(self.agent_keys)
-        self.n_envs, self.buffer_size, self.max_eps_len = n_envs, buffer_size, max_episode_steps
-        self.state_space = state_space
-        self.store_global_state = state_space is not None
-        self.use_actions_mask = kwargs.get("use_actions_mask", False)
-        self.avail_actions_shape = kwargs.get("avail_actions_shape", None)
-        self.use_gae, self.use_advantage_norm = use_gae, use_advnorm
-        self.gamma, self.gae_lambda = gamma, gae_lam
-        k0 = self.agent_keys[0]
-        obs_shape = {k: tuple(space2shape(obs_space[k])) for k in self.agent_keys}
-        act_shape = {k: tuple(space2shape(act_space[k])) for k in self.agent_keys}
-        if any(obs_shape[k] != obs_shape[k0] or act_shape[k] != act_shape[k0] for k in self.agent_keys):
-            raise NotImplementedError("heterogeneous agents are outside the hot-path scope (one parameter-sharing group)")
-        if act_shape[k0] != ():
-            raise NotImplementedError("MARL_OnPolicyBuffer_RNN: Box action spaces (Gaussian MAPPO) are not supported")
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("xuance_b200 buffers are device-resident: device must be CUDA (no CPU fallback)")
-        _lib.load()
-        _lib.use_device(self.device)
-        self._obs_dim = int(np.prod(obs_shape[k0]))
-        self._state_dim = int(np.prod(space2shape(state_space))) if self.store_global_state else 0
-        self._n_act = int(self.avail_actions_shape[k0][0]) if self.use_actions_mask else 0
+        super().__init__(agent_keys, state_space, obs_space, act_space, n_envs, buffer_size, use_gae, use_advnorm,
+                         gamma, gae_lam, device, **kwargs)
+        self.max_eps_len = max_episode_steps
         self._a4 = _pad4(self._n_act)
-        self._rows = self.n_envs * self.n_agents
         self._seg_end = np.zeros((self._rows, self.max_eps_len), np.uint8)
         self._boot = np.zeros((self._rows, self.max_eps_len), np.float32)
         self.clear()
@@ -470,9 +449,6 @@ class MARL_OnPolicyBuffer_RNN:
         """[n_envs * n_agents, T] device view of a staging scalar field (row = env * n_agents + agent)."""
         return self._ep_scal[self.FIELDS.index(name)]
 
-    def _per_agent(self, d, dtype=np.float32):
-        return np.stack([np.asarray(d[k], dtype=dtype) for k in self.agent_keys], axis=1).reshape(self._rows, -1)
-
     # ---- reference :397-414
     def store(self, **step_data):
         T, R = self.max_eps_len, self._rows
@@ -515,8 +491,8 @@ class MARL_OnPolicyBuffer_RNN:
     # ---- reference :437-490
     def finish_path(self, i_env=None, i_step=None, agent_grouping=None, value_next=None, value_normalizer=None,
                     **kwargs):
-        n, T = self.n_agents, self.max_eps_len
-        env_step = min(int(i_step), T)
+        n = self.n_agents
+        env_step = min(int(i_step), self.max_eps_len)
         if env_step > 0:
             rows = slice(i_env * n, (i_env + 1) * n)
             self._seg_end[rows] = 0
@@ -526,56 +502,26 @@ class MARL_OnPolicyBuffer_RNN:
             seg_d = torch.from_numpy(self._seg_end[rows]).to(self.device)
             boot_d = torch.from_numpy(self._boot[rows]).to(self.device)
             cov_d = torch.full((n,), env_step, dtype=torch.int32, device=self.device)
-            vn = None
-            if value_normalizer is not None:
-                groups = {agent_grouping.agent_to_group[k] for k in self.agent_keys} if agent_grouping is not None \
-                    else set(value_normalizer)
-                if len(groups) != 1:
-                    raise NotImplementedError("one parameter-sharing group")
-                vn = value_normalizer[groups.pop()]
-            vp = vn.state_pointers() if vn is not None else (None, None, None)
-            f = lambda name: _lib.ptr(self.field(name)[rows])
-            _lib.call("xb_gae_scan_vn", f('rewards'), f('values'), f('terminals'), _lib.ptr(seg_d), _lib.ptr(boot_d),
-                      None, _lib.ptr(cov_d), f('advantages'), f('returns'), n, T, float(self.gamma),
-                      float(self.gae_lambda if self.gae_lambda is not None else 0.0), 1 if self.use_gae else 0, *vp)
+            self._gae(rows, seg_d, boot_d, None, cov_d, agent_grouping, value_normalizer)
         self.store_episodes(i_env)
-
-    def _gather_rows(self, src, idx_t, row_bytes, shape, dtype):
-        out = torch.empty(shape, dtype=dtype, device=self.device)
-        _lib.call("xb_gather_rows", _lib.ptr(src), _lib.ptr(idx_t), idx_t.numel(), row_bytes, _lib.ptr(out))
-        return out
 
     # ---- reference :492-515
     def sample(self, indexes=None):
         assert self.full, "Not enough transitions for on-policy buffer to random sample"
         idx = np.asarray(indexes, dtype=np.int64).reshape(-1)
-        B, n, T, F = idx.size, self.n_agents, self.max_eps_len, len(self.FIELDS)
+        B, n, T = idx.size, self.n_agents, self.max_eps_len
         seq = (idx[None, :] * n + np.arange(n)[:, None]).reshape(-1)                # agent-major: k * B + b
         seq_t = torch.from_numpy(seq).to(self.device)
         ep_t = torch.from_numpy(np.tile(idx, n)).to(self.device)
-        scal = self._gather_rows(self._scal, seq_t, F * T * 4, (n * B, F, T), torch.float32)
+        scal = self._gather_rows(self._scal, seq_t)
         st = {name: scal[:, i].contiguous() for i, name in enumerate(self.FIELDS)}    # [n*B, T]
-        st['obs'] = self._gather_rows(self._obs, seq_t, T * self._obs_dim * 4, (n * B, T, self._obs_dim), torch.float32)
-        st['filled'] = self._gather_rows(self._filled, ep_t, T * 4, (n * B, T), torch.float32)
+        st['obs'] = self._gather_rows(self._obs, seq_t)
+        st['filled'] = self._gather_rows(self._filled, ep_t)
         if self.use_actions_mask:
-            st['avail_actions'] = self._gather_rows(self._avail, seq_t, T * self._a4, (n * B, T, self._a4), torch.uint8)
+            st['avail_actions'] = self._gather_rows(self._avail, seq_t)
         if self.store_global_state:
-            st['state'] = self._gather_rows(self._state, ep_t, T * self._state_dim * 4, (n * B, T, self._state_dim),
-                                            torch.float32)
-        out = {}
-        for key, v in st.items():
-            if key in ('filled', 'state'):
-                out[key] = v[:B].bool() if key == 'filled' else v[:B]
-            elif key == 'avail_actions':
-                out[key] = {a: v[i * B:(i + 1) * B, :, :self._n_act].bool() for i, a in enumerate(self.agent_keys)}
-            elif key in ('terminals', 'agent_mask'):
-                out[key] = {a: v[i * B:(i + 1) * B].bool() for i, a in enumerate(self.agent_keys)}
-            else:
-                out[key] = {a: v[i * B:(i + 1) * B] for i, a in enumerate(self.agent_keys)}
-        out['batch_size'] = B
-        out['sequence_length'] = T
-        out['_stacked'] = st
-        return out
+            st['state'] = self._gather_rows(self._state, ep_t)
+        return dict(self._split(st, B), batch_size=B, sequence_length=T, _stacked=st)
 
     # ---- checkpoint (the reference does not save its rollout)
     def state_dict(self):

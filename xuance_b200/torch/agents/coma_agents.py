@@ -15,9 +15,10 @@ import torch.nn as nn
 
 from ... import _lib
 from ..rl_models import (CategoricalActor, CounterfactualCentralizedCritic, CounterfactualMultiAgentActorCritic)
-from .mappo_agents import OnPolicyMARLAgents, MARLActionOutput, MAPPO_Agents
+from ..rl_models.gru import check_scope
+from .mappo_agents import OnPolicyMARLAgents
 
-COMA_MAX_ACTIONS, COMA_MAX_AGENTS, GRU_MAX_HIDDEN = 64, 32, 64    # K4C, K13
+COMA_MAX_ACTIONS, COMA_MAX_AGENTS = 64, 32    # K4C
 
 
 class COMA_Agents(OnPolicyMARLAgents):
@@ -37,30 +38,19 @@ class COMA_Agents(OnPolicyMARLAgents):
         self.learner = self._build_learner(self.config, self.agent_grouping, self.model, self.callback)
 
     def _check_scope(self):
-        c = self.config
         if not all(hasattr(self.action_space[k], "n") for k in self.agent_keys):
             raise ValueError("COMA takes Discrete action spaces (Box actions have no counterfactual baseline here)")
         if len(self.group_keys) != 1:
             raise NotImplementedError("COMA: one parameter-sharing group")
         if not self.use_rnn:
             raise NotImplementedError("COMA: use_rnn=False is not supported (recurrent episodes only)")
-        if getattr(c, "rnn", "GRU") != "GRU":
-            raise NotImplementedError("COMA: LSTM representations are not supported (GRU only)")
-        if getattr(c, "N_recurrent_layers", 1) != 1:
-            raise NotImplementedError("COMA: N_recurrent_layers > 1 is not supported (one GRU layer)")
-        if getattr(c, "dropout", 0) > 0:
-            raise NotImplementedError("COMA: dropout > 0 is not supported")
-        if c.recurrent_hidden_size > GRU_MAX_HIDDEN:
-            raise NotImplementedError("COMA: recurrent_hidden_size > %d is not supported (K13), got %d"
-                                      % (GRU_MAX_HIDDEN, c.recurrent_hidden_size))
+        check_scope("COMA", self.config)
         A = max(self.action_space[k].n for k in self.agent_keys)
         if A > COMA_MAX_ACTIONS:
             raise NotImplementedError("COMA: more than %d actions is not supported (K4C), got %d" % (COMA_MAX_ACTIONS, A))
         if self.n_agents > COMA_MAX_AGENTS:
             raise NotImplementedError("COMA: more than %d agents is not supported (K4C), got %d"
                                       % (COMA_MAX_AGENTS, self.n_agents))
-
-    _build_agent_feature_encoder = MAPPO_Agents._build_agent_feature_encoder
 
     def _build_model(self):
         """coma_agents.py:49-115."""
@@ -93,17 +83,14 @@ class COMA_Agents(OnPolicyMARLAgents):
     def _state_rows(self, state, n_envs):
         return torch.as_tensor(np.asarray(state, np.float32), device=self.device).reshape(n_envs, -1)
 
-    @torch.no_grad()
-    def get_actions(self, obs_list, state=None, avail_actions_list=None, rnn_states_actor=None,
-                    rnn_states_critic=None, test_mode=False, deterministic=False, **kwargs):
-        """coma_agents.py:175-273."""
-        n_envs, K = len(obs_list), self.agent_keys
-        obs, avail = self._build_inputs(obs_list, avail_actions_list)
-        obs_d = torch.from_numpy(obs).to(self.device)
-        if self.use_rnn:
-            logits, rnn_states_actor = self.model.logits(obs_d, rnn_states=rnn_states_actor, return_states=True)
-        else:
-            logits = self.model.logits(obs_d)
+    def get_actions(self, *args, **kwargs):
+        """coma_agents.py:175-273; remembers the actions for ``values_next``."""
+        policy_out = super().get_actions(*args, **kwargs)
+        self._last_actions = policy_out.env_actions
+        return policy_out
+
+    def _act(self, obs_d, logits, avail, state, n_envs, rnn_states_critic, test_mode, deterministic):
+        """K4C's epsilon-mixed sampling, then the target critics' Q of the taken actions."""
         logits = logits.contiguous()
         R, A = logits.shape
         av = None if avail is None else torch.from_numpy(avail).to(self.device)
@@ -118,18 +105,10 @@ class COMA_Agents(OnPolicyMARLAgents):
                   _lib.ptr(out[1]))
         if not test_mode:           # the target critics' Q of the taken actions (coma_agents.py:237-261)
             q, rnn_states_critic = self.model.q_values(self._state_rows(state, n_envs), obs_d,
-                                                       out[0].reshape(n_envs, len(K)), rnn_states_critic,
+                                                       out[0].reshape(n_envs, self.n_agents), rnn_states_critic,
                                                        return_states=True, target=True)
             out[2] = q.gather(1, acts_i.long().unsqueeze(1)).squeeze(1)
-        host = out.cpu().numpy().reshape(3, n_envs, len(K))
-        actions_list = [{k: int(host[0, e, i]) for i, k in enumerate(K)} for e in range(n_envs)]
-        self._last_actions = actions_list
-        log_pi, values = {}, {}
-        if not test_mode:
-            log_pi = {k: host[1, :, i].copy() for i, k in enumerate(K)}
-            values = {k: host[2, :, i].copy() for i, k in enumerate(K)}
-        return MARLActionOutput(env_actions=actions_list, log_probs=log_pi, values=values,
-                                rnn_states_actor=rnn_states_actor, rnn_states_critic=rnn_states_critic)
+        return out, rnn_states_critic
 
     @torch.no_grad()
     def values_next(self, i_env, obs_dict, state=None, actions_n=None, rnn_states_critic=None):
@@ -152,18 +131,9 @@ class COMA_Agents(OnPolicyMARLAgents):
         the shuffled minibatch updates with that epsilon."""
         if self.egreedy >= self.end_greedy:
             self.egreedy = self.start_greedy - self.delta_egreedy * self.current_step
-        info_train = {}
-        if self.memory.full:
-            indexes = np.arange(self.buffer_size)
-            for e in range(n_epochs):
-                np.random.shuffle(indexes)
-                for start in range(0, self.buffer_size, self.batch_size):
-                    last = e == n_epochs - 1 and start + self.batch_size >= self.buffer_size
-                    info_train = self.learner.update(self.memory.sample(indexes[start:start + self.batch_size]),
-                                                     self.egreedy, sync=last)
-            self.callback.on_train_epochs_end(self.current_step, policy=self.model, memory=self.memory,
-                                              current_episode=self.current_episode, n_epochs=n_epochs,
-                                              buffer_size=self.buffer_size, update_info=info_train)
-            self.memory.clear()
+        info_train = super().train_epochs(n_epochs)
         info_train["epsilon-greedy"] = self.egreedy
         return info_train
+
+    def _update(self, sample, sync):
+        return self.learner.update(sample, self.egreedy, sync=sync)

@@ -1,10 +1,8 @@
 """DCG agents - mirror of xuance/torch/agents/multi_agent_rl/dcg_agents.py:16-155."""
 import torch.nn as nn
 
-from ..rl_models import (ActivationFunctions, AgentFeatureEncoder, Basic_RNN_K13, ValueHead, DCG_Utility, DCG_Payoff,
-                         Coordination_Graph, DeepCoordinationGraph)
+from ..rl_models import ValueHead, DCG_Utility, DCG_Payoff, Coordination_Graph, DeepCoordinationGraph
 from ..rl_models.dcg import check_graph_limits
-from ...common import space2shape
 from .marl import OffPolicyMARLAgents
 
 
@@ -27,9 +25,6 @@ class DCG_Agents(OffPolicyMARLAgents):
         self.use_global_state = config.agent == "DCG_S"
         if self.use_global_state and self.state_space is None:
             raise ValueError("DCG_S evaluates V(s) on the global state: provide envs or state_space")
-        self.start_greedy, self.end_greedy = config.start_greedy, config.end_greedy
-        self.e_greedy = self.start_greedy
-        self.delta_egreedy = (self.start_greedy - self.end_greedy) / config.decay_step_greedy
         self.model = self._build_model()
         self.memory = self._build_memory()
         self.learner = self._build_learner(self.config, self.agent_grouping, self.model, self.callback)
@@ -42,13 +37,7 @@ class DCG_Agents(OffPolicyMARLAgents):
         graph.set_coordination_graph()
         representations = nn.ModuleDict()
         for group_key, group_agents in self.groups.items():
-            rep = Basic_RNN_K13(input_shape=space2shape(self.observation_space[group_agents[0]]),
-                                hidden_sizes=getattr(cfg, "representation_hidden_size", None), normalize=None,
-                                initialize=nn.init.orthogonal_, activation=ActivationFunctions[cfg.activation],
-                                fc_hidden_sizes=cfg.fc_hidden_sizes, N_recurrent_layers=cfg.N_recurrent_layers,
-                                recurrent_hidden_size=cfg.recurrent_hidden_size, rnn=cfg.rnn, dropout=cfg.dropout,
-                                device=self.device)
-            representations[group_key] = AgentFeatureEncoder(rep)
+            representations[group_key] = self._build_k13_encoder(self.observation_space[group_agents[0]], None)
         H = cfg.recurrent_hidden_size
         utility = DCG_Utility(H, cfg.hidden_utility_dim, n_act, self.device)
         payoffs = DCG_Payoff(2 * H, cfg.hidden_payoff_dim, n_act, cfg.low_rank_payoff, cfg.payoff_rank, self.device)

@@ -22,16 +22,8 @@ import torch.nn as nn
 
 from ... import _lib
 from ...common import MARL_OnPolicyBuffer, MARL_OnPolicyBuffer_RNN
-from ...common.spaces import space2shape
-from ..rl_models import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic, Basic_RNN_K13
-from ..rl_models.qmix import AgentFeatureEncoder
-from .marl import MARLAgents
-
-
-class MARLActionOutput:
-    def __init__(self, env_actions=None, log_probs=None, values=None, rnn_states_actor=None, rnn_states_critic=None):
-        self.env_actions, self.log_probs, self.values = env_actions, log_probs, values
-        self.rnn_states_actor, self.rnn_states_critic = rnn_states_actor, rnn_states_critic
+from ..rl_models import CategoricalActor, CentralizedStateValueCritic, MultiAgentActorCritic
+from .marl import MARLAgents, MARLActionOutput
 
 
 class OnPolicyMARLAgents(MARLAgents):
@@ -70,18 +62,14 @@ class OnPolicyMARLAgents(MARLAgents):
     def store_experience(self, obs_list, avail_actions, actions_list, log_pi_a, rewards_list, values_dict,
                          terminals_list, info, **kwargs):
         """on_policy_marl.py:103-158."""
-        K = self.agent_keys
-        data = {'obs': {k: np.array([d[k] for d in obs_list]) for k in K},
-                'actions': {k: np.array([d[k] for d in actions_list]) for k in K},
-                'log_pi_old': log_pi_a,
-                'rewards': {k: np.array([d[k] for d in rewards_list]) for k in K},
-                'values': values_dict,
-                'terminals': {k: np.array([d[k] for d in terminals_list]) for k in K},
-                'agent_mask': {k: np.array([d['agent_mask'][k] for d in info]) for k in K}}
+        data = {'obs': self._agent_arrays(obs_list), 'actions': self._agent_arrays(actions_list),
+                'log_pi_old': log_pi_a, 'rewards': self._agent_arrays(rewards_list), 'values': values_dict,
+                'terminals': self._agent_arrays(terminals_list),
+                'agent_mask': self._agent_arrays([d['agent_mask'] for d in info])}
         if self.use_global_state:
             data['state'] = np.array(kwargs['state'])
         if self.use_actions_mask:
-            data['avail_actions'] = {k: np.array([d[k] for d in avail_actions]) for k in K}
+            data['avail_actions'] = self._agent_arrays(avail_actions)
         if self.use_rnn:
             data['episode_steps'] = np.array([d['episode_step'] - 1 for d in info])
         self.memory.store(**data)
@@ -96,6 +84,13 @@ class OnPolicyMARLAgents(MARLAgents):
         """The values of the acting rows [n_envs * n_agents] (and the new critic states with return_states)."""
         return self.model.values(obs_d, self._states(state, n_envs), rnn_states=rnn_states, return_states=return_states)
 
+    def _build_agent_feature_encoder(self, representation_choice, group_agents, input_space):
+        if not self.use_rnn:
+            return super()._build_agent_feature_encoder(representation_choice, group_agents, input_space)
+        if representation_choice != "Basic_RNN":
+            raise NotImplementedError("use_rnn=True takes representation: Basic_RNN, got %s" % representation_choice)
+        return self._build_k13_encoder(input_space, self.normalize_fn)
+
     @torch.no_grad()
     def get_actions(self, obs_list, state=None, avail_actions_list=None, rnn_states_actor=None,
                     rnn_states_critic=None, test_mode=False, deterministic=False, **kwargs):
@@ -107,6 +102,20 @@ class OnPolicyMARLAgents(MARLAgents):
             logits, rnn_states_actor = self.model.logits(obs_d, rnn_states=rnn_states_actor, return_states=True)
         else:
             logits = self.model.logits(obs_d)
+        out, rnn_states_critic = self._act(obs_d, logits, avail, state, n_envs, rnn_states_critic, test_mode,
+                                           deterministic)
+        host = out.cpu().numpy().reshape(3, n_envs, len(K))
+        actions_list = [{k: int(host[0, e, i]) for i, k in enumerate(K)} for e in range(n_envs)]
+        log_pi, values = {}, {}
+        if not test_mode:
+            log_pi = {k: host[1, :, i].copy() for i, k in enumerate(K)}
+            values = {k: host[2, :, i].copy() for i, k in enumerate(K)}
+        return MARLActionOutput(env_actions=actions_list, log_probs=log_pi, values=values,
+                                rnn_states_actor=rnn_states_actor, rnn_states_critic=rnn_states_critic)
+
+    def _act(self, obs_d, logits, avail, state, n_envs, rnn_states_critic, test_mode, deterministic):
+        """K10 samples the rows' actions from the actor's logits -> ([3, R] actions, log-probabilities and, outside
+        test_mode, the critic's values; the new critic states)."""
         if avail is not None:
             logits = logits.masked_fill(torch.from_numpy(avail).to(self.device) == 0, -1e10)
         logits = logits.contiguous()
@@ -121,14 +130,7 @@ class OnPolicyMARLAgents(MARLAgents):
                 out[2], rnn_states_critic = self._critic_values(obs_d, state, n_envs, rnn_states_critic, True)
             else:
                 out[2] = self._critic_values(obs_d, state, n_envs)
-        host = out.cpu().numpy().reshape(3, n_envs, len(K))
-        actions_list = [{k: int(host[0, e, i]) for i, k in enumerate(K)} for e in range(n_envs)]
-        log_pi, values = {}, {}
-        if not test_mode:
-            log_pi = {k: host[1, :, i].copy() for i, k in enumerate(K)}
-            values = {k: host[2, :, i].copy() for i, k in enumerate(K)}
-        return MARLActionOutput(env_actions=actions_list, log_probs=log_pi, values=values,
-                                rnn_states_actor=rnn_states_actor, rnn_states_critic=rnn_states_critic)
+        return out, rnn_states_critic
 
     @torch.no_grad()
     def values_next(self, i_env, obs_dict, state=None, rnn_states_critic=None):
@@ -206,14 +208,7 @@ class OnPolicyMARLAgents(MARLAgents):
             for i in range(self.n_envs):
                 if all(terminated_list[i].values()) or truncated[i]:
                     self._finish(i, terminated_list[i], obs_list[i], state[i] if self.use_global_state else None)
-                    obs_list[i] = info[i]["reset_obs"]
-                    envs.buf_obs[i] = info[i]["reset_obs"]
-                    if self.use_actions_mask:
-                        avail_actions[i] = info[i]["reset_avail_actions"]
-                        envs.buf_avail_actions[i] = info[i]["reset_avail_actions"]
-                    if self.use_global_state:
-                        state[i] = info[i]["reset_state"]
-                        envs.buf_state[i] = info[i]["reset_state"]
+                    self._reset_env(envs, i, info, obs_list, state, avail_actions)
                     self.current_episode[i] += 1
                     episode_info = {
                         "Train-Results/Episode-Steps": {"env-%d" % i: info[i]["episode_step"]},
@@ -282,14 +277,7 @@ class OnPolicyMARLAgents(MARLAgents):
                                                             current_step=self.current_step,
                                                             current_episode=self.current_episode,
                                                             n_episodes=n_episodes)
-                    obs_list[i] = info[i]["reset_obs"]
-                    envs.buf_obs[i] = info[i]["reset_obs"]
-                    if self.use_actions_mask:
-                        avail_actions[i] = info[i]["reset_avail_actions"]
-                        envs.buf_avail_actions[i] = info[i]["reset_avail_actions"]
-                    if self.use_global_state:
-                        state[i] = info[i]["reset_state"]
-                        envs.buf_state[i] = info[i]["reset_state"]
+                    self._reset_env(envs, i, info, obs_list, state, avail_actions)
         if test_mode:
             self.log_infos({"Test-Results/Episode-Rewards/Mean-Score": float(np.mean(scores)),
                             "Test-Results/Episode-Rewards/Std-Score": float(np.std(scores))}, self.current_step)
@@ -307,13 +295,15 @@ class OnPolicyMARLAgents(MARLAgents):
                 np.random.shuffle(indexes)
                 for start in range(0, self.buffer_size, self.batch_size):
                     last = e == n_epochs - 1 and start + self.batch_size >= self.buffer_size
-                    info_train = self.learner.update(self.memory.sample(indexes[start:start + self.batch_size]),
-                                                     sync=last)
+                    info_train = self._update(self.memory.sample(indexes[start:start + self.batch_size]), last)
             self.callback.on_train_epochs_end(self.current_step, policy=self.model, memory=self.memory,
                                               current_episode=self.current_episode, n_epochs=n_epochs,
                                               buffer_size=self.buffer_size, update_info=info_train)
             self.memory.clear()
         return info_train
+
+    def _update(self, sample, sync):
+        return self.learner.update(sample, sync=sync)
 
     def test(self, test_episodes, deterministic_policy=True, test_envs=None, close_envs=True):
         return self.run_episodes(n_episodes=test_episodes, run_envs=test_envs, test_mode=True,
@@ -332,19 +322,6 @@ class MAPPO_Agents(OnPolicyMARLAgents):
         self.model = self._build_model()
         self.memory = self._build_memory()
         self.learner = self._build_learner(self.config, self.agent_grouping, self.model, self.callback)
-
-    def _build_agent_feature_encoder(self, representation_choice, group_agents, input_space):
-        if not self.use_rnn:
-            return super()._build_agent_feature_encoder(representation_choice, group_agents, input_space)
-        if representation_choice != "Basic_RNN":
-            raise NotImplementedError("use_rnn=True (recurrent MAPPO) takes representation: Basic_RNN, got %s"
-                                      % representation_choice)
-        c = self.config
-        return AgentFeatureEncoder(Basic_RNN_K13(
-            input_shape=space2shape(input_space), normalize=self.normalize_fn, initialize=nn.init.orthogonal_,
-            activation=self.activation, device=self.device, fc_hidden_sizes=c.fc_hidden_sizes,
-            recurrent_hidden_size=c.recurrent_hidden_size, N_recurrent_layers=getattr(c, "N_recurrent_layers", 1),
-            rnn=getattr(c, "rnn", "GRU"), dropout=getattr(c, "dropout", 0)))
 
     def _build_model(self):
         actors, critics, critic_encoders = nn.ModuleDict(), nn.ModuleDict(), nn.ModuleDict()

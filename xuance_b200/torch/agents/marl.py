@@ -21,15 +21,20 @@ import torch
 import torch.nn as nn
 
 from ...common import AgentGrouping, BaseCallback, MARL_OffPolicyBuffer_RNN, space2shape
-from ..rl_models import (REGISTRY_Representation, ActivationFunctions, AgentFeatureEncoder, DiscreteActionValueCritic,
-                         QMIX_Mixer, VDN_mixer, MixingQNetwork)
+from ..rl_models import (REGISTRY_Representation, ActivationFunctions, AgentFeatureEncoder, Basic_RNN_K13,
+                         DiscreteActionValueCritic, QMIX_Mixer, VDN_mixer, MixingQNetwork)
 from .agent import set_seed, set_device, InitializeFunctions, NormalizeFunctions
 from ..utils import init_distributed_mode
 
 
 class MARLActionOutput:
-    def __init__(self, env_actions=None, rnn_states=None, values=None):
-        self.env_actions, self.rnn_states, self.values = env_actions, rnn_states, values
+    """What ``get_actions`` returns: the off-policy agents fill ``rnn_states``, the on-policy ones ``log_probs``,
+    ``values`` and the actor / critic states."""
+
+    def __init__(self, env_actions=None, rnn_states=None, values=None, log_probs=None, rnn_states_actor=None,
+                 rnn_states_critic=None):
+        self.env_actions, self.rnn_states, self.values, self.log_probs = env_actions, rnn_states, values, log_probs
+        self.rnn_states_actor, self.rnn_states_critic = rnn_states_actor, rnn_states_critic
 
 
 class MARLAgents:
@@ -148,6 +153,28 @@ class MARLAgents:
             raise NotImplementedError("agent-identity embeddings are outside the hot-path scope (mode 'none')")
         return AgentFeatureEncoder(self._build_representation(representation_choice, input_space, self.config))
 
+    def _build_k13_encoder(self, input_space, normalize):
+        """The LayerNorm Basic_RNN whose GRU runs on K13; ``normalize`` None builds it without the LayerNorms."""
+        return AgentFeatureEncoder(Basic_RNN_K13(
+            input_shape=space2shape(input_space), normalize=normalize, initialize=nn.init.orthogonal_,
+            activation=self.activation, device=self.device, fc_hidden_sizes=self.config.fc_hidden_sizes,
+            recurrent_hidden_size=self.config.recurrent_hidden_size,
+            N_recurrent_layers=getattr(self.config, "N_recurrent_layers", 1), rnn=getattr(self.config, "rnn", "GRU"),
+            dropout=getattr(self.config, "dropout", 0)))
+
+    def _agent_arrays(self, per_env):
+        """Per-env dicts [{agent: x}] -> {agent: array over the envs}."""
+        return {k: np.array([d[k] for d in per_env]) for k in self.agent_keys}
+
+    def _reset_env(self, envs, i, info, obs_list, state, avail_actions):
+        """A finished env i goes on from what its reset returned (``info[i]["reset_*"]``), in the rollout's lists and
+        in the env's buffers."""
+        obs_list[i] = envs.buf_obs[i] = info[i]["reset_obs"]
+        if self.use_global_state:
+            state[i] = envs.buf_state[i] = info[i]["reset_state"]
+        if self.use_actions_mask:
+            avail_actions[i] = envs.buf_avail_actions[i] = info[i]["reset_avail_actions"]
+
     def _build_inputs(self, obs_list, avail_actions_list=None):
         """[n_envs * n_agents, obs_dim] (env-major, agent-minor) float32 and the matching uint8 availability rows."""
         K = self.agent_keys
@@ -175,8 +202,9 @@ class OffPolicyMARLAgents(MARLAgents):
                  action_space=None, callback=None):
         super().__init__(config, envs, num_agents, agent_keys, state_space, observation_space, action_space, callback)
         self.on_policy = False
-        self.start_greedy, self.end_greedy = getattr(config, "start_greedy", None), getattr(config, "end_greedy", None)
-        self.delta_egreedy = self.e_greedy = None
+        self.e_greedy = self.start_greedy = config.start_greedy
+        self.end_greedy = config.end_greedy
+        self.delta_egreedy = (self.start_greedy - self.end_greedy) / config.decay_step_greedy    # per environment step
         self.start_noise = self.end_noise = self.delta_noise = self.noise_scale = None     # discrete actions only
         self.buffer_size, self.batch_size = config.buffer_size, config.batch_size
         if self.world_size > 1:                       # global sizes -> this rank's shard (episodes are independent)
@@ -198,22 +226,30 @@ class OffPolicyMARLAgents(MARLAgents):
     def store_experience(self, obs_list, avail_actions, actions_list, obs_next_list, avail_actions_next, rewards_list,
                          terminals_list, info, **kwargs):
         """off_policy_marl.py:112-159 - per-env dicts -> per-agent [n_envs, ...] arrays -> memory.store."""
-        K = self.agent_keys
-        data = {'obs': {k: np.array([d[k] for d in obs_list]) for k in K},
-                'actions': {k: np.array([d[k] for d in actions_list]) for k in K},
-                'obs_next': {k: np.array([d[k] for d in obs_next_list]) for k in K},
-                'rewards': {k: np.array([d[k] for d in rewards_list]) for k in K},
-                'terminals': {k: np.array([d[k] for d in terminals_list]) for k in K},
-                'agent_mask': {k: np.array([d['agent_mask'][k] for d in info]) for k in K}}
+        data = {'obs': self._agent_arrays(obs_list), 'actions': self._agent_arrays(actions_list),
+                'obs_next': self._agent_arrays(obs_next_list), 'rewards': self._agent_arrays(rewards_list),
+                'terminals': self._agent_arrays(terminals_list),
+                'agent_mask': self._agent_arrays([d['agent_mask'] for d in info])}
         if self.use_rnn:
             data['episode_steps'] = np.array([d['episode_step'] - 1 for d in info])
         if self.use_global_state:
             data['state'] = np.array(kwargs['state'])
             data['state_next'] = np.array(kwargs['next_state'])
         if self.use_actions_mask:
-            data['avail_actions'] = {k: np.array([d[k] for d in avail_actions]) for k in K}
-            data['avail_actions_next'] = {k: np.array([d[k] for d in avail_actions_next]) for k in K}
+            data['avail_actions'] = self._agent_arrays(avail_actions)
+            data['avail_actions_next'] = self._agent_arrays(avail_actions_next)
         self.memory.store(**data)
+
+    def _build_q_networks(self):
+        q_networks = nn.ModuleDict()
+        for group_key, group_agents in self.groups.items():
+            ref = group_agents[0]
+            enc = self._build_agent_feature_encoder(self.config.representation, group_agents, self.observation_space[ref])
+            q_networks[group_key] = DiscreteActionValueCritic(
+                representation=enc, action_space=self.action_space[ref], critic_hidden_size=self.config.q_hidden_size,
+                normalizer=self.normalize_fn, initializer=self.initializer, activation=self.activation,
+                device=self.device)
+        return q_networks
 
     def init_rnn_states(self, n_envs):
         return self.model.init_rnn_states(n_envs)
@@ -223,8 +259,6 @@ class OffPolicyMARLAgents(MARLAgents):
 
     def _update_explore_factor(self):
         """off_policy_marl.py:198-210."""
-        if self.e_greedy is None:
-            return
         if self.e_greedy > self.end_greedy:
             self.e_greedy = self.start_greedy - self.delta_egreedy * self.current_step
         else:
@@ -233,7 +267,7 @@ class OffPolicyMARLAgents(MARLAgents):
     def exploration(self, batch_size, pi_actions_dict, avail_actions_list=None):
         """off_policy_marl.py:212-255: with probability epsilon the WHOLE vector step acts at random (one draw per call),
         uniformly over each agent's available actions when masks are in use."""
-        if self.e_greedy is None or np.random.rand() >= self.e_greedy:
+        if np.random.rand() >= self.e_greedy:
             return pi_actions_dict
         if self.use_actions_mask:
             out = []
@@ -317,14 +351,7 @@ class OffPolicyMARLAgents(MARLAgents):
             for i in range(num_envs):
                 if all(terminated_list[i].values()) or truncated[i]:
                     _current_episode += 1
-                    obs_list[i] = info[i]["reset_obs"]
-                    envs.buf_obs[i] = info[i]["reset_obs"]
-                    if self.use_global_state:
-                        state[i] = info[i]["reset_state"]
-                        envs.buf_state[i] = info[i]["reset_state"]
-                    if self.use_actions_mask:
-                        avail_actions[i] = info[i]["reset_avail_actions"]
-                        envs.buf_avail_actions[i] = info[i]["reset_avail_actions"]
+                    self._reset_env(envs, i, info, obs_list, state, avail_actions)
                     if self.use_rnn:
                         rnn_states = self.init_rnn_states_item(i_env=i, rnn_states=rnn_states)
                         if not test_mode:
@@ -375,8 +402,7 @@ class QMIX_Agents(OffPolicyMARLAgents):
         if self.state_space is None:
             raise ValueError("QMIX mixes on the global state: provide envs or state_space")
         self.use_global_state = True
-        self.start_greedy, self.end_greedy = config.start_greedy, config.end_greedy
-        self.e_greedy = self.start_greedy
+        # the reference's QMIX divides decay_step_greedy by n_envs (qmix_agents.py); IQL and DCG do not
         self.delta_egreedy = (self.start_greedy - self.end_greedy) / (config.decay_step_greedy / self.n_envs)
         self.model = self._build_model()
         self.memory = self._build_memory()
@@ -385,17 +411,6 @@ class QMIX_Agents(OffPolicyMARLAgents):
     def _build_mixer(self):
         return QMIX_Mixer(dim_state=self.state_space.shape[0], dim_hidden=self.config.hidden_dim_mixing_net,
                           dim_hypernet_hidden=self.config.hidden_dim_hyper_net, n_agents=self.n_agents, device=self.device)
-
-    def _build_q_networks(self):
-        q_networks = nn.ModuleDict()
-        for group_key, group_agents in self.groups.items():
-            ref = group_agents[0]
-            enc = self._build_agent_feature_encoder(self.config.representation, group_agents, self.observation_space[ref])
-            q_networks[group_key] = DiscreteActionValueCritic(
-                representation=enc, action_space=self.action_space[ref], critic_hidden_size=self.config.q_hidden_size,
-                normalizer=self.normalize_fn, initializer=self.initializer, activation=self.activation,
-                device=self.device)
-        return q_networks
 
     def _build_model(self):
         q_networks = self._build_q_networks()

@@ -1,10 +1,6 @@
 """QTRAN agents - mirror of xuance/torch/agents/multi_agent_rl/qtran_agents.py:17-101."""
-import torch.nn as nn
-
-from ..rl_models import (ActivationFunctions, AgentFeatureEncoder, Basic_RNN_K13, DiscreteActionValueCritic, VDN_mixer,
-                         QTRAN_Base, QTRAN_Alt, QTranMixingNetwork)
+from ..rl_models import VDN_mixer, QTRAN_Base, QTRAN_Alt, QTranMixingNetwork
 from ..rl_models.qtran import check_limits
-from ...common import space2shape
 from .marl import QMIX_Agents
 
 
@@ -26,22 +22,8 @@ class QTRAN_Agents(QMIX_Agents):
                              % (config.q_hidden_size[0], config.recurrent_hidden_size))
         super().__init__(config, envs, num_agents, agent_keys, state_space, observation_space, action_space, callback)
 
-    def _build_q_networks(self):
-        cfg = self.config
-        q_networks = nn.ModuleDict()
-        for group_key, group_agents in self.groups.items():
-            ref = group_agents[0]
-            rep = Basic_RNN_K13(input_shape=space2shape(self.observation_space[ref]),
-                                hidden_sizes=getattr(cfg, "representation_hidden_size", None), normalize=None,
-                                initialize=nn.init.orthogonal_, activation=ActivationFunctions[cfg.activation],
-                                fc_hidden_sizes=cfg.fc_hidden_sizes, N_recurrent_layers=cfg.N_recurrent_layers,
-                                recurrent_hidden_size=cfg.recurrent_hidden_size, rnn=cfg.rnn, dropout=cfg.dropout,
-                                device=self.device)
-            q_networks[group_key] = DiscreteActionValueCritic(
-                representation=AgentFeatureEncoder(rep), action_space=self.action_space[ref],
-                critic_hidden_size=cfg.q_hidden_size, normalizer=self.normalize_fn, initializer=self.initializer,
-                activation=self.activation, device=self.device)
-        return q_networks
+    def _build_agent_feature_encoder(self, representation_choice, group_agents, input_space):
+        return self._build_k13_encoder(input_space, None)
 
     def _build_model(self):
         cfg = self.config

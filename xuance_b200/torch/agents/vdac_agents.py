@@ -8,10 +8,8 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from ...common.spaces import space2shape
-from ..rl_models import (CategoricalActor, StateValueCritic, Basic_RNN_K13, QMIX_Mixer, VDN_mixer,
-                         IndependentActorCritic, ValueDecompositionActorCritic)
-from ..rl_models.qmix import AgentFeatureEncoder
+from ..rl_models import (CategoricalActor, StateValueCritic, QMIX_Mixer, VDN_mixer, IndependentActorCritic,
+                         ValueDecompositionActorCritic)
 from .mappo_agents import OnPolicyMARLAgents
 
 QMIX_MAX_AGENTS = 16     # K9 mix (xb_qmix_mix_fwd / _bwd)
@@ -33,18 +31,6 @@ class IAC_Agents(OnPolicyMARLAgents):
 
     def _check_scope(self):
         pass
-
-    def _build_agent_feature_encoder(self, representation_choice, group_agents, input_space):
-        if not self.use_rnn:
-            return super()._build_agent_feature_encoder(representation_choice, group_agents, input_space)
-        if representation_choice != "Basic_RNN":
-            raise NotImplementedError("use_rnn=True takes representation: Basic_RNN, got %s" % representation_choice)
-        c = self.config
-        return AgentFeatureEncoder(Basic_RNN_K13(
-            input_shape=space2shape(input_space), normalize=self.normalize_fn, initialize=nn.init.orthogonal_,
-            activation=self.activation, device=self.device, fc_hidden_sizes=c.fc_hidden_sizes,
-            recurrent_hidden_size=c.recurrent_hidden_size, N_recurrent_layers=getattr(c, "N_recurrent_layers", 1),
-            rnn=getattr(c, "rnn", "GRU"), dropout=getattr(c, "dropout", 0)))
 
     def _actors_critics(self):
         actors, critics = nn.ModuleDict(), nn.ModuleDict()

@@ -7,6 +7,8 @@ backward's ``dW_hh = sum dgh^T h_{t-1}`` / ``db_hh = sum dgh`` are one GEMM and 
 kernel with T = 1 and a carried state, so a rollout step and step t of the training forward execute the same code.
 
 QMIX keeps its cuDNN ``Basic_RNN`` (rl_models/qmix.py); moving it onto K13 would change its numerics."""
+from types import SimpleNamespace
+
 import torch
 import torch.nn as nn
 
@@ -17,10 +19,23 @@ from .outputs import RepresentationOutput
 MAX_HIDDEN = 64   # K13 keeps W_hh [3H, H] resident in shared memory: 48 KB at H = 64
 
 
-def check_hidden_size(H):
+def check_hidden_size(H, name="K13 GRU sequence kernels"):
     if not 1 <= H <= MAX_HIDDEN:
-        raise NotImplementedError("K13 GRU sequence kernels: recurrent_hidden_size %d is outside the supported 1..%d"
-                                  % (H, MAX_HIDDEN))
+        raise NotImplementedError("%s: recurrent_hidden_size %d is outside the supported 1..%d"
+                                  % (name, H, MAX_HIDDEN))
+
+
+def check_scope(name, config):
+    """Refuse a recurrent representation K13 does not run, naming ``name`` (the algorithm) in the error: K13 runs one
+    GRU layer of 1..MAX_HIDDEN units without dropout.  ``config`` has ``recurrent_hidden_size`` and may have ``rnn``,
+    ``N_recurrent_layers`` and ``dropout`` (defaults GRU, 1, 0)."""
+    if getattr(config, "rnn", "GRU") != "GRU":
+        raise NotImplementedError("%s: LSTM representations are not supported (GRU only)" % name)
+    if getattr(config, "N_recurrent_layers", 1) != 1:
+        raise NotImplementedError("%s: N_recurrent_layers > 1 is not supported (one GRU layer)" % name)
+    if getattr(config, "dropout", 0) > 0:
+        raise NotImplementedError("%s: dropout > 0 is not supported" % name)
+    check_hidden_size(config.recurrent_hidden_size, name)
 
 
 class GRUSequence(torch.autograd.Function):
@@ -79,16 +94,10 @@ class Basic_RNN_K13(nn.Module):
     def __init__(self, input_shape, hidden_sizes=None, normalize=None, initialize=None, activation=None, device=None,
                  **kwargs):
         super().__init__()
-        if kwargs.get("rnn", "GRU") != "GRU":
-            raise NotImplementedError("recurrent MAPPO: LSTM representations are not supported (GRU only)")
-        if kwargs.get("N_recurrent_layers", 1) != 1:
-            raise NotImplementedError("recurrent MAPPO: N_recurrent_layers > 1 is not supported (one GRU layer)")
-        if kwargs.get("dropout", 0) > 0:
-            raise NotImplementedError("recurrent MAPPO: dropout > 0 is not supported")
+        check_scope("Basic_RNN_K13", SimpleNamespace(**kwargs))
         self.input_shape = input_shape
         self.fc_hidden_sizes = kwargs["fc_hidden_sizes"]
         self.recurrent_hidden_size = kwargs["recurrent_hidden_size"]
-        check_hidden_size(self.recurrent_hidden_size)
         self.N_recurrent_layer = 1
         self.lstm = False
         self.normalize, self.device = normalize, device
