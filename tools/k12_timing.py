@@ -53,7 +53,7 @@ def roles():
     out3 = torch.empty(Pn, B * 100, 64, dtype=torch.bfloat16, device=DEV)
     wd3 = tc.split_bf16(tc.dgrad_weight_matrix(convs[2].weight.detach(), P["taps3"]), Pn)
     wd2 = torch.cat([tc.split_bf16(tc.dgrad_weight_matrix(convs[1].weight.detach(), taps), Pn) for _, taps in P["dg2"]], 1).contiguous()
-    report("conv1 forward (gathered cp.async)", lambda: tc.gemm_gather(x, w1, P["fwd1"], relu=True, out_pl=act1, out_ld=32))
+    report("conv1 forward (TMA windows)", lambda: tc.gemm_gather(x, w1, P["fwd1"], relu=True, out_pl=act1, out_ld=32))
     report("conv2 forward (box)", lambda: tc.gemm_box(act1_pairs, w2, P["fwd2"], relu=True, out_pl=d2, out_ld=64))
     report("conv3 forward (box)", lambda: tc.gemm_box(act2, w3, P["fwd3"], relu=True, out_pl=out3, out_ld=64))
     report("conv3 forward (halo)", lambda: tc.gemm_halo(act2, w3, P["h_fwd3"], relu=True, out_pl=out3, out_ld=64))
@@ -73,7 +73,7 @@ def launch_labels(tc, P):
     """(ABI name, label) of every K12 launch of BoxNatureCNN.forward + backward, in launch order (tc_conv.py)."""
     dg = "xb_gemm_halo_tc" if tc.HALO3 else "xb_gemm_box_tc"
     wg = lambda box: "xb_wgrad_box_tc" if box else "xb_wgrad_gather_tc"
-    seq = [("xb_gemm_gather_tc", "conv1 forward"), ("xb_gemm_box_tc", "conv2 forward"), (dg, "conv3 forward"),
+    seq = [("xb_gemm_gather_tc", "conv1 forward (TMA windows)"), ("xb_gemm_box_tc", "conv2 forward"), (dg, "conv3 forward"),
            ("xb_gemm_gather_tc", "Linear forward"), ("xb_wgrad_gather_tc", "Linear weight gradient"),
            ("xb_gemm_gather_tc", "Linear data gradient"), (wg(tc.BOX_WGRAD3), "conv3 weight gradient"),
            (dg, "conv3 data gradient"), (wg(tc.BOX_WGRAD2), "conv2 weight gradient")]

@@ -210,8 +210,8 @@ XB_HD void xb_stage_wgrad(const XbConvGeom &g, const XbUnit *tab, int pt, int64_
 // ---------------------------------------------------------------------------------------------------------------------
 // units per window row: every tap of every site of a grid row
 XB_HD int xb_win_width(const XbConvGeom &g) { return g.sx * (g.OX - 1) + (g.dx[g.T - 1] - g.dx[0]) + 1; }
-// grid rows one chunk of XB_CONV_KC consecutive sites can touch
-XB_HD int xb_win_rows(const XbConvGeom &g) { return (XB_CONV_KC - 2 + g.OX) / g.OX + 1; }
+// grid rows a run of `sites` consecutive sites can touch (a weight-gradient chunk: XB_CONV_KC; a forward item: XB_CONV_TILE_M)
+XB_HD int xb_win_rows(const XbConvGeom &g, int sites = XB_CONV_KC) { return (sites - 2 + g.OX) / g.OX + 1; }
 // first input row and image of window slot R (grid row R; b >= B past the last image)
 XB_HD void xb_win_box(const XbConvGeom &g, int64_t R, int &b, int &iy0) {
     int y, x;

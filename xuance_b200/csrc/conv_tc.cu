@@ -153,6 +153,14 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
+// bulk copy shared -> global (the copy engine, no per-lane stores), completion tracked per issuing thread in bulk groups
+__device__ __forceinline__ void bulk_store(void *dst, uint32_t src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every bulk group this thread committed has finished READING shared memory (its source may be overwritten)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // x = hi + mid + lo, three bf16 values: 24 mantissa bits, |x - hi - mid - lo| <= 2^-24 |x|
 __device__ __forceinline__ void split3_bf16(float x, __nv_bfloat16 &hi, __nv_bfloat16 &mid, __nv_bfloat16 &lo) {
     hi = __float2bfloat16_rn(x);
@@ -948,6 +956,170 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel_wgrad_pairs(const _
     }
 }
 
+// The forward of a raw-pixel first layer (one A plane, C = 8, a full tap rectangle, K = 256, N = 32, bf16 plane outputs
+// whose sites are 64-byte rows, no mask / column sums; selected by xb_gemm_gather_tc) with every transfer on the copy
+// engines.  Work items are the gathered path's: 128 consecutive sites, rows 0-63 / 64-127 for the two consumer warpgroups.
+//   * weights: RESIDENT, loaded once per CTA by TMA (the gathered path's b_tma boxes: per 64-deep chunk {64 k, 32 rows, PB
+//     planes}, 128-byte swizzle);
+//   * input: per item one window (conv_index.h, xb_win_*) of xb_win_rows(g, 128) boxes of KH rows x win_w units, zero fill
+//     for padding and past the last image; two stages.  An item reads all K from it, so it needs no per-chunk loads;
+//   * outputs: the consumers write the split bf16 planes into a staging tile [plane][128 sites][64 B] and, after a named
+//     barrier, lane j of warp 0 copies the run of the item's sites in grid row R0 + j (consecutive real pixels, contiguous
+//     in every plane of the output) with one cp.async.bulk per plane.  Two staging tiles: a tile is rewritten only after the
+//     copies that read it have been waited for (wait_group.read before the barrier of the next item).
+// The consumers read K-major A fragments with ldmatrix at xb_win_site_off + xb_win_tap_off and issue per K step the
+// gathered path's n32 wgmmas on the same fragments, B planes and accumulators in the same order, and the epilogue adds the
+// groups, bias and ReLU as it does: the outputs are bit for bit those of conv_tc_kernel<false, 1, PB, 1>.
+template <int PB>
+__global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel_fwd_win(const __grid_constant__ ConvParams p) {
+    constexpr int KS = 256 / 16;                             // K steps of an item
+    constexpr uint32_t W_CHUNK = PB * 32 * KC * 2, W_BYTES = 4 * W_CHUNK;     // resident weights, per 64-deep chunk / all
+    constexpr uint32_t STG_PLANE = TILE_M * 32 * 2;          // staging: one output plane of an item
+    extern __shared__ __align__(1024) uint8_t smem[];
+    __shared__ __align__(8) uint64_t w_full, full_bar[2], empty_bar[2];
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const XbConvGeom &g = p.g;
+    const uint32_t win_stage = ((uint32_t)p.win_rows * p.win_slot + 1023u) & ~1023u;     // as fwd_win_setup
+    const uint32_t stg_off = W_BYTES + 2u * win_stage, stg_buf = (uint32_t)p.p_out * STG_PLANE;
+    const int64_t n_items = (p.M + TILE_M - 1) / TILE_M;
+    if (tid == 0) {
+        mbar_init(&w_full, 1);
+        for (int s = 0; s < 2; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], CONS_WARPS);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+    const uint32_t smem_base = smem_u32(smem);
+    if (smem_base & 1023u) __trap();                         // the 128-byte swizzle pattern repeats every 1024 B
+    uint32_t t_wait[5] = {0, 0, 0, 0, 0};                   // role timing, slots as in conv_tc_kernel
+    if (p.timing && blockIdx.x < 160 && (tid == 0 || tid == CONS_WARPS * 32)) xb_k12_timing[blockIdx.x][tid == 0 ? 0 : 4] = clock64();
+    auto timed_wait = [&](uint64_t *bar, uint32_t parity, int slot) {
+        if (p.timing) {
+            const uint32_t t0 = clock32();
+            mbar_wait(bar, parity);
+            t_wait[slot] += clock32() - t0;
+        } else {
+            mbar_wait(bar, parity);
+        }
+    };
+
+    if (warp >= CONS_WARPS) {
+        // ------------------------------------------------------------------ producer: one thread issues every copy
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PROD_REGS));
+        if (tid == CONS_WARPS * 32) {
+            mbar_expect_tx(&w_full, W_BYTES);
+#pragma unroll
+            for (int kc = 0; kc < 4; ++kc) tma_load_3d(smem_base + kc * W_CHUNK, &p.tm_b, kc * KC, 0, 0, &w_full);
+            const uint32_t bytes = (uint32_t)(p.win_rows * p.win_kh * p.win_w * 16);
+            uint32_t it = 0;
+            for (int64_t w = blockIdx.x; w < n_items; w += gridDim.x, ++it) {
+                const uint32_t stage = it & 1u;
+                timed_wait(&empty_bar[stage], ((it >> 1) & 1u) ^ 1u, 0);
+                const uint32_t base = smem_base + W_BYTES + stage * win_stage;
+                const int64_t R0 = xb_div((uint32_t)(w * TILE_M), g.div_ox);      // first grid row of the item
+                mbar_expect_tx(&full_bar[stage], bytes);
+                for (int j = 0; j < p.win_rows; ++j) {
+                    int b, iy0;
+                    xb_win_box(g, R0 + j, b, iy0);
+                    // 8-byte elements: unit u is elements 2u, 2u + 1
+                    tma_load_3d(base + (uint32_t)j * p.win_slot, &p.tm_a, 2 * g.dx[0], iy0, b, &full_bar[stage]);
+                }
+            }
+        }
+    } else {
+        // ------------------------------------------------------------------ consumers: wgmma issue + epilogue
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONS_REGS));
+        const int wg = warp >> 2;
+        // this lane's ldmatrix row (see conv_tc_kernel): site m_l + lr of the warpgroup's 64, K unit 2 ks + (mi >> 1)
+        const int mi = lane >> 3, lr = lane & 7, m_l = 16 * (warp & 3) + 8 * (mi & 1);
+        uint32_t tap_off[KS];
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) tap_off[ks] = xb_win_tap_off(g, 8 * (2 * ks + (mi >> 1)), p.win_w);
+        const int rbase = 64 * wg + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+        float bias[4][2];                                    // this thread's 8 columns 8 i + cq + e
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) bias[i][e] = p.bias ? p.bias[8 * i + cq + e] : 0.f;
+        // B as in conv_tc_kernel's forward with b_tma: K step of 16 = 32 B within a chunk, chunks W_CHUNK apart
+        const uint64_t b0 = make_desc_sw128(0, 16, 1024) + (uint64_t)(smem_base >> 4);
+        timed_wait(&w_full, 0, 0);
+        float acc[PB][16];
+        uint32_t it = 0;
+        for (int64_t w = blockIdx.x; w < n_items; w += gridDim.x, ++it) {
+            const uint32_t stage = it & 1u;
+            const int64_t m0 = w * TILE_M;
+            const int64_t R0 = xb_div((uint32_t)m0, g.div_ox);      // first grid row of the item
+            const uint32_t row = smem_base + W_BYTES + stage * win_stage + xb_win_site_off(g, m0 + 64 * wg + m_l + lr, R0, p.win_slot);
+            timed_wait(&full_bar[stage], (it >> 1) & 1u, 0);
+            // every fragment of the item is loaded while no wgmma is in flight (see conv_tc_kernel)
+            uint32_t af[KS][4];
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks) ldmatrix_x4<0>(af[ks], row + tap_off[ks]);
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks)
+                mma_plane<0, PB, 1, 0>(acc, af[ks], b0 + (uint64_t)(((ks >> 2) * W_CHUNK + (ks & 3) * 32) >> 4), ks == 0 ? 0u : 1u);
+            wgmma_commit();
+            timed_wgmma_wait<0>(p.timing, t_wait[3]);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[stage]);
+            const uint32_t t_epi = p.timing ? clock32() : 0u;
+            // ---- epilogue: rows rbase (h = 0) and rbase + 8 (h = 1) into the staging tile, groups added smallest first
+            uint8_t *stg = smem + stg_off + stage * stg_buf;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    float v[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        v[e] = acc[PB - 1][4 * i + 2 * h + e];
+#pragma unroll
+                        for (int gq = PB - 2; gq >= 0; --gq) v[e] += acc[gq][4 * i + 2 * h + e];
+                        v[e] += bias[i][e];
+                        if (p.relu) v[e] = fmaxf(v[e], 0.f);
+                    }
+                    __nv_bfloat16 q0[3], q1[3];
+                    split3_bf16(v[0], q0[0], q0[1], q0[2]);
+                    split3_bf16(v[1], q1[0], q1[1], q1[2]);
+                    uint8_t *dst = stg + (rbase + 8 * h) * 64 + (8 * i + cq) * 2;
+#pragma unroll
+                    for (int q = 0; q < 3; ++q)
+                        if (q < p.p_out) *reinterpret_cast<uint32_t *>(dst + q * STG_PLANE) = pack2(q0[q], q1[q]);
+                }
+            fence_proxy_async();           // written by the generic proxy, read by the bulk copies (async proxy)
+            // the copies of the item before this one have read the other staging tile: free for the next item
+            if (warp == 0) bulk_wait_read_all();
+            asm volatile("bar.sync 1, %0;" ::"n"(CONS_WARPS * 32) : "memory");
+            if (warp == 0 && lane < p.win_rows) {
+                // lane j: the sites of grid row R0 + j in this item, consecutive pixels of one output row
+                const int64_t R = R0 + lane, m1 = m0 + TILE_M < p.M ? m0 + TILE_M : p.M;
+                const int64_t s0 = R * g.OX > m0 ? R * g.OX : m0, s1 = (R + 1) * g.OX < m1 ? (R + 1) * g.OX : m1;
+                if (s0 < s1) {
+                    int b, y, x;
+                    xb_conv_site(g, s0, b, y, x);
+                    const int64_t orow = (((int64_t)b * p.out_H + y * p.oys + p.oy0) * p.out_W + x + p.ox0) * 32;
+                    const uint32_t src = smem_u32(stg) + (uint32_t)(s0 - m0) * 64u, n = (uint32_t)(s1 - s0) * 64u;
+                    for (int q = 0; q < p.p_out; ++q) bulk_store(p.out[q] + orow, src + q * STG_PLANE, n);
+                }
+                bulk_commit();
+            }
+            if (p.timing) t_wait[4] += clock32() - t_epi;
+        }
+        if (warp == 0) bulk_wait_all();
+    }
+    if (p.timing && blockIdx.x < 160) {
+        const unsigned long long now = clock64();
+        unsigned long long *o = xb_k12_timing[blockIdx.x];
+        if (tid == 0) o[0] = now - o[0], o[1] = t_wait[0], o[2] = t_wait[3], o[3] = 0, o[7] = t_wait[4];
+        if (tid == CONS_WARPS * 32) o[4] = now - o[4], o[5] = t_wait[0], o[6] = 0;
+    }
+}
+
 // weight-gradient finish: sum the split partials [splits, K, N] in a fixed order and scatter to torch's [N, C, KH, KW]
 // (column k = (kh, kw, c) of the packed layout -> xb_pack_weight_src); accumulate != 0 adds to dw (autograd .grad).
 // A block owns E = 256 / lanes consecutive (k, n) elements - coalesced rows of the partial matrices - and `lanes` threads
@@ -1317,21 +1489,60 @@ int launch(int pa, int pb, const ConvParams &p, int64_t work, void *stream) {
     return XB_EINVAL;
 }
 
-// conv_tc_kernel_wgrad_win takes a weight gradient whose A operand is one plane of 16-byte units (C = 8) read through a full
-// KH x KW tap rectangle in row-major order, with N = n_tile = 32 and 64 <= K <= 256 (two m64 row blocks per consumer
-// warpgroup) - conv1 over raw pixels, 4 channels folded in pixel pairs.  Fills the window fields and the ring of p.
-bool wgrad_win_setup(ConvParams &p, int planes_a, int planes_b, int N, int n_tile) {
+// The window fields of p (conv_index.h, xb_win_*) for runs of `sites` consecutive sites, if the A operand is one plane of
+// 16-byte units (C = 8) read through a full KH x KW tap rectangle in row-major order.
+bool win_fields(ConvParams &p, int planes_a, int sites) {
     const XbConvGeom &g = p.g;
-    if (planes_a != 1 || g.C != 8 || N != 32 || n_tile != 32 || g.T % 8 != 0 || g.T * g.C > 2 * TILE_M) return false;
+    if (planes_a != 1 || g.C != 8) return false;
     int KW = 1;
     while (KW < g.T && g.dy[KW] == g.dy[0]) ++KW;
     if (g.T % KW != 0) return false;
     for (int t = 0; t < g.T; ++t)
         if (g.dy[t] != g.dy[0] + t / KW || g.dx[t] != g.dx[0] + t % KW) return false;
     const int KH = g.T / KW, win_w = xb_win_width(g);
-    if (2 * win_w > 256 || KH > 256 || p.M + KC >= ((int64_t)1 << 31)) return false;      // box limits, 32-bit site indices
-    p.win_kh = KH, p.win_w = win_w, p.win_rows = xb_win_rows(g);
+    if (2 * win_w > 256 || KH > 256 || p.M + sites >= ((int64_t)1 << 31)) return false;    // box limits, 32-bit site indices
+    p.win_kh = KH, p.win_w = win_w, p.win_rows = xb_win_rows(g, sites);
     p.win_slot = ((uint32_t)(KH * win_w * 16) + 127u) & ~127u;             // TMA destinations 128-byte aligned
+    return true;
+}
+
+// conv_tc_kernel_fwd_win takes a forward whose A operand is as in win_fields with K = 256, N = n_tile = 32 and bf16 plane
+// outputs only (no fp32 output, mask or column sums), each site a contiguous 64-byte row of every output plane (oxs = 1,
+// out_ld = 32, out_c0 = 0) - conv1 over raw pixels into act1.  Fills the window fields and the shared-memory size of p.
+bool fwd_win_setup(ConvParams &p, int planes_a, int planes_b, int N, int n_tile) {
+    const XbConvGeom &g = p.g;
+    if (N != 32 || n_tile != 32 || g.T * g.C != 256 || p.p_out == 0 || p.out_f32 || p.mask || p.colsum) return false;
+    if (p.oxs != 1 || p.out_ld != 32 || p.out_c0 != 0) return false;
+    if (!win_fields(p, planes_a, TILE_M) || p.win_rows > 32) return false;
+    if (p.M + TILE_M + (int64_t)p.win_rows * g.OX >= ((int64_t)1 << 31)) return false;  // the window's last grid row
+    // resident weights, two window stages (1024-byte aligned as the kernel lays them out), two staging tiles
+    const uint32_t win_stage = ((uint32_t)p.win_rows * p.win_slot + 1023u) & ~1023u;
+    const uint32_t bytes = (uint32_t)planes_b * 32u * 256u * 2u + 2u * win_stage + 2u * (uint32_t)p.p_out * TILE_M * 64u;
+    if (bytes > (uint32_t)XB_K12_MAX_DYN_SMEM) return false;
+    p.stages = 2;
+    p.dyn_smem = bytes;
+    return true;
+}
+
+template <int PB>
+int launch_fwd_win(const ConvParams &p, void *stream) {
+    static bool attr = false;
+    if (!attr) {
+        cudaFuncSetAttribute(conv_tc_kernel_fwd_win<PB>, cudaFuncAttributeMaxDynamicSharedMemorySize, XB_K12_MAX_DYN_SMEM);
+        attr = true;
+    }
+    const int64_t items = (p.M + TILE_M - 1) / TILE_M;
+    const int grid = (int)(items < xb_sm_count() ? items : xb_sm_count());
+    conv_tc_kernel_fwd_win<PB><<<grid, THREADS, p.dyn_smem, (cudaStream_t)stream>>>(p);
+    return xb_launch_status();
+}
+
+// conv_tc_kernel_wgrad_win takes a weight gradient whose A operand is one plane of 16-byte units (C = 8) read through a full
+// KH x KW tap rectangle in row-major order, with N = n_tile = 32 and 64 <= K <= 256 (two m64 row blocks per consumer
+// warpgroup) - conv1 over raw pixels, 4 channels folded in pixel pairs.  Fills the window fields and the ring of p.
+bool wgrad_win_setup(ConvParams &p, int planes_a, int planes_b, int N, int n_tile) {
+    const XbConvGeom &g = p.g;
+    if (N != 32 || n_tile != 32 || g.T % 8 != 0 || g.T * g.C > 2 * TILE_M || !win_fields(p, planes_a, KC)) return false;
     // stage: the output-gradient box (4096 B per plane) + the window slots, 1024-byte aligned (the 64-byte swizzle
     // pattern of the box repeats every 512 B of absolute address)
     const uint32_t stage_bytes = ((uint32_t)planes_b * 4096u + (uint32_t)p.win_rows * p.win_slot + 1023u) & ~1023u;
@@ -1468,6 +1679,15 @@ extern "C" int xb_gemm_gather_tc(int planes_a, int planes_b, const void *in, int
     p.out_H = out_H, p.out_W = out_W, p.oys = oys, p.oxs = oxs, p.oy0 = oy0, p.ox0 = ox0;
     p.out_ld = out_ld, p.out_c0 = out_c0;
     p.splits = 1, p.sites_per_split = 0, p.w_ld = 0;
+    if (tma_enabled() && fwd_win_setup(p, planes_a, planes_b, N, n_tile)) {
+        // input windows and resident weights by TMA, outputs by bulk copies (conv_tc_kernel_fwd_win)
+        if (!make_tmap_win(&p.tm_a, in, B, IH, IW, p.win_w, p.win_kh) ||
+            !make_tmap(&p.tm_b, w, (int64_t)T * C, N, planes_b, (int64_t)T * C, w_plane, n_tile))
+            return XB_EINVAL;
+        if (planes_b == 1) return launch_fwd_win<1>(p, stream);
+        if (planes_b == 2) return launch_fwd_win<2>(p, stream);
+        return launch_fwd_win<3>(p, stream);
+    }
     if (tma_enabled()) {
         const int64_t K = (int64_t)T * C;
         // weights [planes_b][N][K]: tiles of {64 k, n_tile rows, all planes}
