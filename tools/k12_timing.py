@@ -58,7 +58,8 @@ def roles():
     report("conv3 forward (box)", lambda: tc.gemm_box(act2, w3, P["fwd3"], relu=True, out_pl=out3, out_ld=64))
     report("conv3 forward (halo)", lambda: tc.gemm_halo(act2, w3, P["h_fwd3"], relu=True, out_pl=out3, out_ld=64))
     report("conv3 data gradient (halo)", lambda: tc.gemm_halo(g3, wd3, P["h_dg3"], out_pl=d2, out_ld=64, relu_mask=act2[0]))
-    report("conv2 data gradient (halo)", lambda: tc.gemm_halo(g3, wd2, P["h_dg2"], out_pl=d1, out_ld=32, relu_mask=act1[0]))
+    cs1 = torch.empty(P["h_dg2"].m_tiles, 32, device=DEV)
+    report("conv2 data gradient (phase pairs)", lambda: tc.gemm_halo(g3, wd2, P["h_dg2"], out_pl=d1, out_ld=32, relu_mask=act1[0], colsum=cs1))
     sp = tc.wgrad_box_splits(B * P["hp2"], 6, 576, 64)
     report("conv3 weight gradient (box)", lambda: tc.wgrad_box(act2, g3, P["fwd3"], 6, sp))
     report("conv2 weight gradient (TMA pairs)", lambda: enc.be.wgrad(act1, g3.view(Pn, -1, 64), P["wg2"], 64, 32, 4, 4))
@@ -78,7 +79,7 @@ def launch_labels(tc, P):
            ("xb_gemm_gather_tc", "Linear data gradient"), (wg(tc.BOX_WGRAD3), "conv3 weight gradient"),
            (dg, "conv3 data gradient"), (wg(tc.BOX_WGRAD2), "conv2 weight gradient")]
     if tc.HALO and P["h_dg2"] is not None:
-        seq.append(("xb_gemm_halo_tc", "conv2 data gradient"))
+        seq.append(("xb_gemm_halo_tc", "conv2 data gradient (phase pairs)"))
     else:
         seq += [("xb_gemm_box_tc", "conv2 data gradient, phase %d" % i) for i in range(len(P["dg2"]))]
     return seq + [("xb_wgrad_gather_tc", "conv1 weight gradient")]

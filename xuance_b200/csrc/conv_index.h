@@ -265,6 +265,42 @@ XB_HD uint32_t xb_pwin_site_off(const XbConvGeom &g, int64_t s, int64_t R0, uint
 // the 128-byte swizzle as TMA applies it: the 16-byte unit (bits 4-6) XOR bits 7-9 of the shared-memory address
 XB_HD uint32_t xb_sw128(uint32_t a) { return a ^ (((a >> 7) & 7u) << 4); }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Data gradient of a stride-2 layer by stride-phase PAIRS (conv_tc.cu, conv_tc_kernel_dgrad_phases): the halo raster's
+// positions P = R * halo_w + hc (raster row R = b * hp + y, pixel x = hc + halo_w0) of the M tile whose first position is
+// p0 are computed in the four phases (py, px) as sub-items; phase (py, px) writes output pixel 2x + px of output row
+// xb_pair_out_row(R, py).  The phases (py, 0) and (py, 1) together write, for each raster row of the tile, ONE run of
+// consecutive pixels of that output row (x1_odd is x1_even or x1_even - 1): the kernel stages the pair's outputs as whole
+// output rows (slot R - xb_pair_row0 of the tile) and stores every run with one bulk copy per plane.  A raster row cut by a
+// tile boundary gives two runs, each stored by its own tile.
+// ---------------------------------------------------------------------------------------------------------------------
+// raster rows an M tile can touch (staging slots)
+XB_HD int xb_pair_slots(int halo_w) { return (XB_CONV_TILE_M - 2 + halo_w) / halo_w + 1; }
+// first raster row of the M tile whose first position is p0 (slot 0)
+XB_HD uint32_t xb_pair_row0(int64_t p0, const XbDiv &div_w) { return xb_div((uint32_t)p0, div_w); }
+// output row of raster row R in the phases of row phase py (first output row oy0, valid raster rows y0 .. y1 of each image
+// of hp rows, `rows` = B * hp raster rows); -1 if that pair writes no pixel of it
+XB_HD int64_t xb_pair_out_row(uint32_t R, uint32_t rows, const XbDiv &div_hp, int hp, int y0, int y1, int oy0, int out_H) {
+    if (R >= rows) return -1;
+    const uint32_t b = xb_div(R, div_hp);
+    const int y = (int)(R - b * (uint32_t)hp);
+    if (y < y0 || y > y1) return -1;
+    return (int64_t)b * out_H + 2 * (y - y0) + oy0;
+}
+// the run [lo, hi] of output pixels that the tile from p0 writes in raster row R: pixels 2x of the positions with
+// 0 <= x <= x1_even and 2x + 1 of those with x <= x1_odd; returns hi - lo + 1 (0: no pixel)
+XB_HD int xb_pair_run(int64_t p0, uint32_t R, int halo_w, int halo_w0, int x1_even, int x1_odd, int &lo, int &hi) {
+    const int64_t r0 = (int64_t)R * halo_w;
+    const int h0 = p0 > r0 ? (int)(p0 - r0) : 0;
+    const int h1 = p0 + XB_CONV_TILE_M - 1 < r0 + halo_w - 1 ? (int)(p0 + XB_CONV_TILE_M - 1 - r0) : halo_w - 1;
+    const int xa = h0 + halo_w0 > 0 ? h0 + halo_w0 : 0, xb = h1 + halo_w0;
+    const int xe = xb < x1_even ? xb : x1_even, xo = xb < x1_odd ? xb : x1_odd;        // last x of each phase
+    lo = xa <= xe ? 2 * xa : 2 * xa + 1;
+    hi = 2 * xe > 2 * xo + 1 ? 2 * xe : 2 * xo + 1;
+    if (xa > xe && xa > xo) lo = 0, hi = -1;
+    return hi - lo + 1;
+}
+
 // shared-memory bytes of one pipeline stage: the P planes of A (hi | [mid |] lo) followed by the P planes of W.
 // P = 2: x = hi + lo (|err| <= 2^-16 |x|, 3 products);  P = 3: x = hi + mid + lo (<= 2^-24 |x|, 6 products)
 XB_HD uint32_t xb_conv_stage_bytes(int N, int P = 2) {

@@ -1120,6 +1120,283 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel_fwd_win(const __gri
     }
 }
 
+// The data gradient of a stride-2 layer as four stride phases (py, px) of N = 32 columns over a resident halo tile (three
+// planes each side, bf16 plane outputs whose pixels are 64-byte rows, ReLU mask and column sums, no bias or fp32 output;
+// selected by xb_gemm_halo_tc) - conv2's data gradient into g1.  Work items, mainloop and producer are conv_tc_kernel's in
+// halo mode: an M tile of 128 positions with its four sub-items back to back on the same halo tile, the same n32 wgmmas
+// on the same fragments, B planes and accumulators in the same order, groups added smallest first.  Only the epilogue
+// differs, and not in its arithmetic:
+//   * staging: phases (py, 0) and (py, 1) are consecutive sub-items and write every pixel of the output rows of the tile's
+//     raster rows (conv_index.h, xb_pair_*).  The consumers write their split planes into a staging tile laid out as those
+//     rows, [plane][slot = raster row - xb_pair_row0][out_W pixels][64 B], and after the second phase a helper thread of
+//     the producer warpgroup stores each run of pixels with one cp.async.bulk per plane.  Nothing else of the output is
+//     written (padding rows stay untouched).  The first phase of the next pair writes the tile once those stores have
+//     read it (stg_empty);
+//   * mask: each consumer loads its 8 mask words of a sub-item BEFORE the sub-item's MMAs, which hide their latency.  (The
+//     masks bulk-copied into staging plane 0 measured slower: that load can start only when the previous pair's stores
+//     have read the tile, and one sub-item of MMAs does not cover it; beside the tile there is no room for them.);
+//   * column sums: the per-warp shuffle sums go to s_colsum[tile parity][sub-item][warp], and the tile's four column-sum
+//     rows are added in the same fixed warp order after ONE consumer barrier per tile.
+// The outputs and column sums are therefore bit for bit those of conv_tc_kernel<false, 3, 3, 1>.
+__global__ void __launch_bounds__(THREADS, 1) conv_tc_kernel_dgrad_phases(const __grid_constant__ ConvParams p) {
+    constexpr int PA = 3, PB = 3, NC = 1, N = 32, N_SUB = 4;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    __shared__ __align__(8) uint64_t full_bar[MAX_STAGES], empty_bar[MAX_STAGES], a_full[2], a_empty[2], stg_full, stg_empty;
+    __shared__ float s_colsum[2][N_SUB][CONS_WARPS][N];
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int S = p.stages, n_chunks = p.halo_chunks, n_slots = xb_pair_slots(p.halo_w);
+    const uint32_t w_plane = xb_conv_w_plane_bytes(N), stage_bytes = PB * w_plane;
+    const uint32_t halo_plane = ((uint32_t)(p.halo_rows * p.halo_w) * 128u + 1023u) & ~1023u;
+    const uint32_t a_buf_bytes = PA * halo_plane, ring_off = 2u * a_buf_bytes;
+    // staging: p_out planes of n_slots output rows, as dgrad_phases_setup
+    const uint32_t slot_bytes = (uint32_t)p.out_W * 64u, stg_plane = (uint32_t)n_slots * slot_bytes;
+    const uint32_t stg_off = ring_off + (uint32_t)S * stage_bytes;
+    const int64_t n_work = (p.halo_positions + TILE_M - 1) / TILE_M;
+    const uint32_t raster_rows = (uint32_t)(p.halo_positions / p.halo_w);
+    auto halo_row_lo = [&](int64_t t) -> int {              // as conv_tc_kernel
+        const uint32_t num = (uint32_t)(t * TILE_M + p.halo_lo + 4 * p.halo_w);
+        return (int)xb_div(num, p.halo_div_w) - 4;
+    };
+    // output row of raster row R in row phase py (-1: none)
+    auto out_row = [&](uint32_t R, int py) -> int64_t {
+        return xb_pair_out_row(R, raster_rows, p.box_div_hp, p.box_hp, p.box_y0, p.sub_y1[2 * py], p.sub_oy0[2 * py], p.out_H);
+    };
+    auto run_of = [&](int64_t p0, uint32_t R, int py, int &lo, int &hi) -> int {
+        return xb_pair_run(p0, R, p.halo_w, p.halo_w0, p.sub_x1[2 * py], p.sub_x1[2 * py + 1], lo, hi);
+    };
+
+    if (tid == 0) {
+        for (int s = 0; s < S; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], CONS_WARPS);
+        }
+        for (int a = 0; a < 2; ++a) {
+            mbar_init(&a_full[a], 1);
+            mbar_init(&a_empty[a], CONS_WARPS);
+        }
+        mbar_init(&stg_full, CONS_WARPS);
+        mbar_init(&stg_empty, 1);
+        mbar_fence_init();
+    }
+    __syncthreads();
+    const uint32_t smem_base = smem_u32(smem);
+    if (smem_base & 1023u) __trap();                         // the 128-byte swizzle pattern repeats every 1024 B
+    uint32_t t_wait[5] = {0, 0, 0, 0, 0};                   // role timing, slots as in conv_tc_kernel
+    if (p.timing && blockIdx.x < 160 && (tid == 0 || tid == CONS_WARPS * 32)) xb_k12_timing[blockIdx.x][tid == 0 ? 0 : 4] = clock64();
+    auto timed_wait = [&](uint64_t *bar, uint32_t parity, int slot) {
+        if (p.timing) {
+            const uint32_t t0 = clock32();
+            mbar_wait(bar, parity);
+            t_wait[slot] += clock32() - t0;
+        } else {
+            mbar_wait(bar, parity);
+        }
+    };
+
+    if (warp >= CONS_WARPS) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PROD_REGS));
+        if (tid == CONS_WARPS * 32) {
+            // ---------------------------------------------------------------- producer: halo tiles and the weight ring
+            uint32_t it = 0, tile_it = 0;
+            for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x, ++tile_it) {
+                const uint32_t buf = tile_it & 1u;
+                timed_wait(&a_empty[buf], ((tile_it >> 1) & 1u) ^ 1u, 1);
+                mbar_expect_tx(&a_full[buf], (uint32_t)PA * (uint32_t)(p.halo_rows * p.halo_w) * 128u);
+                const int r_lo = halo_row_lo(w);
+#pragma unroll
+                for (int q = 0; q < PA; ++q)
+                    tma_load_box(smem_base + buf * a_buf_bytes + q * halo_plane, &p.tm_a, 0, p.halo_w0, r_lo, 1, q, &a_full[buf]);
+                for (int kc = 0; kc < N_SUB * n_chunks; ++kc, ++it) {
+                    const int stage = (int)(it % (uint32_t)S);
+                    timed_wait(&empty_bar[stage], ((it / (uint32_t)S) & 1u) ^ 1u, 0);
+                    mbar_expect_tx(&full_bar[stage], stage_bytes);
+                    tma_load_3d(smem_base + ring_off + (uint32_t)stage * stage_bytes, &p.tm_b, (kc % n_chunks) * KC,
+                                (kc / n_chunks) * N, 0, &full_bar[stage]);
+                }
+            }
+        } else if (tid == CONS_WARPS * 32 + 32) {
+            // ---------------------------------------------------------------- staging: output runs out
+            const uint32_t stg = smem_base + stg_off;
+            uint32_t k = 0;                                  // phase pairs so far
+            for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
+                const int64_t p0 = w * TILE_M;
+                const uint32_t R0 = xb_pair_row0(p0, p.halo_div_w);
+                for (int py = 0; py < 2; ++py, ++k) {
+                    mbar_wait(&stg_full, k & 1u);            // the consumers have written both phases of the pair
+                    for (int j = 0; j < n_slots; ++j) {
+                        int lo, hi;
+                        const int64_t orw = out_row(R0 + j, py);
+                        if (orw >= 0 && run_of(p0, R0 + j, py, lo, hi) > 0)
+                            for (int q = 0; q < p.p_out; ++q)
+                                bulk_store(p.out[q] + (orw * p.out_W + lo) * 32, stg + q * stg_plane + j * slot_bytes + lo * 64,
+                                           (uint32_t)(hi - lo + 1) * 64u);
+                    }
+                    bulk_commit();
+                    bulk_wait_read_all();
+                    mbar_arrive(&stg_empty);                 // the stores have read the staging tile: free for the next pair
+                }
+            }
+            bulk_wait_all();
+        }
+    } else {
+        // ------------------------------------------------------------------ consumers: wgmma issue + epilogue
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONS_REGS));
+        const int wg = warp >> 2;
+        const uint64_t b_tmpl = make_desc_sw128(0, 16, 1024);    // as conv_tc_kernel's forward with b_tma: K step of 16 = 32 B
+        const int mi = lane >> 3, lr = lane & 7, m_l = 16 * (warp & 3) + 8 * (mi & 1);
+        const uint32_t a_lane = (uint32_t)wg * 8192u + (uint32_t)(m_l + lr) * 128u;
+        const int rbase = 64 * wg + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+        float acc[PB * NC][16];
+        uint32_t it = 0, tile_it = 0, k = 0;
+        for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x, ++tile_it) {
+            const uint32_t buf = tile_it & 1u;
+            timed_wait(&a_full[buf], (tile_it >> 1) & 1u, 2);
+            const uint32_t halo_base = smem_base + buf * a_buf_bytes;
+            const int halo_s0 = (int)(w * TILE_M) - halo_row_lo(w) * p.halo_w;     // tile row of the site of MMA row 0
+            // this thread's two rows: raster pixel (x, y), their staging byte offset and their mask element at pixel 2x of
+            // output row 2 (y - y0) of the image
+            const int64_t p0 = w * TILE_M;
+            const uint32_t R0 = xb_pair_row0(p0, p.halo_div_w);
+            int rx[2], ry[2];
+            bool row_ok[2];
+            uint32_t srow[2];
+            int64_t mrow[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int64_t P = p0 + rbase + 8 * h;
+                const uint32_t R = xb_div((uint32_t)P, p.halo_div_w), b = xb_div(R, p.box_div_hp);
+                rx[h] = (int)((uint32_t)P - R * (uint32_t)p.halo_w) + p.halo_w0;
+                ry[h] = (int)(R - b * (uint32_t)p.box_hp);
+                row_ok[h] = P < p.halo_positions && rx[h] >= 0 && ry[h] >= p.box_y0;
+                srow[h] = (R - R0) * slot_bytes + (uint32_t)(rx[h] > 0 ? rx[h] : 0) * 128u;
+                mrow[h] = (((int64_t)b * p.out_H + 2 * (ry[h] - p.box_y0)) * p.mask_W + 2 * rx[h] + p.mask_x0) * 32;
+            }
+            for (int sub = 0; sub < N_SUB; ++sub) {
+                const int px = sub & 1;
+                bool live[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) live[h] = row_ok[h] && rx[h] <= p.sub_x1[sub] && ry[h] <= p.sub_y1[sub];
+                // the ReLU mask of this thread's 16 elements, loaded before the sub-item's MMAs (which hide the latency)
+                uint32_t mw[4][2];
+                {
+                    const int64_t m_off = ((int64_t)p.sub_oy0[sub] * p.mask_W + px) * 32 + cq;
+#pragma unroll
+                    for (int i = 0; i < 4; ++i)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            mw[i][h] = live[h] ? *reinterpret_cast<const uint32_t *>(p.mask + mrow[h] + m_off + 8 * i) : 0u;
+                }
+                uint32_t scale_d = 0;
+                uint32_t af[KC / 16][PA][4];
+                for (int kc = 0; kc < n_chunks; ++kc, ++it) {
+                    const int stage = (int)(it % (uint32_t)S);
+                    timed_wait(&full_bar[stage], (it / (uint32_t)S) & 1u, 0);
+                    const uint32_t w_addr = smem_base + ring_off + (uint32_t)stage * stage_bytes;
+                    const uint32_t a_row = a_lane + halo_base + (uint32_t)(halo_s0 + p.halo_shift[sub * n_chunks + kc]) * 128u;
+                    const uint32_t a_sw = (a_row >> 7) & 7u;
+                    const uint64_t b0 = b_tmpl + (uint64_t)(w_addr >> 4);
+#pragma unroll
+                    for (int ks = 0; ks < KC / 16; ++ks) {
+                        const uint32_t a_addr = a_row + (((uint32_t)(2 * ks + (mi >> 1))) ^ a_sw) * 16u;
+#pragma unroll
+                        for (int q = 0; q < PA; ++q) ldmatrix_x4<0>(af[ks][q], a_addr + (uint32_t)q * halo_plane);
+                    }
+                    wgmma_fence();
+#pragma unroll
+                    for (int ks = 0; ks < KC / 16; ++ks) {
+                        const uint64_t db = b0 + (uint64_t)(ks * (32 >> 4));
+                        mma_plane<0, PB, NC, 0>(acc, af[ks][0], db, scale_d);
+                        mma_plane<0, PB, NC, 1>(acc, af[ks][1], db, 1u);
+                        mma_plane<0, PB, NC, 2>(acc, af[ks][2], db, 1u);
+                        scale_d = 1;
+                    }
+                    wgmma_commit();
+                    timed_wgmma_wait<0>(p.timing, t_wait[3]);
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_bar[stage]);
+                }
+                const uint32_t t_epi = p.timing ? clock32() : 0u;
+                // ---- epilogue: rows rbase (h = 0) and rbase + 8 (h = 1) into the staging tile
+                if (px == 0) mbar_wait(&stg_empty, (k & 1u) ^ 1u);     // the previous pair's stores have read the tile
+                uint8_t *dst[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) dst[h] = smem + stg_off + srow[h] + px * 64;
+                // the mask as one bit per element (bf16 > 0 <=> sign bit clear and not (+)zero), as conv_tc_kernel keeps it
+                uint32_t keep = 0u;
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const uint32_t lo16 = mw[i][h] & 0xffffu, hi16 = mw[i][h] >> 16;
+                        keep |= (uint32_t)(lo16 != 0u && lo16 < 0x8000u) << (4 * (2 * i + h));
+                        keep |= (uint32_t)(hi16 != 0u && hi16 < 0x8000u) << (4 * (2 * i + h) + 1);
+                    }
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int c = 8 * i + cq;                                  // columns c, c + 1
+                    float cs[2] = {0.f, 0.f};
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        float v[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            v[e] = acc[PB - 1][4 * i + 2 * h + e];             // smallest group first
+#pragma unroll
+                            for (int gq = PB - 2; gq >= 0; --gq) v[e] += acc[gq][4 * i + 2 * h + e];
+                            v[e] += 0.f;                                       // conv_tc_kernel's zero bias: -0 -> +0
+                            if (!((keep >> (4 * (2 * i + h) + e)) & 1u)) v[e] = 0.f;
+                        }
+                        if (live[h]) {
+                            __nv_bfloat16 q0[3], q1[3];
+                            split3_bf16(v[0], q0[0], q0[1], q0[2]);
+                            split3_bf16(v[1], q1[0], q1[1], q1[2]);
+#pragma unroll
+                            for (int q = 0; q < 3; ++q)
+                                if (q < p.p_out) *reinterpret_cast<uint32_t *>(dst[h] + q * stg_plane + c * 2) = pack2(q0[q], q1[q]);
+                            cs[0] += v[0], cs[1] += v[1];
+                        }
+                    }
+#pragma unroll
+                    for (int off = 4; off <= 16; off <<= 1) {
+                        cs[0] += __shfl_xor_sync(0xffffffffu, cs[0], off);
+                        cs[1] += __shfl_xor_sync(0xffffffffu, cs[1], off);
+                    }
+                    if (lane < 4) s_colsum[buf][sub][warp][c] = cs[0], s_colsum[buf][sub][warp][c + 1] = cs[1];
+                }
+                if (px == 1) {
+                    // both phases of the pair are staged: hand the tile to the stores
+                    fence_proxy_async();   // written by the generic proxy, read by the bulk copies (async proxy)
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&stg_full);
+                    ++k;
+                }
+                if (p.timing) t_wait[4] += clock32() - t_epi;
+            }
+            // every MMA of this tile has retired (wait above): the halo tile is free
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&a_empty[buf]);
+            const uint32_t t_epi = p.timing ? clock32() : 0u;
+            // the tile's column-sum rows, warps added in a fixed order (deterministic) as conv_tc_kernel does
+            asm volatile("bar.sync 1, %0;" ::"n"(CONS_WARPS * 32) : "memory");
+            for (int i = tid; i < N_SUB * N; i += CONS_WARPS * 32) {
+                const int sub = i / N, c = i - sub * N;
+                float s = s_colsum[buf][sub][0][c];
+#pragma unroll
+                for (int q = 1; q < CONS_WARPS; ++q) s += s_colsum[buf][sub][q][c];
+                p.colsum[(w * N_SUB + sub) * (int64_t)N + c] = s;
+            }
+            if (p.timing) t_wait[4] += clock32() - t_epi;
+        }
+    }
+    if (p.timing && blockIdx.x < 160) {
+        const unsigned long long now = clock64();
+        unsigned long long *o = xb_k12_timing[blockIdx.x];
+        if (tid == 0) o[0] = now - o[0], o[1] = t_wait[0], o[2] = t_wait[3], o[3] = t_wait[2], o[7] = t_wait[4];
+        if (tid == CONS_WARPS * 32) o[4] = now - o[4], o[5] = t_wait[0], o[6] = t_wait[1];
+    }
+}
+
 // weight-gradient finish: sum the split partials [splits, K, N] in a fixed order and scatter to torch's [N, C, KH, KW]
 // (column k = (kh, kw, c) of the packed layout -> xb_pack_weight_src); accumulate != 0 adds to dw (autograd .grad).
 // A block owns E = 256 / lanes consecutive (k, n) elements - coalesced rows of the partial matrices - and `lanes` threads
@@ -1589,6 +1866,39 @@ bool wgrad_pairs_setup(ConvParams &p, int planes_a, int planes_b, int N, int n_t
     return true;
 }
 
+// XB_K12_DGRAD_PHASES=0 keeps every halo launch on conv_tc_kernel (the reference conv_tc_kernel_dgrad_phases must equal)
+bool dgrad_phases_enabled() {
+    static int on = -1;
+    if (on < 0) {
+        const char *e = getenv("XB_K12_DGRAD_PHASES");
+        on = (e && e[0] == '0') ? 0 : 1;
+    }
+    return on == 1;
+}
+
+// conv_tc_kernel_dgrad_phases takes a halo launch with three planes on each side and four stride phases of N = 32 columns
+// that write the same output columns (same_cols) at oys = oxs = 2, in the order (py, px) = (0, 0), (0, 1), (1, 0), (1, 1),
+// where the two phases of a py share their output rows and together write one run of consecutive pixels per raster row
+// (conv_index.h, xb_pair_*); its outputs are bf16 planes only whose pixels are 64-byte rows (out_ld = 32, out_c0 = 0), with
+// a ReLU mask of the same pixel rows and column sums, and without bias or ReLU - conv2's data gradient of BoxNatureCNN.
+// Fills the ring and the shared-memory size of p (halo tiles a_bytes, weight stages, staging tile).
+bool dgrad_phases_setup(ConvParams &p, int planes_a, int planes_b, int n_sub, int N, int same_cols, uint32_t a_bytes) {
+    if (planes_a != 3 || planes_b != 3 || n_sub != 4 || N != 32 || !same_cols || p.oys != 2 || p.oxs != 2) return false;
+    if (p.p_out == 0 || p.out_f32 || p.bias || p.relu || !p.mask || !p.colsum || p.out_ld != 32 || p.out_c0 != 0) return false;
+    for (int py = 0; py < 2; ++py) {
+        const int e = 2 * py, o = e + 1;
+        if (p.sub_oy0[e] != p.sub_oy0[o] || p.sub_y1[e] != p.sub_y1[o] || p.sub_ox0[e] != 0 || p.sub_ox0[o] != 1) return false;
+        if (p.sub_x1[o] != p.sub_x1[e] && p.sub_x1[o] != p.sub_x1[e] - 1) return false;
+    }
+    const uint32_t stg = (uint32_t)p.p_out * (uint32_t)xb_pair_slots(p.halo_w) * (uint32_t)p.out_W * 64u;
+    const uint32_t stage_bytes = 3u * xb_conv_w_plane_bytes(32);
+    if (a_bytes + stg + 2u * stage_bytes > (uint32_t)XB_K12_MAX_DYN_SMEM) return false;
+    const int stages = (int)(((uint32_t)XB_K12_MAX_DYN_SMEM - a_bytes - stg) / stage_bytes);
+    p.stages = stages > MAX_STAGES ? MAX_STAGES : stages;
+    p.dyn_smem = a_bytes + (uint32_t)p.stages * stage_bytes + stg;
+    return true;
+}
+
 }  // namespace
 
 extern "C" int xb_split_bf16(const float *x, int64_t n, int planes, void *out, void *stream) {
@@ -1831,6 +2141,17 @@ extern "C" int xb_gemm_halo_tc(int planes_a, int planes_b, const void *in, int64
     p.out_ld = out_ld, p.out_c0 = out_c0;
     p.splits = 1, p.sites_per_split = 0, p.w_ld = 0;
     const int64_t tiles = (p.halo_positions + TILE_M - 1) / TILE_M;
+    if (dgrad_phases_enabled() && dgrad_phases_setup(p, planes_a, planes_b, n_sub, N, same_cols, a_bytes)) {
+        // the stride phases by pairs: masks in and output rows out by bulk copies (conv_tc_kernel_dgrad_phases)
+        static bool attr = false;
+        if (!attr) {
+            cudaFuncSetAttribute(conv_tc_kernel_dgrad_phases, cudaFuncAttributeMaxDynamicSharedMemorySize, XB_K12_MAX_DYN_SMEM);
+            attr = true;
+        }
+        const int grid = (int)(tiles < xb_sm_count() ? tiles : xb_sm_count());
+        conv_tc_kernel_dgrad_phases<<<grid, THREADS, p.dyn_smem, (cudaStream_t)stream>>>(p);
+        return xb_launch_status();
+    }
     return launch<false>(planes_a, planes_b, p, tiles, stream);
 }
 
